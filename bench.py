@@ -237,11 +237,26 @@ class ClockSampler(object):
                 "reasons": sorted(reasons), "samples": len(sm)}
 
 
+def dump_outputs(out_dir, arrays, seed=1234, max_bytes=32 << 20):
+    """Writes a fixed, seeded row sample of each factor matrix the timed path updated as out_dir/<name>.npy (float32),
+    so that two builds can be compared output for output.  The arrays share max_bytes of row data equally (32768 rows
+    of P and of Q at d = 128, 16384 at d = 256)."""
+    os.makedirs(out_dir, exist_ok=True)
+    for i, (name, t) in enumerate(arrays):
+        rows = t.shape[0]
+        max_rows = max(1, max_bytes // len(arrays) // (4 * max(1, t[0].numel())))
+        if rows > max_rows:
+            idx = np.sort(np.random.default_rng(seed + i).choice(rows, size=max_rows, replace=False))
+            import torch
+            t = t.index_select(0, torch.from_numpy(idx).to(t.device))
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach().float().cpu().numpy().reshape(t.shape[0], -1))
+
+
 def measured_peak():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.isfile(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3; not measured)"
 
 
 # ------------------------------------------------------------------------------------------------
@@ -362,7 +377,9 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--cpu-seconds", type=float, default=12.0)
-    ap.add_argument("--kernel-mode", type=int, default=0, help="0 auto (d=128: tcgen05 kernel + SIMT class 0), 1 generic kernels, 2 tuned SIMT kernels only")
+    ap.add_argument("--kernel-mode", type=int, default=0, help="0 auto (d=128: rows up to the tensor-core threshold on the tuned SIMT kernels, longer rows on the tensor-core kernel), 1 generic kernels, 2 tuned SIMT kernels only")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write a seeded row sample of the factors they computed as DIR/<name>.npy")
     ap.add_argument("--tc-min-class", type=int, default=None, help="first row-length class solved by the tensor-core kernel (default: library's)")
     ap.add_argument("--exchange", default=os.environ.get("BFL_EXCHANGE", "p2p"), choices=["p2p", "allgather"],
                     help="multi-GPU: fused peer stores from the solve kernel (default) or an NCCL all-gather per half-epoch")
@@ -461,6 +478,8 @@ def main():
     barrier()
     launches = _cabi.lib().bfl_kernel_launch_count() - launches0
     ms = t0e.elapsed_time(t1e)
+    if args.dump_outputs and rank == 0:   # before the e2e leg overwrites the factors
+        dump_outputs(args.dump_outputs, [("P", P), ("Q", Q)])
     clocks = sampler.stop() if rank == 0 else None
     if world > 1:
         t = torch.tensor([ms], device=device, dtype=torch.float64)
@@ -479,12 +498,7 @@ def main():
     alg_bytes = [algorithmic_bytes(my_nnz[a], my_rows[a], d) for a in (0, 1)]
     t_solve = sum(np.mean(per_axis_ms[a]) for a in (0, 1)) / 1e3
     achieved = sum(alg_bytes) / t_solve / 1e9
-    # DRAM traffic of the same launches from the committed ncu capture (profiles/run_ncu.sh); single-GPU C2 only
-    traffic, traffic_src = None, None
-    tpath = os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "traffic_c2.json")
-    if world == 1 and args.workload == "c2" and os.path.isfile(tpath):
-        tj = json.load(open(tpath))
-        traffic, traffic_src = tj["user_pass"] + tj["item_pass"], tj["source"]
+    traffic, traffic_src = None, "not measured"   # DRAM traffic needs a hardware-counter profiler
     roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                 "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src, "kernel": "ALS row-solve (user + item launches of one iteration)",
                 "algorithmic_bytes_per_launch": {"user_pass": alg_bytes[0], "item_pass": alg_bytes[1]},

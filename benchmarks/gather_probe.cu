@@ -5,8 +5,8 @@
 //           completion by cp.async.mbarrier.arrive.noinc
 //   mode 2: plain 128-bit loads into registers + st.shared (the synchronous baseline)
 // P producer warps share the ring (stage s belongs to warp s % P); one consumer warp releases a stage as soon as it is
-// full.  Persistent grid of 148 CTAs.  Prints GB/s per configuration.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o gather_probe gather_probe.cu
+// full.  Persistent grid of one CTA per SM.  Prints GB/s per configuration.
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o gather_probe gather_probe.cu
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -104,7 +104,10 @@ __global__ void __launch_bounds__(32 * (MAXP + 1), 1) probe(const float* __restr
 
 int main(int argc, char** argv) {
     const size_t rows = argc > 1 ? (size_t)atoll(argv[1]) : 10000000;
-    const int tiles = 2000, grid = 148;
+    int grid = 0, clk_khz = 0;
+    CK(cudaDeviceGetAttribute(&grid, cudaDevAttrMultiProcessorCount, 0));
+    CK(cudaDeviceGetAttribute(&clk_khz, cudaDevAttrClockRate, 0));
+    const int tiles = 2000;
     float* Y;
     CK(cudaMalloc(&Y, rows * ROWF * 4));
     CK(cudaMemset(Y, 0, rows * ROWF * 4));
@@ -137,9 +140,9 @@ int main(int argc, char** argv) {
                 CK(cudaDeviceSynchronize());
                 float ms;
                 cudaEventElapsedTime(&ms, e0, e1);
-                printf("mode %d (%s) stages %2d producers %d: %8.1f GB/s  (%.0f clk per 32-row tile per SM at 1.965 GHz)\n", mode,
+                printf("mode %d (%s) stages %2d producers %d: %8.1f GB/s  (%.0f clk per 32-row tile per SM at %.3f GHz)\n", mode,
                        mode == 0 ? "bulk 512B" : (mode == 1 ? "LDGSTS 16B/lane" : "LDG+STS"), NS, P, bytes / ms / 1e6,
-                       ms * 1e-3 * 1.965e9 / tiles);
+                       ms * 1e-3 * clk_khz * 1e3 / tiles, clk_khz * 1e-6);
             }
     return 0;
 }

@@ -143,7 +143,9 @@ def main(args):
         t = torch.tensor([ms], device=dev, dtype=torch.float64)
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         ms = float(t.item())
-    drv.finalize()
+    drv.finalize()   # multi-GPU plain SGD: every user range of P comes back from its owner here
+    if getattr(args, "dump_outputs", None) and rank == 0:
+        bench.dump_outputs(args.dump_outputs, [("P", P), ("Q", Q)] + ([("Qb", Qb)] if algo == "bpr" else []))
     mean_trials = None
     if trials is not None:
         tt = trials.to(torch.float32)
@@ -154,8 +156,7 @@ def main(args):
     peak, peak_src = bench.measured_peak()
     alg = algorithmic_bytes(algo, d, nnz, U, I, optimizer, mean_trials if mean_trials is not None else 2.0)
     achieved = alg * steps / (ms / 1e3) / 1e9 / world      # per GPU (every rank streams its own share)
-    tfile = os.path.join(ROOT, "profiles", "traffic_%s.json" % args.workload)
-    traffic = json.load(open(tfile)) if (world == 1 and os.path.isfile(tfile)) else None
+    traffic = None   # DRAM traffic is not measured (needs a hardware-counter profiler)
     out = {"metric": "positives/sec (nnz/s) %s d=%d" % ("BPRMF" if algo == "bpr" else "WARP", d), "value": value,
            "unit": "nnz/s", "n_gpus": world, "steps": steps, "warmup": warmup, "ms_per_step": ms / steps,
            "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "f32", "data": "synthetic",

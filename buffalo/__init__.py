@@ -1,5 +1,5 @@
 """`buffalo` -- import alias of buffalo_b200, so that code written for kakao/buffalo
-(examples/example_als.py, benchmark/test_performance.py) runs unchanged on the B200 backend.
+(examples/example_als.py, benchmark/test_performance.py) runs unchanged on the H100 backend.
 Every submodule path of the reference that the hot path's callers use is mapped onto buffalo_b200."""
 import importlib
 import sys

@@ -1,7 +1,7 @@
-"""buffalo_b200 -- B200-native implementation of kakao/buffalo's matrix-factorisation training hot path
+"""buffalo_b200 -- H100-native implementation of kakao/buffalo's matrix-factorisation training hot path
 (ALS row solves, BPRMF / WARP negative-sampling SGD) behind buffalo's own Python API.
 
-The compute lives in buffalo_b200/csrc (hand-written sm_100a CUDA behind the C ABI of
+The compute lives in buffalo_b200/csrc (hand-written sm_90a CUDA behind the C ABI of
 include/buffalo_b200.h).  There is no CPU fallback.  `import buffalo` resolves to this package
 (see the `buffalo/` alias at the repository root), so scripts written for the reference run unchanged.
 """
@@ -22,7 +22,7 @@ from buffalo_b200.parallel.base import ParALS, ParBPRMF, ParCFR, ParW2V
 def _out_of_scope(name):
     class _Algo(object):
         def __init__(self, *a, **k):
-            raise NotImplementedError(name + " is outside the B200 hot-path scope (ALS, BPRMF, WARP only)")
+            raise NotImplementedError(name + " is outside the H100 hot-path scope (ALS, BPRMF, WARP only)")
     _Algo.__name__ = name
     return _Algo
 

@@ -1,8 +1,8 @@
 """ctypes binding of the C ABI declared in include/buffalo_b200.h.
 
 The shared library is built in-tree (buffalo_b200/libbuffalo_b200.so) by
-``buffalo_b200/csrc/build.sh`` (nvcc, sm_100a only).  There is no CPU fallback: if the
-library is missing, loading raises; if no Blackwell GPU is present, ``init`` fails with the
+``buffalo_b200/csrc/build.sh`` (nvcc, sm_90a only).  There is no CPU fallback: if the
+library is missing, loading raises; if no Hopper (sm_90) GPU is present, ``init`` fails with the
 library's error string.
 """
 import ctypes as C
@@ -89,7 +89,7 @@ PROTOTYPES = {
 
 
 def build(force=False, verbose=False):
-    """Compile every CUDA source for sm_100a into buffalo_b200/libbuffalo_b200.so."""
+    """Compile every CUDA source for sm_90a into buffalo_b200/libbuffalo_b200.so."""
     srcs = [os.path.join(_SRC_DIR, f) for f in os.listdir(_SRC_DIR) if f.endswith((".cu", ".cuh", ".sh"))]
     srcs.append(os.path.join(_HERE, "..", "include", "buffalo_b200.h"))
     newest = max(os.path.getmtime(s) for s in srcs if os.path.exists(s))
@@ -110,7 +110,7 @@ def lib():
         if not os.path.isfile(LIB_PATH):
             raise RuntimeError(
                 "buffalo_b200/libbuffalo_b200.so is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a). There is no CPU fallback.")
+                "(nvcc, sm_90a). There is no CPU fallback.")
         handle = C.CDLL(LIB_PATH)
         for name, (res, args) in PROTOTYPES.items():
             fn = getattr(handle, name)  # AttributeError if the header and the library disagree

@@ -1,11 +1,11 @@
-"""ALS trainer: the reference's Python epoch driver (buffalo/algo/als.py) on top of the B200 backend.
+"""ALS trainer: the reference's Python epoch driver (buffalo/algo/als.py) on top of the H100 backend.
 
 Two feeding modes, same results:
   * resident (default when the CSR fits in device memory): both CSR orientations and the factor matrices live
     on the GPU for the whole of train(); one launch set per half-epoch, no host traffic inside the loop;
   * chunked: the reference's own protocol -- BufferedDataMatrix chunks pushed through
     obj.partial_update(start_x, next_x, indptr, keys, vals, axis) (als.py:115-142).
-The backend is GPU-only; `accelerator` is accepted and ignored (both values run the sm_100a kernels).
+The backend is GPU-only; `accelerator` is accepted and ignored (both values run the sm_90a kernels).
 """
 import json
 import time

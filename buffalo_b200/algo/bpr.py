@@ -1,4 +1,4 @@
-"""BPRMF trainer (buffalo/algo/bpr.py) on the B200 backend."""
+"""BPRMF trainer (buffalo/algo/bpr.py) on the H100 backend."""
 import json
 
 import numpy as np

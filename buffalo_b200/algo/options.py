@@ -2,7 +2,7 @@
 
 The defaults are table-driven here; every value and key matches the cited lines so that option files
 written for the reference load unchanged.  ``accelerator`` is accepted for compatibility: this package has
-a single, GPU-only backend, so both values select the sm_100a kernels.
+a single, GPU-only backend, so both values select the sm_90a kernels.
 """
 from buffalo_b200.misc import aux
 
@@ -67,7 +67,7 @@ class WARPOption(AlgoOption):
 def _out_of_scope(name):
     class _Opt(AlgoOption):
         def get_default_option(self):
-            raise NotImplementedError(name + " is outside the B200 hot-path scope (ALS, BPRMF, WARP only)")
+            raise NotImplementedError(name + " is outside the H100 hot-path scope (ALS, BPRMF, WARP only)")
     _Opt.__name__ = name
     return _Opt
 

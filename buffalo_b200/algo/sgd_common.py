@@ -1,5 +1,5 @@
 """Shared driver for the two negative-sampling trainers (BPRMF, WARP): the epoch loop of
-buffalo/algo/bpr.py:170-252 / warp.py:187-267 on the B200 backend."""
+buffalo/algo/bpr.py:170-252 / warp.py:187-267 on the H100 backend."""
 import time
 
 import numpy as np

@@ -1,4 +1,4 @@
-"""WARP trainer (buffalo/algo/warp.py) on the B200 backend.  The reference has no GPU WARP
+"""WARP trainer (buffalo/algo/warp.py) on the H100 backend.  The reference has no GPU WARP
 (warp.py:30-32 raises NotImplementedError for accelerator=True); here the GPU path is the only path."""
 import numpy as np
 

@@ -78,6 +78,8 @@ int als_apply_options(bfl_als* h, const JsonOpt& j) {
     h->eps = (float)j.number("eps", 1e-10);
     h->cg_tolerance = (float)j.number("cg_tolerance", 1e-10);
     h->kernel_mode = j.integer("_b200_kernel_mode", 0);
+    // rows of classes >= 2 (> 64 nnz) on the tensor-core kernel: the fastest of the routings measured at C2 on an H100
+    // (DESIGN.md 4.1)
     h->tc_min_class = std::max(0, std::min(7, j.integer("_b200_tc_min_class", 2)));
     std::string optimizer = j.string("optimizer", "manual_cg");
     if (h->d >= 128) optimizer = "ialspp";  // als.cc:46
@@ -87,7 +89,7 @@ int als_apply_options(bfl_als* h, const JsonOpt& j) {
     else if (optimizer == "ialspp") h->optimizer_code = 8;
     else
         BFL_FAIL(BFL_ERR_OPTION, "optimizer '" + optimizer +
-                                     "' is not available on the B200 backend (supported: llt, ldlt, manual_cg, ialspp)");
+                                     "' is not available on the H100 backend (supported: llt, ldlt, manual_cg, ialspp)");
     if (BFL_OK != require_device()) return BFL_ERR_CUDA;
     int dev = 0;
     BFL_CUDA(cudaGetDevice(&dev));

@@ -568,14 +568,9 @@ __global__ void __launch_bounds__(DIRECT_THREADS) als_direct_cta_kernel(AlsArgs 
 // slab over its share of the rows in registers (8x8 per thread), writes a partial, and a second
 // kernel sums the partials in fp64.
 // ---------------------------------------------------------------------------------------
-// packed fp32 FMA (Blackwell FFMA2): d = a * b + c on both halves
+// d = a * b + c on both halves of an fp32 pair
 __device__ __forceinline__ float2 gram_ffma2(float2 a, float2 b, float2 c) {
-    unsigned long long ra = *reinterpret_cast<unsigned long long*>(&a);
-    unsigned long long rb = *reinterpret_cast<unsigned long long*>(&b);
-    unsigned long long rc = *reinterpret_cast<unsigned long long*>(&c);
-    unsigned long long rd;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(rd) : "l"(ra), "l"(rb), "l"(rc));
-    return *reinterpret_cast<float2*>(&rd);
+    return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
 }
 
 constexpr int GRAM_TR = 32;       // rows per smem tile

@@ -1,4 +1,4 @@
-// Tensor-core iALS++ row solve for sm_100a (d = 128, block_size 32): the Blackwell-native path of
+// Tensor-core iALS++ row solve for sm_90a (d = 128, block_size 32): the Hopper-native path of
 // lib/algo_impl/als/als.cc:211-358.
 //
 // Algebra.  With M = G + reg*I + sum_c w_c q_c q_c^T (w = alpha*v) and b = sum_c w_c q_c, the reference's block
@@ -8,40 +8,37 @@
 // fixed 3-step CG on 32 x 32 diagonal blocks -- O(d^2) work per row that does not depend on the row length, and the
 // per-nnz work collapses into one rank-1 update  M += (sqrt(w) q)(sqrt(w) q)^T, a dense contraction: tensor cores.
 //
-// Precision.  The contraction runs on tcgen05.mma kind::f16 with a two-term fp16 split of the scaled operand
-// t = 2^e sqrt|w| q = head + tail (head: 11 significant bits, tail: the next 11): head.head + head.tail + tail.head
-// leaves a relative error of ~2^-21 per product, fp32-grade like the reference's arithmetic, at twice the tensor rate and
-// half the shared-memory traffic per entry of the equivalent 3xTF32 scheme (K = 16 per instruction instead of 8).  The
-// power of two 2^e (tc_scale_kernel: from max|Y| and max|w| of the launch) places the largest operand just below 2^15, so
-// nothing overflows fp16 and entries down to 2^-20 of the largest keep a normal tail; the accumulator is multiplied by
-// 2^-2e (exact) when it is read.  b and the loss pieces are accumulated in plain fp32 from the unscaled rows.
+// Precision.  The contraction runs on wgmma (fp16 operands, fp32 accumulator) with a two-term fp16 split of the scaled
+// operand t = 2^e sqrt|w| q = head + tail (head: 11 significant bits, tail: the next 11): head.head + head.tail +
+// tail.head leaves a relative error of ~2^-21 per product, fp32-grade like the reference's arithmetic, at twice the
+// tensor rate and half the shared-memory traffic per entry of the equivalent 3xTF32 scheme (K = 16 per instruction
+// instead of 8).  The power of two 2^e (tc_scale_kernel: from max|Y| and max|w| of the launch) places the largest
+// operand just below 2^15, so nothing overflows fp16 and entries down to 2^-20 of the largest keep a normal tail; the
+// accumulator starts a row at 2^2e (G + reg I) and is multiplied by 2^-2e (exact) when it is read.  b and the loss
+// pieces are accumulated in plain fp32 from the unscaled rows.
 //
-// Pipeline of one persistent CTA (one per SM, 14 warps x 128 registers, warp-specialised, mbarrier hand-offs only, one
-// elected arrival per warp; hand-offs are per GROUP of two consecutive tiles of the CTA's tile stream):
+// Pipeline of one persistent CTA (one per SM, 13 warps, warp-specialised, mbarrier hand-offs only, one elected arrival
+// per warp; hand-offs are per GROUP of two consecutive tiles of the CTA's tile stream):
 //   planner warp     : walks the CTA's rows; every level of the dependent load chain (row id -> offsets -> keys / values)
 //                     is issued whole rows ahead of its use; per tile of 32 entries it writes the gather plan (keys,
 //                     2^e sqrt|w|, w, count / flags) into a 16-slot ring -- it runs up to 8 groups ahead;
-//   8 convert warps  : (a) gathers: two hand-offs ahead of its use, warp cw copies the rows cw, cw + 8, ... of a planned
-//                     tile with one coalesced 16-byte-per-lane cp.async per 512 bytes (SASS LDGSTS) into a ring of raw fp32
-//                     tiles (commit / wait groups + one mbarrier arrival per warp).  The first version gathered with
-//                     512-byte cp.async.bulk copies (TMA): a divergent-address bulk copy compiles to an ELECT / R2UR / UBLKCP
-//                     loop over the lanes, ~63-100 cycles per copy and warp -- one warp sustains 2.3 TB/s chip-wide, four
-//                     or more the 7.0 TB/s HBM read ceiling (benchmarks/gather_probe.cu) -- so it needed six warps that
-//                     did nothing else; spread over the convert warps the cp.async issue is a few instructions per tile;
-//                     (b) convert: thread = (feature m, entry half): reads column m of the raw tile (conflict-free),
-//                     scales, splits, and writes 16-byte groups of 8 consecutive k into the K-major un-swizzled operand
-//                     slabs (8 x 16 B core matrices, conflict-free); accumulates b_m = sum w q_m (exact fp32) and the loss
-//                     pieces in registers; groups of two full tiles take a branch-free straight-line path;
-//   MMA warp         : executes the generic -> async proxy fence for the group it has acquired, then one lane issues
-//                     tcgen05.mma kind::f16 (M = N = 128, K = 16; SASS UTCHMMA), accumulating the row's matrix in tensor
-//                     memory; entries with negative weight travel in their own tiles and are subtracted with the
-//                     instruction descriptor's negate-A bit;
-//   4 epilogue warps : a systolic pipeline over rows.  Thread j owns matrix row j (tensor-memory lane j), warp q column
-//                     block q: tcgen05.ld (SASS LDTM) the accumulator and the resident G + reg*I (tensor memory columns
-//                     0..127), h = M x - b; then warp q folds the deltas of blocks 0..q-1 into its h as they are published,
-//                     runs the 3-step CG of its own 32 x 32 block and publishes its delta.  Nothing in a row's sweep is
-//                     a group-wide barrier, so warp 0 is already on the next row's block 0 while warp 3 finishes this
-//                     one: up to two of the three accumulators are being drained while the third is being filled.
+//   4 convert warps  : (a) gathers: one hand-off ahead of its use, warp cw copies the rows cw, cw + 4, ... of a planned
+//                     tile with one coalesced 16-byte-per-lane cp.async per 512 bytes (SASS LDGSTS) into a ring of raw
+//                     fp32 tiles (commit / wait groups + one mbarrier arrival per warp);
+//                     (b) convert: thread = feature m: reads column m of the raw tile (conflict-free), scales, splits,
+//                     and writes 16-byte groups of 8 consecutive k into the K-major un-swizzled operand slabs (8 x 16 B
+//                     core matrices, conflict-free); accumulates b_m = sum w q_m (exact fp32) and the loss pieces in
+//                     registers; groups of two full tiles take a branch-free straight-line path;
+//   MMA warpgroup    : executes the generic -> async proxy fence for the group it has acquired, then issues wgmma
+//                     m64n128k16 (SASS HGMMA) for the two 64-row halves of the row's matrix, accumulating in registers
+//                     (128 fp32 per thread); entries with negative weight travel in their own tiles and are subtracted
+//                     with the negate-A immediate.  At a row's end it waits for the MMAs, stores 2^-2e x accumulator
+//                     into the shared-memory matrix of the epilogue and reloads 2^2e (G + reg I) for the next row;
+//   4 epilogue warps : a systolic pipeline over the row's blocks.  Thread j owns matrix row j, warp q column block q:
+//                     h = M x - b from the shared matrix; then warp q folds the deltas of blocks 0..q-1 into its h as
+//                     they are published, runs the 3-step CG of its own 32 x 32 block and publishes its delta.  Nothing in
+//                     a row's sweep is a group-wide barrier, so warp 0 is already waiting for the next row while warp 3
+//                     finishes this one; the MMA warpgroup fills the next row's accumulator meanwhile.
 // Rows of any length stream through (no per-nnz state), which removes the long-row cliff of the SIMT classes; rows
 // longer than the split threshold are cut into chunks whose partial matrices are summed in global memory and solved
 // by als_explicit_solve_kernel (als_explicit.cuh).
@@ -50,40 +47,45 @@
 #include "bfl_common.cuh"
 #include <type_traits>
 
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 namespace bfl {
 namespace tc {
 
-using namespace sm100;
+using namespace sm90;
 
-// 14 warps: epilogue 0..3 (warp q owns tensor-memory lane quarter q), planner 4, MMA issue 5, convert 6..13 (two sets of four:
-// each set takes half of a tile's entries)
-constexpr int N_CONV = 8, KH = N_CONV / 4;
-constexpr int W_EPI = 0, W_PLAN = 4, W_MMA = 5, W_CONV = 6;
-constexpr int WARPS = W_CONV + N_CONV, THREADS = WARPS * 32;
+// 16 warps = 4 warpgroups: epilogue 0..3 (warp q owns matrix rows 32q..32q+31), MMA 4..7, convert 8..11, planner 12
+// (warps 13..15 only hand their registers back).  Launched at 128 registers per thread; setmaxnreg then moves registers
+// from the planner's warpgroup to the MMA warpgroup, whose 128 x 128 fp32 accumulator needs 128 of them by itself.  Every
+// SM sub-partition runs one warp of each warpgroup, so the four budgets must sum to 4 x 128.
+constexpr int N_CONV = 4, KH = N_CONV / 4;
+constexpr int W_EPI = 0, W_MMA = 4, W_CONV = 8, W_PLAN = W_CONV + N_CONV;
+constexpr int WARPS = 16, THREADS = WARPS * 32;
+constexpr int REG_MMA = 200, REG_PLAN = 4 * 128 - 128 - 128 - REG_MMA;   // 56: the planner keeps a few row pointers
 constexpr int NXS = 8;     // x buffers of the epilogue pipeline (a fast warp publishes row r + 1 while a slow one reads row r - 3)
 // Hand-offs are per GROUP of PT consecutive tiles of the CTA's tile stream (a group may span rows: every tile carries its own
-// flags): with all the math switched off the barrier round trips of a one-tile hand-off still cost ~700 cycles per tile.
+// flags): the barrier round trips of a one-tile hand-off cost as much as the math of a tile.
 constexpr int PT = 2;      // tiles per hand-off group
-constexpr int NR = 3;      // raw stages (groups)
+constexpr int NR = 2;      // raw stages (groups); the shared-memory matrix of the epilogue leaves no room for a third
 constexpr int NO = 2;      // operand stages (groups)
-constexpr int GATHER_AHEAD = 2;   // groups between a convert warp's gather issue and its use of the group (< NR)
+constexpr int GATHER_AHEAD = 1;   // groups between a convert warp's gather issue and its use of the group (< NR)
 constexpr int NPG = 8, NP = NPG * PT;   // gather-plan ring (small slots): the planner runs up to NPG groups ahead
 constexpr int NBV = 8;     // ring of per-row vectors handed from the convert warps to the epilogue
-// d = 128: 32 gathered rows per stage, three 128-column accumulators (fused solve) behind the resident G + reg I;
-// d = 256 (split-row mode only): 16 rows per stage, one accumulator set of 384 columns: rows 0..127 x all 256 columns
-// and rows 128..255 x columns 128..255 (the remaining quadrant is the transpose of the first one's right half)
+// d = 128: 32 gathered rows per stage; d = 256 (split-row mode only): 16 rows per stage, and the chunk matrix is
+// accumulated in three launches (passes) of 128 x 128 blocks: rows / columns 0..127, rows 0..127 x columns 128..255
+// (its transpose is the remaining quadrant), rows / columns 128..255
 template <int D>
 struct Cfg {
     static constexpr int TILE = D == 128 ? 32 : 16;      // gathered rows per stage
-    static constexpr int NACC = D == 128 ? 3 : 1;        // accumulator sets in tensor memory
     static constexpr int NF = D / 128;                    // features per convert thread
     static constexpr int LBO = D * 16;                    // bytes between the 8-k chunks of an operand slab
     static constexpr int OP_BYTES = TILE * D * 2;         // head (or tail) slab of one stage
 };
-constexpr int NACC_MAX = 3;
 constexpr uint32_t F_FIRST = 1u << 8, F_LAST = 1u << 9, F_NEG = 1u << 10, F_STOP = 1u << 11;
+
+// column c of the epilogue's matrix is stored as 128 floats, row r at (r ^ msw(c)): the MMA warpgroup's fragment stores
+// and the epilogue's reads (thread j reads row j of one column) are both free of bank conflicts
+__device__ __forceinline__ int msw(int c) { return ((c >> 1) & 3) << 3; }
 
 template <int D>
 struct Smem {
@@ -91,11 +93,12 @@ struct Smem {
     // operand slab: element (feature m, entry k) at byte (k/8)*LBO + (m/8)*128 + (m%8)*16 + (k%8)*2
     alignas(1024) unsigned char op[NO][PT][2][Cfg<D>::OP_BYTES];   // [stage][tile of the group][head|tail]
     alignas(128) float raw[NR][PT][TILE * D];          // gathered rows, pitch D
-    alignas(16) float bvec[NBV][KH][D];                // b = sum w q (one partial per convert set)
+    alignas(128) float mat[128 * 128];                 // fused mode: M of the row being solved (column-major, msw)
+    alignas(16) float bvec[NBV][KH][D];                // b = sum w q
     alignas(16) float sumq[NBV][KH][D];                // sum q (loss only)
     alignas(16) float xs[NXS][D];                      // 128-bit reads: every vector below is 16-byte aligned
     alignas(16) float pv[4][32];                       // CG direction of the warp that owns the block
-    alignas(16) float dl[NACC_MAX][4][32];             // [row slot][block]: the block's solution delta
+    alignas(16) float dl[4][32];                       // [block]: the block's solution delta
     alignas(16) float sws[NP][TILE];                   // gather plan: 2^e sqrt|w| per slot
     alignas(16) float wv[NP][TILE];                    //              w per slot
     alignas(16) int32_t keys[NP][TILE];                //              gathered row per slot
@@ -104,8 +107,7 @@ struct Smem {
     uint32_t meta_op[NO][PT];
     int badrow[NXS];
     alignas(8) uint64_t plan_full[NPG], plan_empty[NPG], raw_full[NR], raw_empty[NR], op_full[NO], op_empty[NO];
-    alignas(8) uint64_t acc_full[NACC_MAX], acc_empty[NACC_MAX], x_full[NXS], d_full[NACC_MAX][4];
-    uint32_t tmem_base;
+    alignas(8) uint64_t acc_full, acc_empty, x_full[NXS], d_full[4];
 };
 
 // PARTIAL = false: rows of a.row_list[row_begin..row_end) are solved in place.
@@ -116,6 +118,7 @@ struct TcArgs {
     const int32_t* items;   // PARTIAL: triples (row, chunk, scratch slot)
     float* scratch;         // PARTIAL: per slot D*D matrix + D (b) + D (sum q) + 4 (sum w, ...) floats
     int64_t split;          // PARTIAL: chunk length in nnz
+    int pass;               // PARTIAL, d = 256: which 128 x 128 block of the chunk matrix this launch accumulates (0..2)
     int debug;              // BFL_TC_DEBUG (timing experiments only; results are wrong): 1 no gathers, 2 no MMAs, 4 no convert math, 8 no epilogue math, 16 planner only
 };
 
@@ -160,7 +163,7 @@ __global__ void tc_scale_kernel(const unsigned int* __restrict__ ymax, const uns
 template <int D, bool PARTIAL, bool LOSS1>
 __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
     static_assert(D == 128 || (D == 256 && PARTIAL), "fused row solve: d = 128; split-row mode: d = 128 or 256");
-    constexpr int TILE = Cfg<D>::TILE, NACC = Cfg<D>::NACC, NF = Cfg<D>::NF, LBO = Cfg<D>::LBO;
+    constexpr int TILE = Cfg<D>::TILE, NF = Cfg<D>::NF, LBO = Cfg<D>::LBO;
     extern __shared__ __align__(1024) unsigned char smem_raw_[];
     Smem<D>& S = *reinterpret_cast<Smem<D>*>(smem_raw_);
     const AlsArgs& a = ta.a;
@@ -169,8 +172,7 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
 
     if (tid == 0) {
         for (int i = 0; i < NR; ++i) {
-            // every barrier counts WARPS, not threads: an arrive executed by 32 lanes is 32 serial barrier updates, and with
-            // per-thread arrivals the hand-offs alone cost ~700 cycles per tile (measured with all the math switched off)
+            // every barrier counts WARPS, not threads: an arrive executed by 32 lanes is 32 serial barrier updates
             mbar_init(&S.raw_full[i], N_CONV);
             mbar_init(&S.raw_empty[i], N_CONV);
         }
@@ -180,46 +182,19 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
         }
         for (int i = 0; i < NO; ++i) {
             mbar_init(&S.op_full[i], N_CONV);
-            mbar_init(&S.op_empty[i], 1);
+            mbar_init(&S.op_empty[i], 4);
         }
-        for (int i = 0; i < NACC; ++i) {
-            mbar_init(&S.acc_full[i], 1);
-            mbar_init(&S.acc_empty[i], 4);
-            for (int b = 0; b < 4; ++b) mbar_init(&S.d_full[i][b], 1);
-        }
+        mbar_init(&S.acc_full, 4);
+        mbar_init(&S.acc_empty, 4);
+        for (int b = 0; b < 4; ++b) mbar_init(&S.d_full[b], 1);
         for (int i = 0; i < NXS; ++i) {
             mbar_init(&S.x_full[i], 4);
             S.badrow[i] = 0;
         }
         mbar_init_fence();
     }
-    if (warp == W_MMA) tmem_alloc(&S.tmem_base, 512);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = S.tmem_base;
     const float scale = __ldg(a.tc_scales), inv2 = __ldg(a.tc_scales + 1);
-
-    // G + reg I -> tensor memory columns [0, D) (thread j of the epilogue holds matrix row j)
-    if (!PARTIAL && warp >= W_EPI && warp < W_EPI + 4) {
-        const int q = warp & 3, j = q * 32 + lane;
-#pragma unroll 1
-        for (int c = 0; c < D / 32; ++c) {
-            float v[32];
-#pragma unroll
-            for (int i = 0; i < 32; i += 4) {
-                const float4 g4 = __ldg(reinterpret_cast<const float4*>(a.G + (size_t)j * D + c * 32 + i));
-                v[i] = g4.x; v[i + 1] = g4.y; v[i + 2] = g4.z; v[i + 3] = g4.w;
-            }
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] += (c * 32 + i == j) ? a.reg : 0.f;
-            tmem_st32(tmem + ((uint32_t)(q * 32) << 16) + c * 32, v);
-        }
-        tmem_wait_st();
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
 
     const int64_t nitems = a.row_end - a.row_begin;
     const int64_t my_first = (int64_t)blockIdx.x;
@@ -243,7 +218,9 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
         }
     };
 
-    if (warp == W_PLAN) {
+    if (warp >= W_PLAN) {
+        setmaxnreg_dec<REG_PLAN>();
+        if (warp != W_PLAN) return;   // nothing after this point waits for the CTA as a whole
         // ================= planner: gather plans =================
         uint32_t gsl = 0, rph = 0, pe = 0;   // group slot, phase of plan_empty, tile within the group
         // begin a tile: its plan slot (the group's slots are claimed when its first tile starts)
@@ -409,15 +386,43 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
             __syncwarp();
             tile_end();
         } while (pe != 0);
-    } else if (warp == W_MMA) {
-        // ================= MMA issue =================
-        uint32_t os = 0, oph = 0, acc = 0, aph = 0;
-        const uint32_t idesc = idesc_f16_k(128, 128), idesc_w = idesc_f16_k(128, 256);   // d = 256: N = 256
-        bool row_open = false, stop = false;
+    } else if (warp >= W_MMA && warp < W_MMA + 4) {
+        setmaxnreg_inc<REG_MMA>();
+        // ================= MMA warpgroup =================
+        // The accumulated block: feature rows [r0, r0 + 128) x feature columns [c0, c0 + 128); d0 holds rows r0 .. r0 + 63,
+        // d1 rows r0 + 64 .. r0 + 127 (fragment layout: sm90_ptx.cuh)
+        const int r0 = (D == 256 && ta.pass == 2) ? 128 : 0, c0 = (D == 256 && ta.pass > 0) ? 128 : 0;
+        const int wq = warp - W_MMA;
+        const int fr = 16 * wq + (lane >> 2), fc = 2 * (lane & 3);   // fragment row / column of register 0
+        float d0[64], d1[64];
+        // a new row's accumulator: 2^2e (G + reg I) in fused mode (so that the epilogue reads one matrix), 0 for chunks
+        auto acc_init = [&]() {
+            const float s2 = scale * scale;
+#pragma unroll
+            for (int n = 0; n < 16; ++n)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int r = fr + 8 * h, c = 8 * n + fc;
+                    float2 g0 = make_float2(0.f, 0.f), g1 = make_float2(0.f, 0.f);
+                    if (!PARTIAL) {
+                        g0 = __ldg(reinterpret_cast<const float2*>(a.G + (size_t)r * D + c));
+                        g1 = __ldg(reinterpret_cast<const float2*>(a.G + (size_t)(r + 64) * D + c));
+                        g0.x += r == c ? a.reg : 0.f;
+                        g0.y += r == c + 1 ? a.reg : 0.f;
+                        g1.x += r + 64 == c ? a.reg : 0.f;
+                        g1.y += r + 64 == c + 1 ? a.reg : 0.f;
+                    }
+                    d0[4 * n + 2 * h] = g0.x * s2; d0[4 * n + 2 * h + 1] = g0.y * s2;
+                    d1[4 * n + 2 * h] = g1.x * s2; d1[4 * n + 2 * h + 1] = g1.y * s2;
+                }
+        };
+        uint32_t os = 0, oph = 0, aph = 0;
+        int64_t seq = 0;   // rows (items) finished so far
+        bool stop = false;
+        acc_init();
         while (!stop) {
             mbar_wait(&S.op_full[os], oph);
             fence_proxy_async_smem();   // the convert warps' generic-proxy operand stores -> visible to the tensor core's reads
-            tc_fence_after();
 #pragma unroll 1
             for (int e = 0; e < PT; ++e) {
                 const uint32_t meta = S.meta_op[os][e];
@@ -425,49 +430,83 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                     stop = true;
                     break;
                 }
-                if (meta & F_FIRST) {
-                    mbar_wait(&S.acc_empty[acc], aph ^ 1u);
-                    tc_fence_after();
-                    row_open = false;
-                }
-                if (lane == 0) {
-                    const int ksteps = (int)(meta & 0xffu);
-                    const uint32_t neg = (meta & F_NEG) ? IDESC_NEGATE_A : 0u;
-                    const uint32_t hi = s32(&S.op[os][e][0][0]), lo = s32(&S.op[os][e][1][0]);
-                    for (int ks = 0; ks < ((ta.debug & 2) ? 0 : ksteps); ++ks) {
-                        const uint32_t acc0 = (row_open || ks > 0) ? 1u : 0u;
-                        // K = 16 = two 8-k chunks: LBO apart; neighbouring 8-feature core matrices 128 B apart (SBO)
-                        const uint64_t dh = smem_desc(hi + ks * 2 * LBO, LBO, 128);
-                        const uint64_t dl = smem_desc(lo + ks * 2 * LBO, LBO, 128);
-                        if (D == 128) {
-                            const uint32_t dcol = tmem + D * (1 + acc);
-                            mma_f16(dcol, dh, dh, idesc | neg, acc0);
-                            mma_f16(dcol, dh, dl, idesc | neg, 1u);
-                            mma_f16(dcol, dl, dh, idesc | neg, 1u);
-                        } else {
-                            // rows 0..127 x columns 0..255 -> tensor-memory columns [0, 256)
-                            mma_f16(tmem, dh, dh, idesc_w | neg, acc0);
-                            mma_f16(tmem, dh, dl, idesc_w | neg, 1u);
-                            mma_f16(tmem, dl, dh, idesc_w | neg, 1u);
-                            // rows 128..255 x columns 128..255 -> tensor-memory columns [256, 384): features 128.. start 16
-                            // core matrices (2048 B) into the slab
-                            const uint64_t eh = smem_desc(hi + ks * 2 * LBO + 2048, LBO, 128);
-                            const uint64_t el = smem_desc(lo + ks * 2 * LBO + 2048, LBO, 128);
-                            mma_f16(tmem + 256, eh, eh, idesc | neg, acc0);
-                            mma_f16(tmem + 256, eh, el, idesc | neg, 1u);
-                            mma_f16(tmem + 256, el, eh, idesc | neg, 1u);
-                        }
+                const int ksteps = (ta.debug & 2) ? 0 : (int)(meta & 0xffu);
+                const uint32_t hi = s32(&S.op[os][e][0][0]), lo = s32(&S.op[os][e][1][0]);
+                wgmma_fence();
+#pragma unroll 1
+                for (int ks = 0; ks < ksteps; ++ks) {
+                    // K = 16 = two 8-k chunks LBO apart; neighbouring 8-feature core matrices 128 B apart (SBO); the
+                    // features f of an operand start f / 8 core matrices into the slab
+                    const uint32_t k0 = ks * 2 * LBO;
+                    const uint64_t ah0 = smem_desc(hi + k0 + r0 * 16, LBO, 128), ah1 = smem_desc(hi + k0 + (r0 + 64) * 16, LBO, 128);
+                    const uint64_t al0 = smem_desc(lo + k0 + r0 * 16, LBO, 128), al1 = smem_desc(lo + k0 + (r0 + 64) * 16, LBO, 128);
+                    const uint64_t bh = smem_desc(hi + k0 + c0 * 16, LBO, 128), bl = smem_desc(lo + k0 + c0 * 16, LBO, 128);
+                    if (meta & F_NEG) {
+                        wgmma_m64n128k16_f16<true>(d0, ah0, bh);
+                        wgmma_m64n128k16_f16<true>(d0, ah0, bl);
+                        wgmma_m64n128k16_f16<true>(d0, al0, bh);
+                        wgmma_m64n128k16_f16<true>(d1, ah1, bh);
+                        wgmma_m64n128k16_f16<true>(d1, ah1, bl);
+                        wgmma_m64n128k16_f16<true>(d1, al1, bh);
+                    } else {
+                        wgmma_m64n128k16_f16<false>(d0, ah0, bh);
+                        wgmma_m64n128k16_f16<false>(d0, ah0, bl);
+                        wgmma_m64n128k16_f16<false>(d0, al0, bh);
+                        wgmma_m64n128k16_f16<false>(d1, ah1, bh);
+                        wgmma_m64n128k16_f16<false>(d1, ah1, bl);
+                        wgmma_m64n128k16_f16<false>(d1, al1, bh);
                     }
-                    if (meta & F_LAST) mma_commit(&S.acc_full[acc]);
                 }
-                __syncwarp();
-                row_open = true;
+                wgmma_commit();
                 if (meta & F_LAST) {
-                    if (++acc == NACC) { acc = 0; aph ^= 1u; }
+                    wgmma_wait<0>();
+#pragma unroll
+                    for (int i = 0; i < 64; ++i) { acc_fence(d0[i]); acc_fence(d1[i]); }
+                    mbar_wait_idle(&S.acc_empty, aph ^ 1u);   // the epilogue is done with the previous row
+                    if (PARTIAL) {
+                        // the chunk of item my_first + seq * stride: float atomics (the chunks of one row are summed in
+                        // arrival order); pass 1 of d = 256 also adds the transposed block
+                        const int slot = ta.items[3 * (a.row_begin + my_first + seq * stride) + 2];
+                        float* sc = ta.scratch + (size_t)slot * scratch_floats<D>();
+#pragma unroll
+                        for (int n = 0; n < 16; ++n)
+#pragma unroll
+                            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                                for (int i = 0; i < 2; ++i) {
+                                    const int r = r0 + fr + 8 * h, c = c0 + 8 * n + fc + i;
+                                    const float v0 = d0[4 * n + 2 * h + i] * inv2, v1 = d1[4 * n + 2 * h + i] * inv2;
+                                    atomicAdd(sc + (size_t)r * D + c, v0);
+                                    atomicAdd(sc + (size_t)(r + 64) * D + c, v1);
+                                    if (r0 != c0) {
+                                        atomicAdd(sc + (size_t)c * D + r, v0);
+                                        atomicAdd(sc + (size_t)c * D + r + 64, v1);
+                                    }
+                                }
+                    } else {
+#pragma unroll
+                        for (int n = 0; n < 16; ++n)
+#pragma unroll
+                            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                                for (int i = 0; i < 2; ++i) {
+                                    const int r = fr + 8 * h, c = 8 * n + fc + i;
+                                    S.mat[c * 128 + (r ^ msw(c))] = d0[4 * n + 2 * h + i] * inv2;
+                                    S.mat[c * 128 + ((r + 64) ^ msw(c))] = d1[4 * n + 2 * h + i] * inv2;
+                                }
+                    }
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&S.acc_full);
+                    aph ^= 1u;
+                    ++seq;
+                    acc_init();
                 }
             }
-            if (lane == 0) mma_commit(&S.op_empty[os]);   // (after a stop nobody waits for it any more)
+            wgmma_wait<0>();   // the group's operand reads are done
+#pragma unroll
+            for (int i = 0; i < 64; ++i) { acc_fence(d0[i]); acc_fence(d1[i]); }
             __syncwarp();
+            if (lane == 0) mbar_arrive(&S.op_empty[os]);   // (after a stop nobody waits for it any more)
             if (++os == NO) { os = 0; oph ^= 1u; }
         }
     } else if (warp >= W_CONV && warp < W_CONV + N_CONV) {
@@ -484,11 +523,11 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
 #pragma unroll
         for (int f = 0; f < NF; ++f) { bacc[f] = make_float2(0.f, 0.f); qacc[f] = make_float2(0.f, 0.f); }
         // Gathers.  The convert warps issue the gathers themselves, GATHER_AHEAD groups before they consume the group:
-        // warp cw copies the TILE / 8 rows cw, cw + 8, ... of a planned tile with one coalesced 16-byte-per-lane cp.async per
-        // 512 bytes (SASS LDGSTS; a whole warp instruction moves a full row segment, and the issue cost is spread over
-        // eight warps that have issue slots to spare -- the 512-byte TMA bulk copies this replaces cost ~63-100 issue
-        // cycles each in a dedicated warp, see DESIGN.md) as one commit group per tile; before converting tile t a warp
-        // waits for its own group of tile t (cp.async.wait_group) and posts one arrival on the tile's mbarrier.
+        // warp cw copies the TILE / N_CONV rows cw, cw + N_CONV, ... of a planned tile with one coalesced 16-byte-per-lane
+        // cp.async per 512 bytes (SASS LDGSTS; a whole warp instruction moves a full row segment, so the issue cost is a
+        // few instructions per row -- a TMA bulk copy per gathered row would serialise on one issuing thread) as one
+        // commit group per group; before converting a group a warp waits for its own copies (cp.async.wait_group) and
+        // posts one arrival on the stage's mbarrier.
         const int cw = cta >> 5;
         uint32_t gs = 0, gph = 0, grs = 0, grph = 0;   // plan group slot / raw stage of the next group to gather
         bool plan_end = false;
@@ -502,17 +541,17 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
             const uint32_t gm0 = S.meta_raw[gs * PT], gm1 = S.meta_raw[gs * PT + 1];
             if (PT == 2 && !(ta.debug & 1) && ((gm0 | gm1) & F_STOP) == 0 && (gm0 & 0xffu) == TILE && (gm1 & 0xffu) == TILE) {
                 // two full tiles (the common case): straight-line copies, no per-row predicates
-                int32_t kk[PT][TILE / 8];
+                int32_t kk[PT][TILE / N_CONV];
 #pragma unroll
                 for (int e = 0; e < PT; ++e)
 #pragma unroll
-                    for (int i = 0; i < TILE / 8; ++i) kk[e][i] = S.keys[gs * PT + e][cw + 8 * i];
+                    for (int i = 0; i < TILE / N_CONV; ++i) kk[e][i] = S.keys[gs * PT + e][cw + N_CONV * i];
 #pragma unroll
                 for (int e = 0; e < PT; ++e)
 #pragma unroll
-                    for (int i = 0; i < TILE / 8; ++i) {
+                    for (int i = 0; i < TILE / N_CONV; ++i) {
                         const float* src = a.Y + (int64_t)kk[e][i] * a.ld + lane * 4;
-                        float* dst = &S.raw[grs][e][(cw + 8 * i) * D + lane * 4];
+                        float* dst = &S.raw[grs][e][(cw + N_CONV * i) * D + lane * 4];
 #pragma unroll
                         for (int c = 0; c < D / 128; ++c) cp_async16_cg(dst + c * 128, src + c * 128);
                     }
@@ -525,8 +564,8 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                 } else {
                     const int gcnt = (ta.debug & 1) ? 0 : (int)(gmeta & 0xffu);
 #pragma unroll
-                    for (int i = 0; i < TILE / 8; ++i) {
-                        const int slot = cw + 8 * i;
+                    for (int i = 0; i < TILE / N_CONV; ++i) {
+                        const int slot = cw + N_CONV * i;
                         if (slot < gcnt) {
                             const float* src = a.Y + (int64_t)S.keys[gs * PT + e][slot] * a.ld + lane * 4;
                             float* dst = &S.raw[grs][e][slot * D + lane * 4];
@@ -735,68 +774,33 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
             if (++os == NO) { os = 0; oph ^= 1u; }
         }
     } else {
-        // ================= epilogue: explicit-matrix block Gauss-Seidel / CG, systolic over rows =================
-        const int q = warp & 3;                  // tensor-memory lane quarter == column block owned by this warp
+        // ================= epilogue: explicit-matrix block Gauss-Seidel / CG, systolic over the blocks of a row =================
+        const int q = warp & 3;                  // column block owned by this warp
         const int j = q * 32 + lane;             // matrix row
-        const uint32_t lane_off = (uint32_t)(q * 32) << 16;
         float* pv = S.pv[q];
         double l_nume = 0.0, l_deno = 0.0;
         const float tol = a.tol;
         if constexpr (PARTIAL) {
-            // add every chunk's matrix / vectors to the row's scratch block (float atomics: the chunks of one row are
-            // summed in arrival order); the four warps are independent here
+            // the chunk's matrix went to scratch straight from the MMA warpgroup; add its vectors (once per chunk: pass 0)
             int row = 0, slot = 0, nrow = 0, nslot = 0;
             int64_t beg, n = 0, nbeg, nn = 0;
             if (my_first < nitems) item_info(my_first, row, beg, n, slot);
             for (int64_t seq = 0; my_first + seq * stride < nitems; ++seq) {
                 const int64_t nit = my_first + (seq + 1) * stride;
                 if (nit < nitems) item_info(nit, nrow, nbeg, nn, nslot);
-                const uint32_t acc = (uint32_t)(seq % NACC), aph = (uint32_t)((seq / NACC) & 1);
+                const uint32_t aph = (uint32_t)(seq & 1);
                 const uint32_t bs = (uint32_t)(seq & (NBV - 1));
-                mbar_wait_idle(&S.acc_full[acc], aph);
-                tc_fence_after();
+                mbar_wait_idle(&S.acc_full, aph);
                 float* sc = ta.scratch + (size_t)slot * scratch_floats<D>();
-                if constexpr (D == 128) {
-                    const uint32_t dbase = tmem + lane_off + D * (1 + acc);
-#pragma unroll 1
-                    for (int c = 0; c < D / 32; ++c) {
-                        float v[32];
-                        tmem_ld32(dbase + c * 32, v);
-                        tmem_wait_ld();
-#pragma unroll
-                        for (int i = 0; i < 32; ++i) atomicAdd(sc + (size_t)j * D + c * 32 + i, v[i] * inv2);
+                if (ta.pass == 0) {
+                    for (int jj = j; jj < D; jj += 128) {
+                        atomicAdd(sc + (size_t)D * D + jj, S.bvec[bs][0][jj] + (KH == 2 ? S.bvec[bs][KH - 1][jj] : 0.f));
+                        if (LOSS1) atomicAdd(sc + (size_t)D * D + D + jj, S.sumq[bs][0][jj] + (KH == 2 ? S.sumq[bs][KH - 1][jj] : 0.f));
                     }
-                } else {
-                    // tensor-memory columns [0,256): matrix rows 0..127; [256,384): rows 128..255 x columns 128..255;
-                    // rows 128..255 x columns 0..127 are the transpose of rows 0..127 x columns 128..255
-#pragma unroll 1
-                    for (int c = 0; c < 8; ++c) {
-                        float v[32];
-                        tmem_ld32(tmem + lane_off + c * 32, v);
-                        tmem_wait_ld();
-#pragma unroll
-                        for (int i = 0; i < 32; ++i) {
-                            atomicAdd(sc + (size_t)j * D + c * 32 + i, v[i] * inv2);
-                            if (c >= 4) atomicAdd(sc + (size_t)(c * 32 + i) * D + j, v[i] * inv2);
-                        }
-                    }
-#pragma unroll 1
-                    for (int c = 0; c < 4; ++c) {
-                        float v[32];
-                        tmem_ld32(tmem + lane_off + 256 + c * 32, v);
-                        tmem_wait_ld();
-#pragma unroll
-                        for (int i = 0; i < 32; ++i) atomicAdd(sc + (size_t)(128 + j) * D + 128 + c * 32 + i, v[i] * inv2);
-                    }
+                    if (LOSS1 && j == 0) atomicAdd(sc + (size_t)D * D + 2 * D, S.wsum[bs][0] + (KH == 2 ? S.wsum[bs][KH - 1] : 0.f));
                 }
-                for (int jj = j; jj < D; jj += 128) {
-                    atomicAdd(sc + (size_t)D * D + jj, S.bvec[bs][0][jj] + (KH == 2 ? S.bvec[bs][KH - 1][jj] : 0.f));
-                    if (LOSS1) atomicAdd(sc + (size_t)D * D + D + jj, S.sumq[bs][0][jj] + (KH == 2 ? S.sumq[bs][KH - 1][jj] : 0.f));
-                }
-                if (LOSS1 && j == 0) atomicAdd(sc + (size_t)D * D + 2 * D, S.wsum[bs][0] + (KH == 2 ? S.wsum[bs][KH - 1] : 0.f));
-                tc_fence_before();
                 __syncwarp();
-                if (lane == 0) mbar_arrive(&S.acc_empty[acc]);
+                if (lane == 0) mbar_arrive(&S.acc_empty);
                 row = nrow; slot = nslot; n = nn;
             }
         } else {
@@ -819,6 +823,8 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&S.x_full[0]);
             }
+            // element (j, c) of the row's matrix
+            auto mat = [&](int c) -> float { return S.mat[c * 128 + (j ^ msw(c))]; };
             for (int64_t seq = 0; row >= 0; ++seq) {
                 // look-ahead loads
                 const int row3 = row_of(seq + 3);
@@ -829,56 +835,44 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                     __syncwarp();
                     if (lane == 0) mbar_arrive(&S.x_full[(seq + 1) & (NXS - 1)]);
                 }
-                const uint32_t acc = (uint32_t)(seq % NACC), aph = (uint32_t)((seq / NACC) & 1);
+                const uint32_t aph = (uint32_t)(seq & 1);
                 const uint32_t bs = (uint32_t)(seq & (NBV - 1));
                 const uint32_t xsl = (uint32_t)(seq & (NXS - 1));
                 const float* xs = S.xs[xsl];
                 mbar_wait(&S.x_full[xsl], (uint32_t)((seq / NXS) & 1));
-                mbar_wait_idle(&S.acc_full[acc], aph);
-                tc_fence_after();
+                mbar_wait_idle(&S.acc_full, aph);
                 if (ta.debug & 8) {
-                    tc_fence_before();
                     __syncwarp();
-                    if (lane == 0) mbar_arrive(&S.acc_empty[acc]);
+                    if (lane == 0) mbar_arrive(&S.acc_empty);
                     row = row1; row1 = row2; row2 = row3;
                     xj = x1; x1 = x2;
                     continue;
                 }
-                const uint32_t dbase = tmem + lane_off + 128 * (1 + acc);
                 const float bj = S.bvec[bs][0][j] + (KH == 2 ? S.bvec[bs][KH - 1][j] : 0.f);
-                // ---- h = (G + reg I) x + 2^-2e A x - b  (A = the accumulator); keep the diagonal block of M in registers ----
-                float hG = 0.f, hD = 0.f;
+                // ---- h = M x - b; keep the diagonal block of M in registers ----
+                float hM = 0.f;
                 float md[32];
 #pragma unroll
                 for (int c = 0; c < D / 32; ++c) {
-                    float dv[32], gv[32];
-                    tmem_ld32(dbase + c * 32, dv);
-                    tmem_ld32(tmem + lane_off + c * 32, gv);
-                    tmem_wait_ld();
-                    float h0 = 0.f, h1 = 0.f, g0 = 0.f, g1 = 0.f;
+                    float h0 = 0.f, h1 = 0.f;
 #pragma unroll
                     for (int i = 0; i < 32; i += 4) {
                         const float4 x4 = *reinterpret_cast<const float4*>(xs + c * 32 + i);
-                        h0 = fmaf(dv[i], x4.x, h0); h1 = fmaf(dv[i + 1], x4.y, h1);
-                        h0 = fmaf(dv[i + 2], x4.z, h0); h1 = fmaf(dv[i + 3], x4.w, h1);
-                        g0 = fmaf(gv[i], x4.x, g0); g1 = fmaf(gv[i + 1], x4.y, g1);
-                        g0 = fmaf(gv[i + 2], x4.z, g0); g1 = fmaf(gv[i + 3], x4.w, g1);
+                        const float m0 = mat(c * 32 + i), m1 = mat(c * 32 + i + 1), m2 = mat(c * 32 + i + 2), m3 = mat(c * 32 + i + 3);
+                        h0 = fmaf(m0, x4.x, h0); h1 = fmaf(m1, x4.y, h1);
+                        h0 = fmaf(m2, x4.z, h0); h1 = fmaf(m3, x4.w, h1);
+                        if (c == q) { md[i] = m0; md[i + 1] = m1; md[i + 2] = m2; md[i + 3] = m3; }
                     }
-                    hD += h0 + h1;
-                    hG += g0 + g1;
-                    if (c == q) {
-#pragma unroll
-                        for (int i = 0; i < 32; ++i) md[i] = fmaf(dv[i], inv2, gv[i]);
-                    }
+                    hM += h0 + h1;
                 }
-                hD *= inv2;
                 if (a.compute_loss) {
                     // als.cc:298-321 with the pre-update row: reg*kappa*|x|^2 (both axes); item side additionally
-                    // x G x + sum_obs[(1+w)(yhat-1)^2 - yhat^2] = x G x + x D x - 2 x.(b + sum q) + (n + sum w)
+                    // x G x + sum_obs[(1+w)(yhat-1)^2 - yhat^2] = x G x + x D x - 2 x.(b + sum q) + (n + sum w),
+                    // where x (G + D) x = x M x - reg |x|^2
                     const float kappa = a.adaptive_reg ? nlen : 1.0f;
                     double t = (double)(kappa * a.reg * xj * xj);
                     if (a.axis == 1) {
-                        t += (double)xj * (double)(hG - a.reg * xj) + (double)xj * (double)hD -
+                        t += (double)xj * (double)hM - (double)(a.reg * xj * xj) -
                              2.0 * (double)xj * ((double)bj + (double)S.sumq[bs][0][j] + (KH == 2 ? (double)S.sumq[bs][KH - 1][j] : 0.0));
                         if (j == 0) {
                             const double ws = (double)S.wsum[bs][0] + (KH == 2 ? (double)S.wsum[bs][KH - 1] : 0.0);
@@ -888,30 +882,28 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                     }
                     l_nume += t;
                 }
-                float h = hG + hD - bj;
+                float h = hM - bj;
                 // ---- fold in the deltas of the earlier blocks as they appear: h -= M[j, B] . delta_B ----
 #pragma unroll 1
                 for (int B = 0; B < q; ++B) {
-                    float dv[32], gv[32];
-                    tmem_ld32(dbase + B * 32, dv);
-                    tmem_ld32(tmem + lane_off + B * 32, gv);
-                    mbar_wait(&S.d_full[acc][B], aph);
-                    tmem_wait_ld();
+                    float mv[32];
+#pragma unroll
+                    for (int i = 0; i < 32; ++i) mv[i] = mat(B * 32 + i);
+                    mbar_wait(&S.d_full[B], aph);
                     float u0 = 0.f, u1 = 0.f;
 #pragma unroll
                     for (int i = 0; i < 32; i += 4) {
-                        const float4 d4 = *reinterpret_cast<const float4*>(&S.dl[acc][B][i]);
-                        u0 = fmaf(fmaf(dv[i], inv2, gv[i]), d4.x, u0);
-                        u1 = fmaf(fmaf(dv[i + 1], inv2, gv[i + 1]), d4.y, u1);
-                        u0 = fmaf(fmaf(dv[i + 2], inv2, gv[i + 2]), d4.z, u0);
-                        u1 = fmaf(fmaf(dv[i + 3], inv2, gv[i + 3]), d4.w, u1);
+                        const float4 d4 = *reinterpret_cast<const float4*>(&S.dl[B][i]);
+                        u0 = fmaf(mv[i], d4.x, u0);
+                        u1 = fmaf(mv[i + 1], d4.y, u1);
+                        u0 = fmaf(mv[i + 2], d4.z, u0);
+                        u1 = fmaf(mv[i + 3], d4.w, u1);
                     }
                     h -= u0 + u1;
                 }
-                // this warp's reads of the accumulator are done
-                tc_fence_before();
+                // this warp's reads of the matrix are done
                 __syncwarp();
-                if (lane == 0) mbar_arrive(&S.acc_empty[acc]);
+                if (lane == 0) mbar_arrive(&S.acc_empty);
                 // ---- 3-step CG on the own diagonal block (als.cc:324-345) ----
                 float xv = 0.f;
                 {
@@ -948,10 +940,10 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                 a.X[(int64_t)row * a.ld + j] = v;
                 for (int pr = 0; pr < a.n_peer; ++pr) a.peerX[pr][(int64_t)row * a.ld + j] = v;
                 if (q < 3) {
-                    S.dl[acc][q][lane] = xv;
+                    S.dl[q][lane] = xv;
                     if (badw && lane == 0) atomicOr(&S.badrow[xsl], 1);
                     __syncwarp();
-                    if (lane == 0) mbar_arrive(&S.d_full[acc][q]);
+                    if (lane == 0) mbar_arrive(&S.d_full[q]);
                 }
                 // the warp of the last block has seen every earlier block's flag (set before that block's delta was
                 // published) and zeroes the whole row if any block came out non-finite
@@ -981,9 +973,6 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == W_MMA) tmem_dealloc(tmem, 512);
 }
 
 // ---- host side ---------------------------------------------------------------------------------
@@ -1052,14 +1041,16 @@ int tc_launch_partial(const AlsArgs& a, const int32_t* items, int64_t nitems, fl
     BFL_CUDA(cudaMemsetAsync(scratch, 0, sizeof(float) * scratch_floats<D>() * (size_t)nslots, st));
     const size_t smem = sizeof(Smem<D>);
     const int grid = (int)std::min<int64_t>(nitems, (int64_t)num_sms);
-    if (a.compute_loss && a.axis == 1) {
-        BFL_CUDA(cudaFuncSetAttribute(als_tc_kernel<D, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        als_tc_kernel<D, true, true><<<grid, THREADS, smem, st>>>(ta);
-    } else {
-        BFL_CUDA(cudaFuncSetAttribute(als_tc_kernel<D, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        als_tc_kernel<D, true, false><<<grid, THREADS, smem, st>>>(ta);
+    for (ta.pass = 0; ta.pass < (D == 128 ? 1 : 3); ++ta.pass) {
+        if (a.compute_loss && a.axis == 1) {
+            BFL_CUDA(cudaFuncSetAttribute(als_tc_kernel<D, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            als_tc_kernel<D, true, true><<<grid, THREADS, smem, st>>>(ta);
+        } else {
+            BFL_CUDA(cudaFuncSetAttribute(als_tc_kernel<D, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            als_tc_kernel<D, true, false><<<grid, THREADS, smem, st>>>(ta);
+        }
+        BFL_LAUNCHED();
     }
-    BFL_LAUNCHED();
     return BFL_OK;
 }
 
@@ -1073,6 +1064,7 @@ inline int tc_launch(const AlsArgs& a, int num_sms, cudaStream_t st) {
     ta.items = nullptr;
     ta.scratch = nullptr;
     ta.split = 0;
+    ta.pass = 0;
     ta.debug = getenv("BFL_TC_DEBUG") ? atoi(getenv("BFL_TC_DEBUG")) : 0;
     const size_t smem = sizeof(Smem<128>);
     const int grid = (int)std::min<int64_t>(nrows, (int64_t)num_sms);

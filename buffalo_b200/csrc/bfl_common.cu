@@ -24,11 +24,12 @@ int require_device() {
     }
     int dev = 0;
     BFL_CUDA(cudaGetDevice(&dev));
-    int major = 0;
+    int major = 0, minor = 0;
     BFL_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-    if (major != 10)
-        BFL_FAIL(BFL_ERR_CUDA, "buffalo_b200 kernels are compiled for sm_100a only; current device has compute capability major " +
-                                   std::to_string(major));
+    BFL_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
+    if (major != 9 || minor != 0)   // sm_90a code (wgmma) runs on compute capability 9.0 only
+        BFL_FAIL(BFL_ERR_CUDA, "buffalo_b200 kernels are compiled for sm_90a only; current device has compute capability " +
+                                   std::to_string(major) + "." + std::to_string(minor));
     return BFL_OK;
 }
 
@@ -199,7 +200,7 @@ bool JsonOpt::load(const char* path, std::string* err) {
 extern "C" {
 const char* bfl_last_error(void) { return bfl::t_last_error.c_str(); }
 int bfl_abi_version(void) { return 1; }
-int bfl_compiled_sm(void) { return 100; }
+int bfl_compiled_sm(void) { return 90; }
 int64_t bfl_kernel_launch_count(void) { return (int64_t)bfl::g_launches.load(); }
 void* bfl_ipc_open(const void* handle64) {
     if (!handle64) {

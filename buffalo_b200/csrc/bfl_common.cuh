@@ -1,4 +1,4 @@
-// Shared host/device helpers for the buffalo_b200 CUDA backend (sm_100a only).
+// Shared host/device helpers for the buffalo_b200 CUDA backend (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,5 +1,5 @@
 #!/bin/bash
-# Builds libbuffalo_b200.so (sm_100a only) next to the Python package.
+# Builds libbuffalo_b200.so (sm_90a only) next to the Python package.
 set -e
 HERE="$(cd "$(dirname "$0")" && pwd)"
 OUT="$HERE/../libbuffalo_b200.so"
@@ -8,7 +8,7 @@ SRCS="$HERE/bfl_common.cu $HERE/als.cu"
 [ -f "$HERE/sgd.cu" ] && SRCS="$SRCS $HERE/sgd.cu"
 [ -f "$HERE/topk.cu" ] && SRCS="$SRCS $HERE/topk.cu"
 [ -f "$HERE/ingest.cu" ] && SRCS="$SRCS $HERE/ingest.cu"
-"$NVCC" -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 \
+"$NVCC" -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 \
     -ccbin /usr/bin/g++ -Xcompiler -fPIC,-O3,-Wall -shared \
     ${BFL_PTXAS_V:+-Xptxas -v} -o "$OUT" $SRCS
 echo "built $OUT"

@@ -182,18 +182,28 @@ int bits_for(long long v) {
 extern "C" {
 
 // Cumulative popularity table on the device: cum[i] = sum_{j <= i} count(j)^power (int64), bpr.py:99-111.
+// grid cap of the grid-stride helper kernels: 16 CTAs of 256 threads per SM of the current device
+static int ingest_grid_cap() {
+    int dev = 0, sms = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+        sms <= 0)
+        sms = 1;
+    return sms * 16;
+}
+
 int bfl_popularity_table_device(const int32_t* d_keys, int64_t nnz, int32_t n_items, int power, int64_t* d_cum, void* stream) {
     if (BFL_OK != require_device()) return BFL_ERR_CUDA;
+    const int cap = ingest_grid_cap();
     if (!d_cum || n_items <= 0 || nnz < 0 || (nnz > 0 && !d_keys) || power < 0) BFL_FAIL(BFL_ERR_ARG, "bad popularity-table arguments");
     cudaStream_t st = (cudaStream_t)stream;
     BFL_CUDA(cudaMemsetAsync(d_cum, 0, sizeof(int64_t) * n_items, st));
     if (nnz > 0) {
-        hist_i32_kernel<<<(unsigned)std::min<int64_t>((nnz + 255) / 256, 148 * 16), 256, 0, st>>>(
+        hist_i32_kernel<<<(unsigned)std::min<int64_t>((nnz + 255) / 256, cap), 256, 0, st>>>(
             d_keys, nnz, reinterpret_cast<long long*>(d_cum), n_items);
         BFL_LAUNCHED();
     }
     if (power != 1) {
-        ipow_kernel<<<(unsigned)std::min<int64_t>((n_items + 255) / 256, 148 * 16), 256, 0, st>>>(
+        ipow_kernel<<<(unsigned)std::min<int64_t>((n_items + 255) / 256, cap), 256, 0, st>>>(
             reinterpret_cast<long long*>(d_cum), n_items, power);
         BFL_LAUNCHED();
     }
@@ -227,7 +237,7 @@ int bfl_csr_from_triples_device(const int32_t* d_major, const int32_t* d_minor, 
     // indptr: histogram of the major index + inclusive scan
     BFL_CUDA(cudaMemsetAsync(d_indptr, 0, sizeof(int64_t) * num_major, st));
     if (nnz == 0) return BFL_OK;
-    const unsigned g = (unsigned)std::min<int64_t>((nnz + 255) / 256, 148 * 16);
+    const unsigned g = (unsigned)std::min<int64_t>((nnz + 255) / 256, ingest_grid_cap());
     hist_i32_kernel<<<g, 256, 0, st>>>(d_major, nnz, reinterpret_cast<long long*>(d_indptr), num_major);
     BFL_LAUNCHED();
     int rc = inclusive_scan_i64(reinterpret_cast<long long*>(d_indptr), reinterpret_cast<long long*>(d_indptr), num_major, st);

@@ -46,7 +46,7 @@ class Stream(Data):
             self.open(path)
             return
         if self.opt.data.sppmi:
-            raise NotImplementedError("SPPMI (CoFactor only) is outside the B200 hot-path scope")
+            raise NotImplementedError("SPPMI (CoFactor only) is outside the H100 hot-path scope")
         sessions = [ln.split() for ln in _lines(self.opt.input.main)]
         uids = _lines(self.opt.input.uid) if self.opt.input.uid else None
         num_users = len(uids) if uids is not None else len(sessions)

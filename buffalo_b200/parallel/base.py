@@ -83,7 +83,7 @@ class ParBPRMF(ParALS):
 
 def _unsupported(name):
     def ctor(*a, **k):
-        raise NotImplementedError(name + " is outside the B200 hot-path scope")
+        raise NotImplementedError(name + " is outside the H100 hot-path scope")
     return ctor
 
 

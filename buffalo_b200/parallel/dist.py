@@ -1,6 +1,6 @@
 """Row-sharded multi-GPU driver for ALS (SURVEY.md 8e): one process per GPU, contiguous user / item row ranges
 per rank, full factor replicas everywhere, ONE exchange step per half-epoch -- an in-place all-gather of the
-freshly updated factor shard over NCCL (NVLink 5 / NVSwitch).  The same class drives the gloo CPU tests
+freshly updated factor shard over NCCL (NVLink / NVSwitch).  The same class drives the gloo CPU tests
 (tests/test_dist_cpu.py) with a CPU row-update function, so the sharding / exchange logic is covered without GPUs.
 """
 import numpy as np

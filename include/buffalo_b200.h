@@ -1,5 +1,5 @@
 /*
- * buffalo_b200.h -- C ABI of the B200-native matrix-factorisation training backend.
+ * buffalo_b200.h -- C ABI of the H100-native matrix-factorisation training backend.
  *
  * This is the drop-in boundary: every entry point below replaces one method of the
  * reference's Cython holder classes (the `self.obj` object driven by
@@ -22,7 +22,7 @@
  *  - "host" entry points take host pointers and perform the H2D/D2H copies themselves,
  *    exactly like the reference CUDA backend (als.cu:361-364,403); "device" entry points
  *    take device pointers (e.g. torch CUDA tensor storage) and run entirely on `stream`.
- *  - there is no CPU fallback: every entry point fails loudly when no sm_100 device is
+ *  - there is no CPU fallback: every entry point fails loudly when no sm_90 device is
  *    present.
  */
 #ifndef BUFFALO_B200_H_

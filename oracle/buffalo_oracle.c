@@ -14,14 +14,14 @@
  * restatement (oracle/np_mirror.py) in tests/test_oracle.py.
  *
  * Third-party arithmetic the reference delegates to and that is absent from
- * /root/reference: Eigen @ 3147391d (3rd/eigen3, .SUBMODULES.json:9-15) for
+ * the reference repository: Eigen @ 3147391d (3rd/eigen3, .SUBMODULES.json:9-15) for
  * A.llt().solve / A.ldlt().solve (lib/algo.cc:53,56) and the dense row/GEMM
  * expressions.  Restated here as plain fp32 loops (Cholesky LL^T and unpivoted
  * LDL^T); summation order inside Eigen's kernels is not reproducible and is not
  * part of the contract (tolerance 1e-3 relative on factors, BASELINE.json).
  *
  * Every function cites the reference file:line it follows (paths relative to
- * /root/reference).  Plain C11 + OpenMP; build with oracle/Makefile.
+ * the reference repository).  Plain C11 + OpenMP; build with oracle/Makefile.
  */
 #include <math.h>
 #include <stdint.h>

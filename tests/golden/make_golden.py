@@ -3,7 +3,7 @@
 There are no golden vectors in the reference (SURVEY.md 8c) and it cannot be built here, so these
 fixtures freeze the outputs of oracle/buffalo_oracle.c (itself cross-checked against the NumPy fp64
 restatement) at small sizes.  The CUDA parity tests replay them through the C ABI on the GPU box,
-where /root/reference and a working gcc are not required.
+where neither the reference checkout nor a working gcc is required.
 
 Run from the repo root:  python tests/golden/make_golden.py
 """

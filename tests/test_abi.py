@@ -1,5 +1,5 @@
 """CPU-side checks of the drop-in boundary: the C-ABI library loads, exports every symbol that
-include/buffalo_b200.h declares, and refuses to run without a Blackwell GPU (no CPU fallback)."""
+include/buffalo_b200.h declares, and refuses to run without a Hopper (sm_90) GPU (no CPU fallback)."""
 import ctypes
 import os
 import re
@@ -25,10 +25,10 @@ def test_header_symbols_exported():
     assert set(names) == set(_cabi.PROTOTYPES), set(names) ^ set(_cabi.PROTOTYPES)
 
 
-def test_library_is_sm100_only():
+def test_library_is_sm90_only():
     from buffalo_b200 import _cabi
     lib = _cabi.lib()
-    assert lib.bfl_compiled_sm() == 100
+    assert lib.bfl_compiled_sm() == 90
     assert lib.bfl_abi_version() == 1
 
 

@@ -138,7 +138,7 @@ def test_c1_config_training_trajectory(cuda_lib):
 @pytest.mark.parametrize("d", [128, 64, 32, 96, 256])
 def test_tuned_kernel_all_row_length_classes(cuda_lib, d):
     """Rows are binned by length (<=32, 64, 128, 256, 512, 1536, 12288, longer).  Default (_b200_kernel_mode=0):
-    at d=128 every row above 32 nnz goes through the tcgen05 kernel (als_tc.cuh: fused up to 12288 nnz, split-row +
+    at d=128 every row above 32 nnz goes through the tensor-core kernel (als_tc.cuh: fused up to 12288 nnz, split-row +
     explicit solve beyond), at d=256 the rows beyond 12288 do, everything else through the tuned SIMT kernels;
     _b200_kernel_mode=2 = SIMT kernels only (rows beyond 12288 on the generic kernel), 1 = generic kernels.
     One input that hits every class, checked against the oracle and the generic kernel."""
@@ -190,7 +190,7 @@ def test_tuned_kernel_all_row_length_classes(cuda_lib, d):
 @pytest.mark.parametrize("d", [128, 256])
 def test_long_rows_split_tensor_core_path(cuda_lib, d):
     """Rows far beyond the SIMT kernels' cap (2e4, 2e5 and 1e6 nnz; Zipf head items of BASELINE configs[4]) are cut into
-    8192-entry chunks over the SMs, their explicit matrices summed by the tcgen05 kernel and solved by
+    8192-entry chunks over the SMs, their explicit matrices summed by the tensor-core (wgmma) kernel and solved by
     als_explicit_solve_kernel.  Bar: 1e-3 against the fp32 oracle; where the oracle's own sequential fp32 sums over
     1e6 terms drift further than that from the fp64 mirror, the GPU must be at least as close to the mirror."""
     from oracle import np_mirror

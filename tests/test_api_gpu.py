@@ -1,4 +1,4 @@
-"""End-to-end tests of the drop-in Python API on the GPU: `import buffalo` resolves to the B200 backend and the
+"""End-to-end tests of the drop-in Python API on the GPU: `import buffalo` resolves to the H100 backend and the
 reference's own usage (examples/example_als.py, tests/algo/base.py) works unchanged.  The reference's quality
 floors (tests/algo/base.py:83-97: ALS ndcg > 0.06, map > 0.04; BPR/WARP ndcg > 0.03, map > 0.02 on ml-100k) are
 applied to a synthetic ml-100k-shaped matrix with planted low-rank structure (the real file is an LFS pointer)."""
