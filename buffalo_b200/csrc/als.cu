@@ -20,6 +20,7 @@ struct bfl_als {
                           // rows of 513..1536 nnz on the re-gathering class
     int tc_min_class = 2; // first row-length class (als_fast.cuh) solved by the tensor-core kernel (rows of <= 64 nnz stay on
                           // the SIMT classes 0, 1: an epilogue per row costs more than their whole SIMT solve; measured 400 vs 411 ms)
+    int64_t sub_chunk_nnz = 16ll << 20;   // host-pointer path: entries per pipelined sub-chunk of one partial_update call
 
     // factors: either owned device mirrors of retained host pointers, or borrowed device memory
     float* hostP = nullptr;
@@ -81,6 +82,8 @@ int als_apply_options(bfl_als* h, const JsonOpt& j) {
     // rows of classes >= 2 (> 64 nnz) on the tensor-core kernel: the fastest of the routings measured at C2 on an H100
     // (DESIGN.md 4.1)
     h->tc_min_class = std::max(0, std::min(7, j.integer("_b200_tc_min_class", 2)));
+    h->sub_chunk_nnz = (int64_t)j.number("_b200_sub_chunk_nnz", (double)(16ll << 20));
+    if (h->sub_chunk_nnz < 1) BFL_FAIL(BFL_ERR_OPTION, "_b200_sub_chunk_nnz must be positive");
     std::string optimizer = j.string("optimizer", "manual_cg");
     if (h->d >= 128) optimizer = "ialspp";  // als.cc:46
     if (optimizer == "llt") h->optimizer_code = 0;
@@ -199,7 +202,7 @@ int solve_rows(bfl_als* h, int axis, int64_t row_begin, int64_t row_end, const i
     if (h->kernel_mode != 1 && fast_als_applicable(h->optimizer_code, h->d, h->vdim, h->block_size)) {
         const int32_t* left = nullptr;
         int64_t nleft = 0;
-        // d = 128: classes tcmin..5 (33..1536 nnz) on the fused tensor-core kernel, classes 6, 7 (longer) in its split-row
+        // d = 128: classes tcmin..5 (65..1536 nnz by default) on the fused tensor-core kernel, classes 6, 7 (longer) in its split-row
         // mode; d = 256: classes 6, 7 (beyond 1536 nnz) in split-row mode
         int tcmin = FAST_NCLASS, splitmin = FAST_NCLASS;
         if (h->kernel_mode == 0 && tc::tc_applicable(h->optimizer_code, h->d, h->vdim, h->block_size)) {
@@ -364,7 +367,7 @@ int bfl_als_partial_update(bfl_als_t* h, int32_t start_x, int32_t next_x, const 
     // The chunk is cut into row-aligned sub-chunks of <= SUB entries and software-pipelined over three streams:
     // H2D of sub-chunk k+1 (keys, vals) | row solves of sub-chunk k | D2H of the rows updated by sub-chunk k-1.
     // With pinned host buffers the PCIe traffic of the reference protocol (als.cu:361-364,403) overlaps the math.
-    const int64_t SUB = 16ll << 20;
+    const int64_t SUB = h->sub_chunk_nnz;
     int64_t maxsub = 0;
     std::vector<int64_t> cut;  // row boundaries
     cut.push_back(start_x);

@@ -11,65 +11,11 @@ import os
 import numpy as np
 import pytest
 
-from tests.helpers import init_factors, make_csr, rel_err, transpose_csr
+from tests.helpers import (FACTOR_TOL, check_loss, check_rows, csr_from_lengths, full_opt, gpu_half, init_factors,
+                           make_csr, oracle_half, rel_err, transpose_csr)
 
 pytestmark = pytest.mark.gpu
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-FACTOR_TOL = 1e-3
-
-
-def full_opt(**kw):
-    opt = dict(d=20, optimizer="manual_cg", num_workers=8, compute_loss_on_training=True, alpha=8.0, reg_u=0.1,
-               reg_i=0.1, block_size=32, adaptive_reg=False, num_cg_max_iters=3, eps=1e-10, cg_tolerance=1e-10)
-    opt.update(kw)
-    return opt
-
-
-def gpu_half(opt, P, Q, indptr, keys, vals, axis, chunks=1, placeholder=None):
-    """One half-epoch through the host-pointer C ABI (init / initialize_model / precompute / partial_update)."""
-    from buffalo_b200 import backend
-    obj = backend.CuALS()
-    assert obj.init(opt)
-    vdim = obj.get_vdim()
-    d = opt["d"]
-    Pp = np.zeros((P.shape[0], vdim), np.float32)
-    Qp = np.zeros((Q.shape[0], vdim), np.float32)
-    Pp[:, :d], Qp[:, :d] = P[:, :d], Q[:, :d]
-    obj.initialize_model(Pp, Qp)
-    if placeholder is not None:
-        obj.set_placeholder(placeholder[0], placeholder[1], len(keys))
-    obj.precompute(axis)
-    rows = P.shape[0] if axis == 0 else Q.shape[0]
-    bounds = np.linspace(0, rows, chunks + 1).astype(int)
-    nume = deno = 0.0
-    for a, b in zip(bounds[:-1], bounds[1:]):
-        beg = 0 if a == 0 else int(indptr[a - 1])
-        end = int(indptr[b - 1]) if b > 0 else 0
-        k = np.ascontiguousarray(keys[beg:end]) if end > beg else np.zeros(1, np.int32)
-        v = np.ascontiguousarray(vals[beg:end]) if end > beg else np.zeros(1, np.float32)
-        n_, d_ = obj.partial_update(int(a), int(b), indptr, k, v, axis)
-        nume += n_
-        deno += d_
-    X = Pp if axis == 0 else Qp
-    assert not X[:, d:].any(), "padding columns must stay zero"
-    return X[:, :d].copy(), nume, deno
-
-
-def oracle_half(opt, P, Q, indptr, keys, vals, axis):
-    import oracle
-    o = oracle.OracleALS()
-    o.init(opt)
-    P1, Q1 = P.copy(), Q.copy()
-    o.initialize_model(P1, Q1)
-    o.precompute(axis)
-    rows = P.shape[0] if axis == 0 else Q.shape[0]
-    n, dn = o.partial_update(0, rows, indptr, keys, vals, axis)
-    return (P1 if axis == 0 else Q1), n, dn
-
-
-def check_loss(n, dn, n0, dn0):
-    assert abs(n - n0) <= 1e-4 * max(1.0, abs(n0)), (n, n0)
-    assert abs(dn - dn0) <= 1e-4 * max(1.0, abs(dn0)), (dn, dn0)
 
 
 @pytest.mark.parametrize("case", json.load(open(os.path.join(GOLDEN, "golden_als.json")))["cases"],
@@ -135,13 +81,14 @@ def test_c1_config_training_trajectory(cuda_lib):
         assert abs(rmse_g - rmse_o) < 1e-4 * rmse_o
 
 
-@pytest.mark.parametrize("d", [128, 64, 32, 96, 256])
+@pytest.mark.parametrize("d", [128, 64, 32, 96, 160, 192, 224, 256])
 def test_tuned_kernel_all_row_length_classes(cuda_lib, d):
     """Rows are binned by length (<=32, 64, 128, 256, 512, 1536, 12288, longer).  Default (_b200_kernel_mode=0):
-    at d=128 every row above 32 nnz goes through the tensor-core kernel (als_tc.cuh: fused up to 12288 nnz, split-row +
-    explicit solve beyond), at d=256 the rows beyond 12288 do, everything else through the tuned SIMT kernels;
+    at d=128 the rows of 65..1536 nnz go through the fused tensor-core kernel (als_tc.cuh), the longer ones through its
+    split-row mode (2048-entry chunks + explicit solve); at d=256 the rows beyond 1536 nnz take the split-row mode;
+    everything else runs on the tuned SIMT kernels (d = 160..256 read the Gram matrix through L1/L2).
     _b200_kernel_mode=2 = SIMT kernels only (rows beyond 12288 on the generic kernel), 1 = generic kernels.
-    One input that hits every class, checked against the oracle and the generic kernel."""
+    One input that hits every class, checked row by row against the oracle and against the generic kernel."""
     rng = np.random.default_rng(d)
     lengths = np.concatenate([rng.integers(1, 33, 300), rng.integers(33, 65, 200), rng.integers(65, 129, 150),
                               rng.integers(129, 257, 80), rng.integers(257, 513, 40), rng.integers(513, 1025, 20),
@@ -149,9 +96,7 @@ def test_tuned_kernel_all_row_length_classes(cuda_lib, d):
                               [12289, 13000, 1536, 1537, 1024, 1025, 512, 513, 32, 33, 0, 0, 1]])
     rng.shuffle(lengths)
     U, I = len(lengths), 14000
-    keys = np.concatenate([np.sort(rng.choice(I, size=n, replace=False)) for n in lengths]).astype(np.int32)
-    indptr = np.cumsum(lengths).astype(np.int64)
-    vals = rng.integers(1, 4, len(keys)).astype(np.float32)
+    indptr, keys, vals = csr_from_lengths(lengths, I, rng)
     opt = full_opt(d=d, optimizer="ialspp", block_size=32)
     P = init_factors(U, d, d, 1, scale=0.05, signed=True)
     Q = init_factors(I, d, d, 2, scale=0.05, signed=True)
@@ -164,8 +109,8 @@ def test_tuned_kernel_all_row_length_classes(cuda_lib, d):
         assert rel_err(Xf, X0) < FACTOR_TOL and rel_err(Xg, X0) < FACTOR_TOL and rel_err(Xs, X0) < FACTOR_TOL
         assert rel_err(Xf, Xg) < FACTOR_TOL
         # no single row is off either (the Frobenius norm would hide one bad row-length class)
-        row_err = np.linalg.norm(Xf - X0, axis=1) / np.maximum(np.linalg.norm(X0, axis=1), 1e-6)
-        assert row_err.max() < 5e-3, (int(row_err.argmax()), int(lengths[row_err.argmax()]), float(row_err.max()))
+        row_err = check_rows({"default": Xf, "simt": Xs}, X0, P, Q, indptr, keys, vals, o, 0, label="d=%d" % d)
+        assert row_err["default"].max() < 5e-3, (int(row_err["default"].argmax()), float(row_err["default"].max()))
         check_loss(nf, dnf, n0, dn0)
         check_loss(ns, dns, n0, dn0)
         Xr, nr, dnr = gpu_half(dict(o, _b200_kernel_mode=4), P, Q, indptr, keys, vals, 0)   # 513..1536 re-gathered
@@ -190,16 +135,14 @@ def test_tuned_kernel_all_row_length_classes(cuda_lib, d):
 @pytest.mark.parametrize("d", [128, 256])
 def test_long_rows_split_tensor_core_path(cuda_lib, d):
     """Rows far beyond the SIMT kernels' cap (2e4, 2e5 and 1e6 nnz; Zipf head items of BASELINE configs[4]) are cut into
-    8192-entry chunks over the SMs, their explicit matrices summed by the tensor-core (wgmma) kernel and solved by
-    als_explicit_solve_kernel.  Bar: 1e-3 against the fp32 oracle; where the oracle's own sequential fp32 sums over
-    1e6 terms drift further than that from the fp64 mirror, the GPU must be at least as close to the mirror."""
-    from oracle import np_mirror
+    2048-entry chunks over the SMs, their explicit matrices summed by the tensor-core (wgmma) kernel and solved by
+    als_explicit_solve_kernel.  Bar (check_rows): 1e-3 against the fp32 oracle per row; where the oracle's own
+    sequential fp32 sums over 1e6 terms drift further than that from the fp64 mirror, the GPU must be at least as close
+    to the mirror."""
     rng = np.random.default_rng(d + 1)
     lengths = np.array([20000, 200000, 1000000, 700, 12289, 40, 16385, 8193], dtype=np.int64)
     U, I = len(lengths), 1_200_000
-    keys = np.concatenate([np.sort(rng.choice(I, size=n, replace=False)) for n in lengths]).astype(np.int32)
-    indptr = np.cumsum(lengths).astype(np.int64)
-    vals = rng.integers(1, 4, len(keys)).astype(np.float32)
+    indptr, keys, vals = csr_from_lengths(lengths, I, rng)
     opt = full_opt(d=d, optimizer="ialspp", block_size=32)
     P = init_factors(U, d, d, 1, scale=0.05, signed=True)
     Q = init_factors(I, d, d, 2, scale=0.05, signed=True)
@@ -208,15 +151,8 @@ def test_long_rows_split_tensor_core_path(cuda_lib, d):
         Pa, Qa = (P, Q) if axis == 0 else (Q, P)
         X0, n0, dn0 = oracle_half(opt, Pa, Qa, indptr, keys, vals, axis)
         Xf, nf, dnf = gpu_half(opt, Pa, Qa, indptr, keys, vals, axis)
-        row_err = np.linalg.norm(Xf - X0, axis=1) / np.maximum(np.linalg.norm(X0, axis=1), 1e-6)
-        if row_err.max() >= FACTOR_TOL:
-            # judge against the fp64 mirror row by row
-            Xup, Yop = (Pa, Qa) if axis == 0 else (Qa, Pa)
-            Xm, _, _ = np_mirror.als_half_epoch(Xup[:U], Yop, indptr, keys, vals, opt, axis)
-            eg = np.linalg.norm(Xf - Xm, axis=1) / np.maximum(np.linalg.norm(Xm, axis=1), 1e-6)
-            eo = np.linalg.norm(X0 - Xm, axis=1) / np.maximum(np.linalg.norm(Xm, axis=1), 1e-6)
-            assert (eg <= np.maximum(eo * 1.5, FACTOR_TOL)).all(), (axis, eg.tolist(), eo.tolist())
-        assert np.isfinite(Xf).all()
+        Xup, Yop = (Pa, Qa) if axis == 0 else (Qa, Pa)
+        check_rows({"default": Xf}, X0, Xup, Yop, indptr, keys, vals, opt, axis, label="axis %d" % axis)
         assert abs(nf - n0) <= 2e-4 * max(1.0, abs(n0)), (nf, n0)
         assert abs(dnf - dn0) <= 1e-4 * max(1.0, abs(dn0)), (dnf, dn0)
 
@@ -252,8 +188,9 @@ def test_d128_reference_init_three_iterations(cuda_lib):
 
 
 def test_chunked_equals_whole_and_placeholder(cuda_lib):
-    # BufferedDataMatrix feeds row-aligned chunks (buffered_data.py:85-118); results must not depend on chunking
-    U, I, nnz, d = 2000, 1500, 60000, 128
+    # BufferedDataMatrix feeds row-aligned chunks (buffered_data.py:85-118); results must not depend on chunking.
+    # ~160 entries per item, so that the item rows (axis 1) run on the fused tensor-core kernel
+    U, I, nnz, d = 2000, 1500, 240000, 128
     indptr, keys, vals, _ = make_csr(U, I, nnz, seed=99, empty_rows=30)
     cind, ckeys, cvals = transpose_csr(indptr, keys, vals, U, I)
     opt = full_opt(d=d)
