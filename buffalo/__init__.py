@@ -11,6 +11,7 @@ from buffalo_b200 import __version__  # noqa: F401
 _ALIASES = {
     "buffalo.algo": "buffalo_b200.algo", "buffalo.algo.als": "buffalo_b200.algo.als",
     "buffalo.algo.bpr": "buffalo_b200.algo.bpr", "buffalo.algo.warp": "buffalo_b200.algo.warp",
+    "buffalo.algo.plsi": "buffalo_b200.algo.plsi",
     "buffalo.algo.base": "buffalo_b200.algo.base", "buffalo.algo.options": "buffalo_b200.algo.options",
     "buffalo.data": "buffalo_b200.data", "buffalo.data.base": "buffalo_b200.data.base",
     "buffalo.data.mm": "buffalo_b200.data.mm", "buffalo.data.stream": "buffalo_b200.data.stream",

@@ -77,6 +77,24 @@ PROTOTYPES = {
     "bfl_sgd_epoch": (C.c_int, [_vp]),
     "bfl_sgd_current_lr": (_d, [_vp]),
     "bfl_sgd_read_stats": (C.c_int, [_vp, _pd, _pi64]),
+    # PLSI
+    "bfl_plsi_create": (_vp, []),
+    "bfl_plsi_destroy": (None, [_vp]),
+    "bfl_plsi_init": (C.c_int, [_vp, _cs]),
+    "bfl_plsi_init_json": (C.c_int, [_vp, _cs]),
+    "bfl_plsi_get_vdim": (C.c_int, [_vp]),
+    "bfl_plsi_initialize_model": (C.c_int, [_vp, _vp, _i32, _vp, _i32]),
+    "bfl_plsi_set_model": (C.c_int, [_vp, _vp, _i32, _vp, _i32]),
+    "bfl_plsi_reset": (C.c_int, [_vp]),
+    "bfl_plsi_partial_update": (C.c_int, [_vp, _i32, _i32, _vp, _vp, _vp, _pd]),
+    "bfl_plsi_normalize": (C.c_int, [_vp, _f, _f]),
+    "bfl_plsi_swap": (C.c_int, [_vp]),
+    "bfl_plsi_release": (C.c_int, [_vp]),
+    "bfl_plsi_bind_factors_device": (C.c_int, [_vp, _vp, _i64, _vp, _i64]),
+    "bfl_plsi_bind_csr_device": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64]),
+    "bfl_plsi_update_device": (C.c_int, [_vp, _i64, _i64, _vp, _vp]),
+    "bfl_plsi_normalize_device": (C.c_int, [_vp, _f, _f, _vp]),
+    "bfl_plsi_swap_device": (C.c_int, [_vp, _vp]),
     # evaluation top-k
     "bfl_topk_device": (C.c_int, [_vp, _i64, C.c_int, _vp, _i64, C.c_int, _vp, C.c_int, C.c_int, _vp, _vp, _vp]),
     "bfl_topk_host": (C.c_int, [_vp, _i64, C.c_int, _vp, _i64, C.c_int, _vp, C.c_int, C.c_int, _vp, _vp]),

@@ -3,5 +3,6 @@
 from buffalo_b200.algo.als import ALS, inited_CUALS
 from buffalo_b200.algo.base import Algo, Serializable
 from buffalo_b200.algo.bpr import BPRMF, inited_CUBPR
-from buffalo_b200.algo.options import AlgoOption, ALSOption, BPRMFOption, WARPOption
+from buffalo_b200.algo.options import AlgoOption, ALSOption, BPRMFOption, PLSIOption, WARPOption
+from buffalo_b200.algo.plsi import PLSI
 from buffalo_b200.algo.warp import WARP

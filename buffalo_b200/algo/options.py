@@ -25,6 +25,9 @@ _WARP = dict(accelerator=False, evaluation_period=5, num_workers=1, hyper_thread
              reg_j=0.0, optimizer="adagrad", lr=0.05, min_lr=0.0001, beta1=0.9, beta2=0.999, eps=1e-10,
              per_coordinate_normalize=False, model_path="", data_opt={})   # options.py:286-311
 
+_PLSI = dict(d=20, num_iters=10, num_workers=1, alpha1=1.0, alpha2=1.0, eps=1e-10, model_path="", save_factors=False,
+             data_opt={}, inherit_opt={})                                  # options.py:372-384
+
 ALS_OPTIMIZERS = ["llt", "ldlt", "manual_cg", "eigen_cg", "eigen_bicg", "eigen_gmres", "eigen_dgmres",
                   "eigen_minres", "ialspp"]                                 # options.py:90-94
 B200_ALS_OPTIMIZERS = ["llt", "ldlt", "manual_cg", "ialspp"]
@@ -64,15 +67,18 @@ class WARPOption(AlgoOption):
     _specific = _WARP
 
 
+class PLSIOption(AlgoOption):
+    _specific = _PLSI
+
+
 def _out_of_scope(name):
     class _Opt(AlgoOption):
         def get_default_option(self):
-            raise NotImplementedError(name + " is outside the H100 hot-path scope (ALS, BPRMF, WARP only)")
+            raise NotImplementedError(name + " is outside the H100 hot-path scope (ALS, BPRMF, WARP, PLSI only)")
     _Opt.__name__ = name
     return _Opt
 
 
 EALSOption = _out_of_scope("EALSOption")
 CFROption = _out_of_scope("CFROption")
-PLSIOption = _out_of_scope("PLSIOption")
 W2VOption = _out_of_scope("W2VOption")

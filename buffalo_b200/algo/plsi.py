@@ -1,0 +1,255 @@
+"""pLSI trainer: the reference's Python EM driver (buffalo/algo/plsi.py) on top of the H100 backend.
+
+Two feeding modes, same results:
+  * resident (default when the rowwise CSR and the factors fit in device memory): the CSR and the factor matrices live
+    on the GPU for the whole of train(); one update / normalize / swap launch set per iteration;
+  * chunked: the reference's own protocol -- reset, obj.partial_update(start_x, next_x, indptr, keys, vals) per
+    BufferedDataMatrix chunk, normalize, swap (plsi.py:132-160).
+The factor arrays are [rows, d] (plsi.py:107-111: not padded).
+"""
+import json
+import time
+
+import numpy as np
+
+from buffalo_b200 import data as _data
+from buffalo_b200.algo.base import Algo, Serializable
+from buffalo_b200.algo.options import PLSIOption
+from buffalo_b200.backend import CuPLSI
+from buffalo_b200.data.base import Data
+from buffalo_b200.data.buffered_data import BufferedDataMatrix
+from buffalo_b200.evaluate import Evaluable
+from buffalo_b200.misc import log
+
+
+class PLSI(Algo, PLSIOption, Evaluable, Serializable):
+    """Probabilistic latent semantic indexing trained by EM -- drop-in for buffalo.algo.plsi.PLSI."""
+
+    def __init__(self, opt_path=None, *args, **kwargs):
+        Algo.__init__(self, *args, **kwargs)
+        PLSIOption.__init__(self, *args, **kwargs)
+        Evaluable.__init__(self, *args, **kwargs)
+        Serializable.__init__(self, *args, **kwargs)
+        if opt_path is None:
+            opt_path = PLSIOption().get_default_option()
+        self.logger = log.get_logger("PLSI")
+        self.opt, self.opt_path = self.get_option(opt_path)
+        self.obj = CuPLSI()
+        assert self.obj.init(bytes(self.opt_path, "utf-8")), \
+            "putting parameter to cython object failed (%s)" % getattr(self.obj, "last_error", "")
+        self.data = None
+        data = kwargs.get("data")
+        data_opt = kwargs.get("data_opt", self.opt.get("data_opt"))
+        if data_opt:
+            self.data = _data.load(data_opt)
+            assert self.data.data_type == "matrix"
+            self.data.create()
+        elif isinstance(data, Data):
+            self.data = data
+        self.logger.info("PLSI ({})".format(json.dumps(self.opt, indent=2)))
+        if self.data:
+            self.logger.info(self.data.show_info())
+            assert self.data.data_type in ["matrix"]
+
+    @staticmethod
+    def new(path, data_fields=[]):
+        return PLSI.instantiate(PLSIOption, path, data_fields)
+
+    def set_data(self, data):
+        assert isinstance(data, Data), "Wrong instance: {}".format(type(data))
+        self.data = data
+
+    def normalize(self, group="item"):
+        if group == "item":
+            self.Q /= (np.sum(self.Q, axis=0, keepdims=True) + self.opt.eps)
+        elif group == "user":
+            self.P /= (np.sum(self.P, axis=1, keepdims=True) + self.opt.eps)
+
+    def inherit(self):
+        """Copies the rows of a saved model whose ids also occur here (plsi.py:62-89)."""
+        def _inherit(key):
+            if key == "user":
+                self.build_userid_map()
+            else:
+                self.build_itemid_map()
+            curr_idmap = self._idmanager.userid_map if key == "user" else self._idmanager.itemid_map
+            prev_idmap = prev_model._idmanager.userid_map if key == "user" else prev_model._idmanager.itemid_map
+            curr_obj = self.P if key == "user" else self.Q
+            prev_obj = prev_model.P if key == "user" else prev_model.Q
+            curr_d, prev_d = curr_obj.shape[1], prev_obj.shape[1]
+            assert curr_d == prev_d, f"Dimension mismatch. Current dimension: {curr_d} / Previous dimension: {prev_d}"
+            for k, curr_idx in curr_idmap.items():
+                if k in prev_idmap:
+                    curr_obj[curr_idx] = prev_obj[prev_idmap[k]]
+
+        if not self.opt["inherit_opt"]:
+            return
+        inherit_opt = self.opt.inherit_opt
+        prev_model = PLSI.new(inherit_opt.model_path)
+        if inherit_opt.get("inherit_user", False):
+            self.logger.info("Inherit from previous user matrix")
+            _inherit("user")
+        if inherit_opt.get("inherit_item", False):
+            self.logger.info("Inherit from previous item matrix")
+            _inherit("item")
+
+    def initialize(self):
+        super().initialize()
+        self.buf = BufferedDataMatrix()
+        self.buf.initialize(self.data)
+        self.buf.set_group("rowwise")
+        self.init_factors()
+        self.inherit()
+
+    def init_factors(self):
+        assert self.data, "Did not set data"
+        header = self.data.get_header()
+        self.num_items = header["num_items"]
+        self.num_users = header["num_users"]
+        self.num_nnz = header["num_nnz"]
+        self.vdim = self.obj.get_vdim()
+        for name, rows in [("P", self.num_users), ("Q", self.num_items)]:
+            setattr(self, name, None)
+            setattr(self, name, np.zeros((rows, self.opt.d), dtype="float32"))
+        self.obj.initialize_model(self.P, self.Q)
+
+    # ---- queries (host) -----------------------------------------------------------------------
+    def _get_topk_recommendation(self, rows, topk, pool=None):
+        topks = super()._get_topk_recommendation(self.P[rows], self.Q, pb=None, Qb=None, pool=pool, topk=topk,
+                                                 num_workers=self.opt.num_workers)
+        return zip(rows, topks)
+
+    def _get_most_similar_item(self, col, topk, pool):
+        return super()._get_most_similar_item(col, topk, self.Q, True, pool)      # plsi.py:121-122
+
+    def get_scores(self, row_col_pairs):
+        return {(r, c): self.P[r].dot(self.Q[c]) for r, c in row_col_pairs}
+
+    def _get_scores(self, row, col):
+        return (self.P[row] * self.Q[col]).sum(axis=1)
+
+    def _get_feature(self, index, group="item"):
+        if group == "item":
+            return self.Q[index]
+        elif group == "user":
+            return self.P[index]
+        return None
+
+    # ---- training -----------------------------------------------------------------------------
+    def _iterate(self):
+        """The reference protocol: reset, partial_update per rowwise chunk, normalize, swap (plsi.py:132-160)."""
+        self.obj.reset()
+        loss_nume, loss_deno = 0.0, 0.0
+        feed_t, update_t, updated = 0.0, 0.0, 0
+        for sz in self.buf.fetch_batch():
+            st = time.time()
+            start_x, next_x, indptr, keys, vals = self.buf.get()
+            feed_t += time.time() - st
+            st = time.time()
+            loss_nume += self.obj.partial_update(start_x, next_x, indptr, keys, vals)
+            update_t += time.time() - st
+            loss_deno += np.sum(vals)
+            updated += sz
+        self.obj.normalize(self.opt.alpha1, self.opt.alpha2)
+        self.obj.swap()
+        self.logger.debug(f"updated processed({updated}) elapsed(data feed: {feed_t:0.5f} update: {update_t:0.5f})")
+        return loss_nume, loss_deno
+
+    def _resident_capable(self):
+        if self.opt.get("_b200_resident") is False:
+            return False
+        try:
+            import torch
+            free, _ = torch.cuda.mem_get_info()
+        except Exception:
+            return False
+        h = self.data.get_header()
+        # rowwise CSR + factors + the item accumulator
+        need = h["num_nnz"] * 8 + h["num_users"] * (self.vdim * 4 + 9) + h["num_items"] * self.vdim * 8
+        return need * 1.3 < free
+
+    def _train_resident(self, training_callback):
+        import torch
+        dev = torch.device("cuda", torch.cuda.current_device())
+        d = self.opt.d
+
+        def padded(F):
+            T = torch.zeros((F.shape[0], self.vdim), dtype=torch.float32, device=dev)
+            T[:, :d] = torch.from_numpy(F).to(dev)
+            return T
+        tP, tQ = padded(self.P), padded(self.Q)
+        self.obj.bind_factors(tP, tQ)
+        grp = self.data.get_group("rowwise")
+        n = int(grp["indptr"][-1]) if len(grp["indptr"]) else 0
+        vals = np.ascontiguousarray(grp["val"][:n], dtype=np.float32)
+        t = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a, dtype=dt)).to(dev)  # noqa: E731
+        self.obj.bind_csr(t(grp["indptr"][:], np.int64), t(grp["key"][:n] if n else np.zeros(1), np.int32),
+                          t(vals if n else np.zeros(1), np.float32))
+        loss_deno = float(np.sum(vals, dtype=np.float64))
+        loss = torch.zeros(1, dtype=torch.float64, device=dev)
+        rows = self.P.shape[0]
+
+        def sync_back():
+            self.P[:] = tP[:, :d].cpu().numpy()
+            self.Q[:] = tQ[:, :d].cpu().numpy()
+
+        def one_iteration():
+            loss.zero_()
+            self.obj.update_device(0, rows, loss)
+            self.obj.normalize_device(self.opt.alpha1, self.opt.alpha2)
+            self.obj.swap_device()
+            return float(loss.cpu().numpy()[0]), loss_deno
+        try:
+            return self._epoch_loop(one_iteration, sync_back, training_callback)
+        finally:
+            sync_back()
+            self.obj.set_model(self.P, self.Q)   # leave the holder on host-pointer semantics
+
+    def _train_chunked(self, training_callback):
+        return self._epoch_loop(self._iterate, lambda: None, training_callback)
+
+    def _epoch_loop(self, one_iteration, sync_back, training_callback):
+        best_loss, loss, self.validation_result = 1e+10, None, {}
+        for i in range(self.opt.num_iters):
+            start_t = time.time()
+            nume, deno = one_iteration()
+            train_t = time.time() - start_t
+            loss = nume / (deno + self.opt.eps)                              # plsi.py:171
+            metrics = {"train_loss": loss}
+            if self.opt.validation and self.opt.evaluation_on_learning and self.periodical(self.opt.evaluation_period, i):
+                start_t = time.time()
+                sync_back()
+                self.validation_result = self.get_validation_results()
+                vali_t = time.time() - start_t
+                val_str = " ".join([f"{k}:{v:0.5f}" for k, v in self.validation_result.items()])
+                self.logger.info(f"Validation: {val_str} Elapsed {vali_t:0.3f} secs")
+                metrics.update({"val_%s" % k: v for k, v in self.validation_result.items()})
+                if callable(training_callback):
+                    training_callback(i, metrics)
+            self.logger.info("Iteration %d: Loss %.3f Elapsed %.3f secs" % (i + 1, loss, train_t))
+            if self.opt.save_best:
+                sync_back()
+            best_loss = self.save_best_only(loss, best_loss, i)
+            if self.early_stopping(loss):
+                break
+        return loss
+
+    def train(self, training_callback=None):
+        self.logger.info(f"Train pLSI, K: {self.opt.d}, alpha1: {self.opt.alpha1}, "
+                         f"alpha2: {self.opt.alpha2}, num_workers: {self.opt.num_workers}")
+        for name in ("P", "Q"):          # factors replaced or inherited by the user: the backend needs float32 [rows, d]
+            setattr(self, name, np.ascontiguousarray(getattr(self, name), dtype=np.float32))
+        self.obj.set_model(self.P, self.Q)
+        if self._resident_capable():
+            loss = self._train_resident(training_callback)
+        else:
+            loss = self._train_chunked(training_callback)
+        ret = {"train_loss": loss}
+        ret.update({"val_%s" % k: v for k, v in self.validation_result.items()})
+        return ret
+
+    def _get_data(self):
+        return super()._get_data() + [("opt", self.opt), ("Q", self.Q), ("P", self.P)]
+
+    def get_evaluation_metrics(self):
+        return ["train_loss", "val_rmse", "val_ndcg", "val_map", "val_accuracy", "val_error"]

@@ -1,8 +1,8 @@
 """Backend holder objects: the `self.obj` of the algo drivers.
 
-``CuALS`` / ``CuSGD`` expose exactly the method set of the reference's Cython holders
+``CuALS`` / ``CuSGD`` / ``CuPLSI`` expose exactly the method set of the reference's Cython holders
 (buffalo/algo/_als.pyx:28-63, buffalo/algo/cuda/_als.pyx:25-67, buffalo/algo/_bpr.pyx:34-92,
-buffalo/algo/cuda/_bpr.pyx:27-80, buffalo/algo/_warp.pyx:34-92) on top of the C ABI, plus a
+buffalo/algo/cuda/_bpr.pyx:27-80, buffalo/algo/_warp.pyx:34-92, buffalo/algo/_plsi.pyx:13-57) on top of the C ABI, plus a
 device-resident path that takes torch CUDA tensors (PyTorch is used for device memory and
 streams only).
 """
@@ -302,6 +302,110 @@ class CuSGD(object):
         loss, n = C.c_double(0.0), C.c_int64(0)
         _cabi.check(self._lib.bfl_sgd_read_stats(self._h, C.byref(loss), C.byref(n)), "read_stats")
         return loss.value, n.value
+
+
+class CuPLSI(object):
+    """pLSI backend (CyPLSI, buffalo/algo/_plsi.pyx:13-57).  Holder methods take the [rows, d] host arrays of
+    buffalo/algo/plsi.py:107-111; the device-resident path takes [rows, vdim] torch CUDA tensors."""
+
+    def __init__(self):
+        self._lib = _cabi.lib()
+        self._h = self._lib.bfl_plsi_create()
+        if not self._h:
+            raise MemoryError("bfl_plsi_create")
+        self._keep = []
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            self._lib.bfl_plsi_destroy(h)
+
+    # --- reference method set -------------------------------------------------------------
+    def init(self, opt_path):
+        """opt_path: bytes/str path of the JSON option file (plsi.py:31), or a dict."""
+        data, is_path = _opt_bytes(opt_path)
+        rc = self._lib.bfl_plsi_init(self._h, data) if is_path else self._lib.bfl_plsi_init_json(self._h, data)
+        if rc == 1:  # BFL_ERR_OPTION
+            self.last_error = self._lib.bfl_last_error().decode("utf-8", "replace")
+            return False
+        _cabi.check(rc, "bfl_plsi_init")
+        if is_path:
+            with open(data.decode("utf-8")) as fin:
+                self._d = int(json.load(fin)["d"])
+        else:
+            self._d = int(json.loads(data.decode("utf-8"))["d"])
+        return True
+
+    def get_vdim(self):
+        return self._lib.bfl_plsi_get_vdim(self._h)
+
+    def _factors(self, P, Q):
+        pP, pQ = _host(P, np.float32, 2, "P"), _host(Q, np.float32, 2, "Q")
+        if P.shape[1] != self._d or Q.shape[1] != self._d:
+            raise ValueError("factor matrices must have d=%d columns" % self._d)
+        self._keep = [P, Q]  # native side retains the pointers (plsi.cc:46-47)
+        return pP, pQ
+
+    def initialize_model(self, P, Q):
+        """Fills P [users, d] and Q [items, d] in place with the normalised random start (plsi.cc:44-70)."""
+        pP, pQ = self._factors(P, Q)
+        _cabi.check(self._lib.bfl_plsi_initialize_model(self._h, pP, P.shape[0], pQ, Q.shape[0]), "initialize_model")
+
+    def set_model(self, P, Q):
+        """Retains P and Q and uploads their current values (inherited or user-replaced factors)."""
+        pP, pQ = self._factors(P, Q)
+        _cabi.check(self._lib.bfl_plsi_set_model(self._h, pP, P.shape[0], pQ, Q.shape[0]), "set_model")
+
+    def reset(self):
+        _cabi.check(self._lib.bfl_plsi_reset(self._h), "reset")
+
+    def partial_update(self, start_x, next_x, indptr, keys, vals):
+        loss = C.c_double(0.0)
+        _cabi.check(self._lib.bfl_plsi_partial_update(self._h, int(start_x), int(next_x),
+                                                      _host(indptr, np.int64, 1, "indptr"),
+                                                      _host(keys, np.int32, 1, "keys"),
+                                                      _host(vals, np.float32, 1, "vals"), C.byref(loss)),
+                    "partial_update")
+        return loss.value
+
+    def normalize(self, alpha1, alpha2):
+        _cabi.check(self._lib.bfl_plsi_normalize(self._h, float(alpha1), float(alpha2)), "normalize")
+
+    def swap(self):
+        _cabi.check(self._lib.bfl_plsi_swap(self._h), "swap")
+
+    def release(self):
+        _cabi.check(self._lib.bfl_plsi_release(self._h), "release")
+        self._keep = []
+
+    # --- device-resident path ---------------------------------------------------------------
+    def bind_factors(self, P, Q):
+        """P, Q: torch float32 CUDA tensors [rows, vdim] (padding columns zero), updated in place."""
+        vdim = self.get_vdim()
+        assert P.shape[1] == vdim and Q.shape[1] == vdim, "factor tensors need vdim=%d columns" % vdim
+        self._keep = [P, Q]
+        _cabi.check(self._lib.bfl_plsi_bind_factors_device(self._h, _dev(P, "float32", "P"), P.shape[0],
+                                                           _dev(Q, "float32", "Q"), Q.shape[0]), "bind_factors")
+
+    def bind_csr(self, indptr, keys, vals):
+        """Rowwise CSR: indptr int64[rows] END offsets, keys int32[nnz], vals float32[nnz] torch CUDA tensors."""
+        self._keep += [indptr, keys, vals]
+        _cabi.check(self._lib.bfl_plsi_bind_csr_device(self._h, _dev(indptr, "int64", "indptr"),
+                                                       _dev(keys, "int32", "keys"), _dev(vals, "float32", "vals"),
+                                                       indptr.shape[0], keys.shape[0]), "bind_csr")
+
+    def update_device(self, row_begin, row_end, loss=None, stream=None):
+        """loss: optional torch float64 CUDA tensor[1] receiving (+=) -sum v log(norm)."""
+        lp = _dev(loss, "float64", "loss") if loss is not None else None
+        _cabi.check(self._lib.bfl_plsi_update_device(self._h, int(row_begin), int(row_end), lp, _stream_ptr(stream)),
+                    "update_device")
+
+    def normalize_device(self, alpha1, alpha2, stream=None):
+        _cabi.check(self._lib.bfl_plsi_normalize_device(self._h, float(alpha1), float(alpha2), _stream_ptr(stream)),
+                    "normalize_device")
+
+    def swap_device(self, stream=None):
+        _cabi.check(self._lib.bfl_plsi_swap_device(self._h, _stream_ptr(stream)), "swap_device")
 
 
 def device_available():

@@ -1,0 +1,595 @@
+// pLSI backend: EM pass, normalisation and initialisation kernels + C ABI.
+// Replaces plsi::CPLSI (lib/algo_impl/plsi/plsi.cc) behind CyPLSI (buffalo/algo/_plsi.pyx:13-57).
+//
+// One EM iteration is reset -> update over the rowwise CSR -> normalize -> swap (buffalo/algo/plsi.py:132-160).
+// The update is one pass over the rows: every nonzero (x, c, v) gathers the current item row Q[c], forms
+// latent = max(P[x] * Q[c], 1e-10) over the d real columns, and adds v * latent / sum(latent) into the new user row
+// and into the new item row.  Only row x's warp reads P[x] during the pass, so the new user row overwrites P[x] in
+// place; the new item rows go to the library-owned accumulator Qacc through float4 atomics.  A per-row flag records
+// which user rows the pass wrote: a row the pass never reached counts as zero in normalize, as the reference's
+// zeroed accumulator would.
+//
+// Layout: factor rows have pitch vdim = ceil4(d) on the device; padding columns stay zero.  The holder entry points
+// take the caller's [rows x d] host arrays (plsi.py:107-111 does not pad) and copy with a pitch conversion.
+#include <algorithm>
+#include <cmath>
+#include <new>
+#include <vector>
+
+#include "bfl_common.cuh"
+
+using namespace bfl;
+
+namespace {
+
+constexpr float kLatentFloor = 1e-10f;   // plsi.cc:95
+constexpr int kColsumBlocks = 512;       // fixed partial count: the column sums do not depend on the device
+
+__device__ __forceinline__ void red4(float* p, float4 v) { atomicAdd(reinterpret_cast<float4*>(p), v); }
+
+__device__ __forceinline__ float4 ld4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
+
+// latent of one float4 slice starting at column col; columns >= d are padding and contribute nothing
+__device__ __forceinline__ float4 latent4(float4 p, float4 q, int col, int d) {
+    float4 l;
+    l.x = col + 0 < d ? fmaxf(p.x * q.x, kLatentFloor) : 0.f;
+    l.y = col + 1 < d ? fmaxf(p.y * q.y, kLatentFloor) : 0.f;
+    l.z = col + 2 < d ? fmaxf(p.z * q.z, kLatentFloor) : 0.f;
+    l.w = col + 3 < d ? fmaxf(p.w * q.w, kLatentFloor) : 0.f;
+    return l;
+}
+
+struct EmArgs {
+    float* P;                // [P_rows x vdim]: current rows in, new (unnormalised) rows out
+    const float* Q;          // [Q_rows x vdim] current item factors (read only during the pass)
+    float* Qacc;             // [Q_rows x vdim] new item factors, accumulated with atomics
+    uint8_t* visited;        // [P_rows] set for every row the pass writes
+    const int64_t* ends;     // ends[i] = end offset of row row_begin + i; ends[-1] is valid when row_begin > 0
+    const int32_t* keys;     // entry j at keys[j - shift]
+    const float* vals;
+    int64_t shift;
+    int64_t row_begin, n_rows;
+    double* loss;            // += -sum v * log(norm) (nullable)
+    int d, vdim;
+};
+
+// One warp per user row.  A row is split into float4 slices; G lanes (a group) cover one entry's slices, NV slices
+// per lane when a row has more than 32 slices, and the 32 / G groups of the warp take different entries.  Keys and
+// values are loaded 32 at a time, coalesced, and broadcast by shuffles; each group keeps U item rows in flight.
+template <int G, int NV, int U>
+__global__ void __launch_bounds__(256) plsi_em_kernel(const EmArgs a) {
+    constexpr int NG = 32 / G;
+    __shared__ double s_loss[8];
+    const int lane = threadIdx.x & 31, g = lane / G, gl = lane % G;
+    const int nv4 = a.vdim >> 2;
+    const int64_t warp0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    double lacc = 0.0;
+    for (int64_t i = warp0; i < a.n_rows; i += nwarps) {
+        const int64_t x = a.row_begin + i;
+        const int64_t beg = (x == 0) ? 0 : a.ends[i - 1];
+        const int64_t end = a.ends[i];
+        float* prow = a.P + x * a.vdim;
+        float4 p[NV], acc[NV];
+#pragma unroll
+        for (int k = 0; k < NV; ++k) {
+            const int s = gl + G * k;
+            p[k] = s < nv4 ? *reinterpret_cast<const float4*>(prow + 4 * s) : make_float4(0.f, 0.f, 0.f, 0.f);
+            acc[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+        for (int64_t base = beg; base < end; base += 32) {
+            const int cnt = (int)min((int64_t)32, end - base);
+            const int my_key = lane < cnt ? __ldg(a.keys + (base + lane - a.shift)) : 0;
+            const float my_val = lane < cnt ? __ldg(a.vals + (base + lane - a.shift)) : 0.f;
+            for (int t = 0; t < cnt; t += NG * U) {
+                int c[U];
+                float v[U];
+                bool ok[U];
+                float4 q[U][NV];
+#pragma unroll
+                for (int u = 0; u < U; ++u) {
+                    const int e = t + u * NG + g;
+                    ok[u] = e < cnt;
+                    c[u] = __shfl_sync(FULL, my_key, e & 31);
+                    v[u] = __shfl_sync(FULL, my_val, e & 31);
+#pragma unroll
+                    for (int k = 0; k < NV; ++k) {
+                        const int s = gl + G * k;
+                        q[u][k] = (ok[u] && s < nv4) ? ld4(a.Q + (int64_t)c[u] * a.vdim + 4 * s)
+                                                     : make_float4(0.f, 0.f, 0.f, 0.f);
+                    }
+                }
+#pragma unroll
+                for (int u = 0; u < U; ++u) {
+                    float4 l[NV];
+                    float ps = 0.f;
+#pragma unroll
+                    for (int k = 0; k < NV; ++k) {
+                        l[k] = latent4(p[k], q[u][k], 4 * (gl + G * k), a.d);
+                        ps += (l[k].x + l[k].y) + (l[k].z + l[k].w);
+                    }
+#pragma unroll
+                    for (int o = G / 2; o > 0; o >>= 1) ps += __shfl_xor_sync(FULL, ps, o);
+                    // lanes past the chunk's end add zeros to acc and skip the atomics
+                    const float w = ok[u] ? v[u] / ps : 0.f;
+                    if (ok[u] && gl == 0) lacc -= (double)v[u] * (double)logf(ps);
+                    float* qrow = a.Qacc + (int64_t)c[u] * a.vdim;
+#pragma unroll
+                    for (int k = 0; k < NV; ++k) {
+                        const int s = gl + G * k;
+                        const float4 ctb = make_float4(l[k].x * w, l[k].y * w, l[k].z * w, l[k].w * w);
+                        acc[k].x += ctb.x; acc[k].y += ctb.y; acc[k].z += ctb.z; acc[k].w += ctb.w;
+                        if (ok[u] && s < nv4) red4(qrow + 4 * s, ctb);
+                    }
+                }
+            }
+        }
+        // the groups of the warp hold partial sums of the same row: fold them into group 0
+#pragma unroll
+        for (int k = 0; k < NV; ++k) {
+#pragma unroll
+            for (int o = G; o < 32; o <<= 1) {
+                acc[k].x += __shfl_xor_sync(FULL, acc[k].x, o);
+                acc[k].y += __shfl_xor_sync(FULL, acc[k].y, o);
+                acc[k].z += __shfl_xor_sync(FULL, acc[k].z, o);
+                acc[k].w += __shfl_xor_sync(FULL, acc[k].w, o);
+            }
+            const int s = gl + G * k;
+            if (g == 0 && s < nv4) *reinterpret_cast<float4*>(prow + 4 * s) = acc[k];
+        }
+        if (lane == 0) a.visited[x] = 1;
+    }
+    if (a.loss) {
+        lacc = warp_sum_d(lacc);
+        if (lane == 0) s_loss[threadIdx.x >> 5] = lacc;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            double s = 0.0;
+            for (int w = 0; w < (int)(blockDim.x >> 5); ++w) s += s_loss[w];
+            if (s != 0.0) atomicAdd(a.loss, s);
+        }
+    }
+}
+
+// P rows: (row + alpha1) / sum(row + alpha1) over the d real columns (plsi.cc:115-119).  A row the last pass did not
+// write is the reference's zeroed accumulator row.  visited == null: every row is taken as it is.  G lanes per row.
+template <int G>
+__global__ void __launch_bounds__(256) plsi_normalize_rows_kernel(float* P, const uint8_t* visited, int64_t rows,
+                                                                  int d, int vdim, float alpha1) {
+    const int lane = threadIdx.x & 31, gl = lane % G;
+    const int nv4 = vdim >> 2;
+    const int64_t grp0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / G;
+    const int64_t ngrp = ((int64_t)gridDim.x * blockDim.x) / G;
+    const int64_t span = (rows + (32 / G) - 1) / (32 / G) * (32 / G);   // whole warps iterate together
+    for (int64_t x = grp0; x < span; x += ngrp) {
+        const bool live = x < rows;
+        const bool zero = live && visited && !visited[x];
+        float* row = P + (live ? x : 0) * vdim;
+        float ps = 0.f;
+        for (int s = gl; s < nv4; s += G) {
+            float4 v = (live && !zero) ? *reinterpret_cast<const float4*>(row + 4 * s) : make_float4(0.f, 0.f, 0.f, 0.f);
+            const int col = 4 * s;
+            ps += (col + 0 < d ? v.x + alpha1 : 0.f) + (col + 1 < d ? v.y + alpha1 : 0.f) +
+                  (col + 2 < d ? v.z + alpha1 : 0.f) + (col + 3 < d ? v.w + alpha1 : 0.f);
+        }
+#pragma unroll
+        for (int o = G / 2; o > 0; o >>= 1) ps += __shfl_xor_sync(FULL, ps, o);
+        if (!live) continue;
+        for (int s = gl; s < nv4; s += G) {
+            float4 v = zero ? make_float4(0.f, 0.f, 0.f, 0.f) : *reinterpret_cast<const float4*>(row + 4 * s);
+            const int col = 4 * s;
+            v.x = col + 0 < d ? (v.x + alpha1) / ps : 0.f;
+            v.y = col + 1 < d ? (v.y + alpha1) / ps : 0.f;
+            v.z = col + 2 < d ? (v.z + alpha1) / ps : 0.f;
+            v.w = col + 3 < d ? (v.w + alpha1) / ps : 0.f;
+            *reinterpret_cast<float4*>(row + 4 * s) = v;
+        }
+    }
+}
+
+// Q columns, stage 1: per-CTA fp64 partial column sums over a fixed contiguous item range.
+__global__ void __launch_bounds__(256) plsi_colsum_partial_kernel(const float* Q, int64_t rows, int vdim,
+                                                                  int64_t rows_per_blk, double* part) {
+    __shared__ double s_part[1024];
+    const int nv4 = vdim >> 2;
+    const int par = blockDim.x / nv4;             // rows summed side by side
+    const int r = threadIdx.x / nv4, s = threadIdx.x % nv4;
+    const int64_t lo = (int64_t)blockIdx.x * rows_per_blk, hi = min(rows, lo + rows_per_blk);
+    double a0 = 0.0, a1 = 0.0, a2 = 0.0, a3 = 0.0;
+    if (r < par) {
+        for (int64_t i = lo + r; i < hi; i += par) {
+            const float4 v = *reinterpret_cast<const float4*>(Q + i * vdim + 4 * s);
+            a0 += v.x; a1 += v.y; a2 += v.z; a3 += v.w;
+        }
+        double* dst = s_part + r * vdim + 4 * s;
+        dst[0] = a0; dst[1] = a1; dst[2] = a2; dst[3] = a3;
+    }
+    __syncthreads();
+    for (int k = threadIdx.x; k < vdim; k += blockDim.x) {
+        double t = 0.0;
+        for (int j = 0; j < par; ++j) t += s_part[j * vdim + k];
+        part[(int64_t)blockIdx.x * vdim + k] = t;
+    }
+}
+
+// Q columns, stage 2: the partials in block order, plus rows * alpha2 (the reference adds alpha2 to every entry).
+__global__ void plsi_colsum_final_kernel(const double* part, int nblk, int vdim, int64_t rows, float alpha2,
+                                         double* colsum) {
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= vdim) return;
+    double t = 0.0;
+    for (int b = 0; b < nblk; ++b) t += part[(int64_t)b * vdim + k];
+    colsum[k] = t + (double)rows * (double)alpha2;
+}
+
+// Q columns, stage 3: (q + alpha2) / column sum (plsi.cc:120-124); padding columns stay zero.
+__global__ void __launch_bounds__(256) plsi_scale_cols_kernel(float* Q, int64_t rows, int d, int vdim, float alpha2,
+                                                              const double* colsum) {
+    const int nv4 = vdim >> 2;
+    const int64_t n = rows * nv4;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x) {
+        const int s = (int)(e % nv4);
+        const int col = 4 * s;
+        float4* p = reinterpret_cast<float4*>(Q) + e;
+        float4 v = *p;
+        v.x = col + 0 < d ? (float)((double)(v.x + alpha2) / colsum[col + 0]) : 0.f;
+        v.y = col + 1 < d ? (float)((double)(v.y + alpha2) / colsum[col + 1]) : 0.f;
+        v.z = col + 2 < d ? (float)((double)(v.z + alpha2) / colsum[col + 2]) : 0.f;
+        v.w = col + 3 < d ? (float)((double)(v.w + alpha2) / colsum[col + 3]) : 0.f;
+        *p = v;
+    }
+}
+
+// |N(0, 1/d)| per real column (plsi.cc:51-64), from Philox4x32-10 keyed by (seed, matrix, element): Box-Muller on
+// the first two words.  Padding columns are zero.
+__global__ void __launch_bounds__(256) plsi_init_kernel(float* F, int64_t rows, int d, int vdim, uint32_t seed,
+                                                        uint32_t matrix) {
+    const int64_t n = rows * vdim;
+    const float sd = 1.0f / (float)d;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t r = e / vdim;
+        const int col = (int)(e % vdim);
+        float v = 0.f;
+        if (col < d) {
+            const uint64_t idx = (uint64_t)r * (uint64_t)d + (uint64_t)col;
+            uint32_t o[4];
+            philox4x32_10((uint32_t)idx, (uint32_t)(idx >> 32), matrix, 0x504C5349u, seed, 0x5EEDu, o);
+            const float u1 = ((float)(o[0] >> 8) + 1.0f) * (1.0f / 16777216.0f);   // (0, 1]
+            const float u2 = (float)(o[1] >> 8) * (1.0f / 16777216.0f);
+            v = fabsf(sqrtf(-2.0f * logf(u1)) * cospif(2.0f * u2)) * sd;
+        }
+        F[e] = v;
+    }
+}
+
+}  // namespace
+
+struct bfl_plsi {
+    bool opt_set = false;
+    int d = 0, vdim = 0;
+    uint32_t seed = 0;
+
+    float *hostP = nullptr, *hostQ = nullptr;   // caller's [rows x d] arrays (holder path)
+    DevBuf<float> ownP, ownQ;                   // holder path: the library's device copies
+    DevBuf<float> Qacc;                         // new item factors of the running iteration
+    float *dP = nullptr, *dQ = nullptr;
+    int64_t P_rows = 0, Q_rows = 0;
+    bool factors_ready = false;
+    DevBuf<uint8_t> visited;
+    DevBuf<double> colpart, colsum, d_loss;
+
+    DevBuf<int64_t> stage_ends;
+    DevBuf<int32_t> stage_keys;
+    DevBuf<float> stage_vals;
+    const int64_t* d_indptr = nullptr;
+    const int32_t* d_keys = nullptr;
+    const float* d_vals = nullptr;
+    int64_t csr_rows = 0, csr_nnz = 0;
+
+    cudaStream_t stream = nullptr;
+    int num_sms = 132;
+};
+
+namespace {
+
+int plsi_apply_options(bfl_plsi* h, const JsonOpt& j) {
+    h->d = j.integer("d", 20);
+    if (h->d <= 0 || h->d > 512) BFL_FAIL(BFL_ERR_OPTION, "d must be in [1, 512]");
+    h->vdim = (h->d + 3) / 4 * 4;
+    h->seed = (uint32_t)j.integer("random_seed", 0);
+    if (BFL_OK != require_device()) return BFL_ERR_CUDA;
+    int dev = 0;
+    BFL_CUDA(cudaGetDevice(&dev));
+    BFL_CUDA(cudaDeviceGetAttribute(&h->num_sms, cudaDevAttrMultiProcessorCount, dev));
+    if (!h->stream) BFL_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
+    if (BFL_OK != h->d_loss.reserve(1)) return BFL_ERR_CUDA;
+    h->opt_set = true;
+    return BFL_OK;
+}
+
+int grid_for(const bfl_plsi* h, int64_t work, int per_block, int blocks_per_sm) {
+    return (int)std::max<int64_t>(1, std::min<int64_t>((work + per_block - 1) / per_block,
+                                                       (int64_t)h->num_sms * blocks_per_sm));
+}
+
+// zero the accumulator and the row flags (plsi.cc:40-42)
+int reset_acc(bfl_plsi* h, cudaStream_t st) {
+    BFL_CUDA(cudaMemsetAsync(h->Qacc.p, 0, sizeof(float) * (size_t)h->Q_rows * h->vdim, st));
+    BFL_CUDA(cudaMemsetAsync(h->visited.p, 0, (size_t)h->P_rows, st));
+    return BFL_OK;
+}
+
+int alloc_state(bfl_plsi* h) {
+    if (BFL_OK != h->Qacc.reserve((size_t)h->Q_rows * h->vdim)) return BFL_ERR_CUDA;
+    if (BFL_OK != h->visited.reserve((size_t)h->P_rows)) return BFL_ERR_CUDA;
+    if (BFL_OK != h->colpart.reserve((size_t)kColsumBlocks * h->vdim)) return BFL_ERR_CUDA;
+    if (BFL_OK != h->colsum.reserve((size_t)h->vdim)) return BFL_ERR_CUDA;
+    return reset_acc(h, h->stream);
+}
+
+int launch_em(bfl_plsi* h, const EmArgs& a, cudaStream_t st) {
+    if (a.n_rows <= 0) return BFL_OK;
+    const int grid = grid_for(h, a.n_rows, 8, 16);
+    const int nv4 = h->vdim / 4;
+    if (nv4 <= 1) plsi_em_kernel<1, 1, 2><<<grid, 256, 0, st>>>(a);
+    else if (nv4 <= 2) plsi_em_kernel<2, 1, 2><<<grid, 256, 0, st>>>(a);
+    else if (nv4 <= 4) plsi_em_kernel<4, 1, 2><<<grid, 256, 0, st>>>(a);
+    else if (nv4 <= 8) plsi_em_kernel<8, 1, 2><<<grid, 256, 0, st>>>(a);
+    else if (nv4 <= 16) plsi_em_kernel<16, 1, 4><<<grid, 256, 0, st>>>(a);
+    else if (nv4 <= 32) plsi_em_kernel<32, 1, 4><<<grid, 256, 0, st>>>(a);
+    else if (nv4 <= 64) plsi_em_kernel<32, 2, 4><<<grid, 256, 0, st>>>(a);
+    else plsi_em_kernel<32, 4, 2><<<grid, 256, 0, st>>>(a);
+    BFL_LAUNCHED();
+    return BFL_OK;
+}
+
+int normalize_rows(bfl_plsi* h, float* P, const uint8_t* visited, float alpha1, cudaStream_t st) {
+    const int nv4 = h->vdim / 4;
+    const int G = nv4 <= 1 ? 1 : nv4 <= 2 ? 2 : nv4 <= 4 ? 4 : nv4 <= 8 ? 8 : nv4 <= 16 ? 16 : 32;
+    const int grid = grid_for(h, h->P_rows, 256 / G, 32);
+    switch (G) {
+        case 1: plsi_normalize_rows_kernel<1><<<grid, 256, 0, st>>>(P, visited, h->P_rows, h->d, h->vdim, alpha1); break;
+        case 2: plsi_normalize_rows_kernel<2><<<grid, 256, 0, st>>>(P, visited, h->P_rows, h->d, h->vdim, alpha1); break;
+        case 4: plsi_normalize_rows_kernel<4><<<grid, 256, 0, st>>>(P, visited, h->P_rows, h->d, h->vdim, alpha1); break;
+        case 8: plsi_normalize_rows_kernel<8><<<grid, 256, 0, st>>>(P, visited, h->P_rows, h->d, h->vdim, alpha1); break;
+        case 16: plsi_normalize_rows_kernel<16><<<grid, 256, 0, st>>>(P, visited, h->P_rows, h->d, h->vdim, alpha1); break;
+        default: plsi_normalize_rows_kernel<32><<<grid, 256, 0, st>>>(P, visited, h->P_rows, h->d, h->vdim, alpha1); break;
+    }
+    BFL_LAUNCHED();
+    return BFL_OK;
+}
+
+int normalize_cols(bfl_plsi* h, float* Q, float alpha2, cudaStream_t st) {
+    const int64_t rpb = std::max<int64_t>(1, (h->Q_rows + kColsumBlocks - 1) / kColsumBlocks);
+    const int nblk = (int)((h->Q_rows + rpb - 1) / rpb);
+    plsi_colsum_partial_kernel<<<nblk, 256, 0, st>>>(Q, h->Q_rows, h->vdim, rpb, h->colpart.p);
+    BFL_LAUNCHED();
+    plsi_colsum_final_kernel<<<(h->vdim + 127) / 128, 128, 0, st>>>(h->colpart.p, nblk, h->vdim, h->Q_rows, alpha2,
+                                                                     h->colsum.p);
+    BFL_LAUNCHED();
+    plsi_scale_cols_kernel<<<grid_for(h, h->Q_rows * (h->vdim / 4), 256, 16), 256, 0, st>>>(Q, h->Q_rows, h->d, h->vdim,
+                                                                                           alpha2, h->colsum.p);
+    BFL_LAUNCHED();
+    return BFL_OK;
+}
+
+// plsi.cc:108-125: alpha1 /= d, alpha2 /= num_items (in float, as the reference)
+int normalize_all(bfl_plsi* h, float alpha1, float alpha2, cudaStream_t st) {
+    const float a1 = alpha1 / (float)h->d, a2 = alpha2 / (float)h->Q_rows;
+    int rc = normalize_rows(h, h->dP, h->visited.p, a1, st);
+    if (rc != BFL_OK) return rc;
+    return normalize_cols(h, h->Qacc.p, a2, st);
+}
+
+int copy_rows(float* dst, size_t dpitch, const float* src, size_t spitch, int64_t rows, int d, cudaMemcpyKind kind,
+              cudaStream_t st) {
+    if (rows <= 0) return BFL_OK;
+    BFL_CUDA(cudaMemcpy2DAsync(dst, dpitch * sizeof(float), src, spitch * sizeof(float), sizeof(float) * d, (size_t)rows,
+                               kind, st));
+    return BFL_OK;
+}
+
+// holder path: device copies of the caller's [rows x d] arrays, padding columns zeroed
+int adopt_host(bfl_plsi* h, float* P, int32_t P_rows, float* Q, int32_t Q_rows) {
+    if (!h || !h->opt_set) BFL_FAIL(BFL_ERR_STATE, "init() must succeed before initialize_model()");
+    if (!P || !Q || P_rows <= 0 || Q_rows <= 0) BFL_FAIL(BFL_ERR_ARG, "bad factor arguments");
+    h->hostP = P; h->hostQ = Q;
+    h->P_rows = P_rows; h->Q_rows = Q_rows;
+    if (BFL_OK != h->ownP.reserve((size_t)P_rows * h->vdim)) return BFL_ERR_CUDA;
+    if (BFL_OK != h->ownQ.reserve((size_t)Q_rows * h->vdim)) return BFL_ERR_CUDA;
+    h->dP = h->ownP.p; h->dQ = h->ownQ.p;
+    h->factors_ready = false;
+    return alloc_state(h);
+}
+
+int download(bfl_plsi* h) {
+    int rc = copy_rows(h->hostP, h->d, h->dP, h->vdim, h->P_rows, h->d, cudaMemcpyDeviceToHost, h->stream);
+    if (rc != BFL_OK) return rc;
+    rc = copy_rows(h->hostQ, h->d, h->dQ, h->vdim, h->Q_rows, h->d, cudaMemcpyDeviceToHost, h->stream);
+    if (rc != BFL_OK) return rc;
+    BFL_CUDA(cudaStreamSynchronize(h->stream));
+    return BFL_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+bfl_plsi_t* bfl_plsi_create(void) { return new (std::nothrow) bfl_plsi(); }
+
+void bfl_plsi_destroy(bfl_plsi_t* h) {
+    if (!h) return;
+    if (h->stream) cudaStreamDestroy(h->stream);
+    delete h;
+}
+
+int bfl_plsi_init(bfl_plsi_t* h, const char* opt_path) {
+    if (!h || !opt_path) BFL_FAIL(BFL_ERR_ARG, "null argument");
+    JsonOpt j;
+    std::string err;
+    if (!j.load(opt_path, &err)) BFL_FAIL(BFL_ERR_OPTION, err);
+    return plsi_apply_options(h, j);
+}
+
+int bfl_plsi_init_json(bfl_plsi_t* h, const char* json_text) {
+    if (!h || !json_text) BFL_FAIL(BFL_ERR_ARG, "null argument");
+    JsonOpt j;
+    std::string err;
+    if (!j.parse(json_text, &err)) BFL_FAIL(BFL_ERR_OPTION, "Failed to parse: " + err);
+    return plsi_apply_options(h, j);
+}
+
+int bfl_plsi_get_vdim(bfl_plsi_t* h) { return h ? h->vdim : 0; }
+
+int bfl_plsi_initialize_model(bfl_plsi_t* h, float* P, int32_t P_rows, float* Q, int32_t Q_rows) {
+    int rc = adopt_host(h, P, P_rows, Q, Q_rows);
+    if (rc != BFL_OK) return rc;
+    cudaStream_t st = h->stream;
+    plsi_init_kernel<<<grid_for(h, (int64_t)P_rows * h->vdim, 256, 16), 256, 0, st>>>(h->dP, P_rows, h->d, h->vdim,
+                                                                                      h->seed, 0u);
+    BFL_LAUNCHED();
+    plsi_init_kernel<<<grid_for(h, (int64_t)Q_rows * h->vdim, 256, 16), 256, 0, st>>>(h->dQ, Q_rows, h->d, h->vdim,
+                                                                                      h->seed, 1u);
+    BFL_LAUNCHED();
+    if (BFL_OK != (rc = normalize_rows(h, h->dP, nullptr, 0.f, st))) return rc;
+    if (BFL_OK != (rc = normalize_cols(h, h->dQ, 0.f, st))) return rc;
+    if (BFL_OK != (rc = download(h))) return rc;
+    h->factors_ready = true;
+    return BFL_OK;
+}
+
+int bfl_plsi_set_model(bfl_plsi_t* h, float* P, int32_t P_rows, float* Q, int32_t Q_rows) {
+    int rc = adopt_host(h, P, P_rows, Q, Q_rows);
+    if (rc != BFL_OK) return rc;
+    cudaStream_t st = h->stream;
+    BFL_CUDA(cudaMemsetAsync(h->dP, 0, sizeof(float) * (size_t)P_rows * h->vdim, st));
+    BFL_CUDA(cudaMemsetAsync(h->dQ, 0, sizeof(float) * (size_t)Q_rows * h->vdim, st));
+    if (BFL_OK != (rc = copy_rows(h->dP, h->vdim, P, h->d, P_rows, h->d, cudaMemcpyHostToDevice, st))) return rc;
+    if (BFL_OK != (rc = copy_rows(h->dQ, h->vdim, Q, h->d, Q_rows, h->d, cudaMemcpyHostToDevice, st))) return rc;
+    BFL_CUDA(cudaStreamSynchronize(st));
+    h->factors_ready = true;
+    return BFL_OK;
+}
+
+int bfl_plsi_reset(bfl_plsi_t* h) {
+    if (!h || !h->factors_ready) BFL_FAIL(BFL_ERR_STATE, "initialize_model() must precede reset()");
+    int rc = reset_acc(h, h->stream);
+    if (rc != BFL_OK) return rc;
+    BFL_CUDA(cudaStreamSynchronize(h->stream));
+    return BFL_OK;
+}
+
+int bfl_plsi_partial_update(bfl_plsi_t* h, int32_t start_x, int32_t next_x, const int64_t* indptr,
+                            const int32_t* keys, const float* vals, double* loss) {
+    if (loss) *loss = 0.0;
+    if (!h || !h->factors_ready || !h->hostP) BFL_FAIL(BFL_ERR_STATE, "initialize_model() must precede partial_update()");
+    if (next_x == start_x) return BFL_OK;
+    if (start_x < 0 || next_x > h->P_rows || next_x < start_x || !indptr) BFL_FAIL(BFL_ERR_ARG, "bad chunk arguments");
+    const int64_t beg = start_x == 0 ? 0 : indptr[start_x - 1];
+    const int64_t n = indptr[next_x - 1] - beg;
+    if (n > 0 && (!keys || !vals)) BFL_FAIL(BFL_ERR_ARG, "null keys / vals");
+    cudaStream_t st = h->stream;
+    // the chunk's end offsets, preceded by the previous row's end when start_x > 0
+    const int64_t lead = start_x > 0 ? 1 : 0;
+    const int64_t n_ends = next_x - start_x + lead;
+    if (BFL_OK != h->stage_ends.reserve((size_t)n_ends)) return BFL_ERR_CUDA;
+    BFL_CUDA(cudaMemcpyAsync(h->stage_ends.p, indptr + start_x - lead, sizeof(int64_t) * n_ends, cudaMemcpyHostToDevice, st));
+    if (n > 0) {
+        if (BFL_OK != h->stage_keys.reserve((size_t)n)) return BFL_ERR_CUDA;
+        if (BFL_OK != h->stage_vals.reserve((size_t)n)) return BFL_ERR_CUDA;
+        BFL_CUDA(cudaMemcpyAsync(h->stage_keys.p, keys, sizeof(int32_t) * n, cudaMemcpyHostToDevice, st));
+        BFL_CUDA(cudaMemcpyAsync(h->stage_vals.p, vals, sizeof(float) * n, cudaMemcpyHostToDevice, st));
+    }
+    BFL_CUDA(cudaMemsetAsync(h->d_loss.p, 0, sizeof(double), st));
+    EmArgs a;
+    a.P = h->dP; a.Q = h->dQ; a.Qacc = h->Qacc.p; a.visited = h->visited.p;
+    a.ends = h->stage_ends.p + lead; a.keys = h->stage_keys.p; a.vals = h->stage_vals.p; a.shift = beg;
+    a.row_begin = start_x; a.n_rows = next_x - start_x; a.loss = h->d_loss.p; a.d = h->d; a.vdim = h->vdim;
+    int rc = launch_em(h, a, st);
+    if (rc != BFL_OK) return rc;
+    double out = 0.0;
+    BFL_CUDA(cudaMemcpyAsync(&out, h->d_loss.p, sizeof(double), cudaMemcpyDeviceToHost, st));
+    BFL_CUDA(cudaStreamSynchronize(st));   // the staging buffers are reused by the next chunk
+    if (loss) *loss = out;
+    return BFL_OK;
+}
+
+int bfl_plsi_normalize(bfl_plsi_t* h, float alpha1, float alpha2) {
+    if (!h || !h->factors_ready) BFL_FAIL(BFL_ERR_STATE, "initialize_model() must precede normalize()");
+    int rc = normalize_all(h, alpha1, alpha2, h->stream);
+    if (rc != BFL_OK) return rc;
+    BFL_CUDA(cudaStreamSynchronize(h->stream));
+    return BFL_OK;
+}
+
+int bfl_plsi_swap(bfl_plsi_t* h) {
+    if (!h || !h->factors_ready || !h->hostP) BFL_FAIL(BFL_ERR_STATE, "initialize_model() must precede swap()");
+    // the normalised accumulator becomes the current item matrix; the old one is the next accumulator
+    std::swap(h->ownQ.p, h->Qacc.p);
+    std::swap(h->ownQ.cap, h->Qacc.cap);
+    h->dQ = h->ownQ.p;
+    return download(h);
+}
+
+int bfl_plsi_release(bfl_plsi_t* h) {
+    if (!h) BFL_FAIL(BFL_ERR_ARG, "null handle");
+    if (h->stream) BFL_CUDA(cudaStreamSynchronize(h->stream));
+    h->ownP.release(); h->ownQ.release(); h->Qacc.release(); h->visited.release();
+    h->colpart.release(); h->colsum.release();
+    h->stage_ends.release(); h->stage_keys.release(); h->stage_vals.release();
+    h->hostP = h->hostQ = nullptr;
+    h->dP = h->dQ = nullptr;
+    h->P_rows = h->Q_rows = 0;
+    h->factors_ready = false;
+    return BFL_OK;
+}
+
+int bfl_plsi_bind_factors_device(bfl_plsi_t* h, float* dP, int64_t P_rows, float* dQ, int64_t Q_rows) {
+    if (!h || !h->opt_set) BFL_FAIL(BFL_ERR_STATE, "init() must succeed before binding factors");
+    if (!dP || !dQ || P_rows <= 0 || Q_rows <= 0) BFL_FAIL(BFL_ERR_ARG, "bad factor arguments");
+    if (((uintptr_t)dP | (uintptr_t)dQ) & 15) BFL_FAIL(BFL_ERR_ARG, "device factor pointers must be 16-byte aligned");
+    h->hostP = h->hostQ = nullptr;
+    h->ownP.release(); h->ownQ.release();
+    h->dP = dP; h->dQ = dQ;
+    h->P_rows = P_rows; h->Q_rows = Q_rows;
+    int rc = alloc_state(h);
+    if (rc != BFL_OK) return rc;
+    BFL_CUDA(cudaStreamSynchronize(h->stream));
+    h->factors_ready = true;
+    return BFL_OK;
+}
+
+int bfl_plsi_bind_csr_device(bfl_plsi_t* h, const int64_t* d_indptr, const int32_t* d_keys, const float* d_vals,
+                             int64_t rows, int64_t nnz) {
+    if (!h || !h->opt_set) BFL_FAIL(BFL_ERR_STATE, "init() must precede bind_csr");
+    if (!d_indptr || (nnz > 0 && (!d_keys || !d_vals)) || rows <= 0) BFL_FAIL(BFL_ERR_ARG, "bad CSR arguments");
+    h->d_indptr = d_indptr; h->d_keys = d_keys; h->d_vals = d_vals;
+    h->csr_rows = rows; h->csr_nnz = nnz;
+    return BFL_OK;
+}
+
+int bfl_plsi_update_device(bfl_plsi_t* h, int64_t row_begin, int64_t row_end, double* d_loss, void* stream) {
+    if (!h || !h->factors_ready) BFL_FAIL(BFL_ERR_STATE, "factors not bound");
+    if (!h->d_indptr) BFL_FAIL(BFL_ERR_STATE, "no device CSR bound");
+    if (h->csr_rows != h->P_rows) BFL_FAIL(BFL_ERR_STATE, "the bound CSR and P disagree on the number of rows");
+    if (row_begin < 0 || row_end > h->csr_rows || row_end < row_begin) BFL_FAIL(BFL_ERR_ARG, "bad row range");
+    EmArgs a;
+    a.P = h->dP; a.Q = h->dQ; a.Qacc = h->Qacc.p; a.visited = h->visited.p;
+    a.ends = h->d_indptr + row_begin; a.keys = h->d_keys; a.vals = h->d_vals; a.shift = 0;
+    a.row_begin = row_begin; a.n_rows = row_end - row_begin; a.loss = d_loss; a.d = h->d; a.vdim = h->vdim;
+    return launch_em(h, a, (cudaStream_t)stream);
+}
+
+int bfl_plsi_normalize_device(bfl_plsi_t* h, float alpha1, float alpha2, void* stream) {
+    if (!h || !h->factors_ready) BFL_FAIL(BFL_ERR_STATE, "factors not bound");
+    return normalize_all(h, alpha1, alpha2, (cudaStream_t)stream);
+}
+
+int bfl_plsi_swap_device(bfl_plsi_t* h, void* stream) {
+    if (!h || !h->factors_ready) BFL_FAIL(BFL_ERR_STATE, "factors not bound");
+    cudaStream_t st = (cudaStream_t)stream;
+    BFL_CUDA(cudaMemcpyAsync(h->dQ, h->Qacc.p, sizeof(float) * (size_t)h->Q_rows * h->vdim, cudaMemcpyDeviceToDevice, st));
+    return reset_acc(h, st);
+}
+
+}  // extern "C"

@@ -3,7 +3,7 @@
  *
  * This is the drop-in boundary: every entry point below replaces one method of the
  * reference's Cython holder classes (the `self.obj` object driven by
- * buffalo/algo/{als,bpr,warp}.py).  Plain pointers and sizes only -- no torch, numpy or
+ * buffalo/algo/{als,bpr,warp,plsi}.py).  Plain pointers and sizes only -- no torch, numpy or
  * C++ types cross the boundary.  INTEGRATION.md shows the ctypes / Cython stub a
  * reference maintainer would add to bind it.  All file:line citations are relative to
  * the reference repository root.
@@ -215,6 +215,59 @@ int bfl_sgd_set_trace_device(bfl_sgd_t* h, int32_t* d_trials, int32_t* d_negs);
 int bfl_sgd_epoch(bfl_sgd_t* h);
 double bfl_sgd_current_lr(bfl_sgd_t* h);
 int bfl_sgd_read_stats(bfl_sgd_t* h, double* loss_sum, int64_t* num_updates);
+
+/* ======================================================================================
+ * PLSI -- replaces CyPLSI (buffalo/algo/_plsi.pyx:13-57 -> plsi::CPLSI, lib/algo_impl/plsi/plsi.cc)
+ *
+ * One iteration is reset -> partial_update per rowwise chunk -> normalize -> swap (buffalo/algo/plsi.py:132-160).
+ * The new user rows are written over the current ones on the device as the pass goes (only a row's own update
+ * reads it); the new item rows accumulate in a library-owned matrix.  Each user row must be updated at most once
+ * between reset and normalize; a row the pass never reached counts as zero in normalize, like the reference's
+ * zeroed accumulator.  The holder path keeps its own device copy of the factors: changes the caller makes to the
+ * host arrays take effect through bfl_plsi_set_model.
+ * ====================================================================================== */
+typedef struct bfl_plsi bfl_plsi_t;
+
+/* CyPLSI.__cinit__ / __dealloc__ */
+bfl_plsi_t* bfl_plsi_create(void);
+void bfl_plsi_destroy(bfl_plsi_t* h);
+/* CPLSI::init(opt_path) (plsi.cc:21-30): d in [1, 512] (else BFL_ERR_OPTION), random_seed */
+int bfl_plsi_init(bfl_plsi_t* h, const char* opt_path);
+int bfl_plsi_init_json(bfl_plsi_t* h, const char* json_text);
+/* device row pitch of the factor matrices: ceil4(d) */
+int bfl_plsi_get_vdim(bfl_plsi_t* h);
+/* CPLSI::initialize_model(P, P_rows, Q, Q_rows) (plsi.cc:44-70).  HOST pointers, [rows x d] float32 (not padded),
+ * retained.  Fills them with |N(0, 1/d)| drawn on the device from Philox4x32-10 keyed by (random_seed, matrix,
+ * element), then divides every P row by its sum and every Q column by its sum. */
+int bfl_plsi_initialize_model(bfl_plsi_t* h, float* P, int32_t P_rows, float* Q, int32_t Q_rows);
+/* retain and upload the caller's current [rows x d] arrays without drawing (no reference counterpart: the
+ * reference reads the caller's arrays directly, so inherited or replaced factors need this here) */
+int bfl_plsi_set_model(bfl_plsi_t* h, float* P, int32_t P_rows, float* Q, int32_t Q_rows);
+/* CPLSI::reset (plsi.cc:40-42): zero the item accumulator and the record of updated rows */
+int bfl_plsi_reset(bfl_plsi_t* h);
+/* CPLSI::partial_update(start_x, next_x, indptr, keys, vals) (plsi.cc:72-106).  HOST buffers: `indptr` is the
+ * global end-offset array, `keys` / `vals` the chunk starting at row start_x.  *loss receives -sum v log(norm) of
+ * the chunk (fp64). */
+int bfl_plsi_partial_update(bfl_plsi_t* h, int32_t start_x, int32_t next_x, const int64_t* indptr,
+                            const int32_t* keys, const float* vals, double* loss);
+/* CPLSI::normalize(alpha1, alpha2) (plsi.cc:108-125): alpha1 /= d, alpha2 /= num_items, then every P row
+ * (+alpha1) and every Q column (+alpha2) is divided by its sum.  Column sums are fp64 and deterministic. */
+int bfl_plsi_normalize(bfl_plsi_t* h, float alpha1, float alpha2);
+/* CPLSI::swap (plsi.cc:127-130): the new factors become current and are copied into the retained host arrays */
+int bfl_plsi_swap(bfl_plsi_t* h);
+/* CPLSI::release (plsi.cc:36-38): free the device state */
+int bfl_plsi_release(bfl_plsi_t* h);
+
+/* ---- device-resident path: caller-owned DEVICE pointers, [rows x vdim] factors, work on `stream` ---- */
+int bfl_plsi_bind_factors_device(bfl_plsi_t* h, float* dP, int64_t P_rows, float* dQ, int64_t Q_rows);
+/* the rowwise CSR (rows == P_rows) */
+int bfl_plsi_bind_csr_device(bfl_plsi_t* h, const int64_t* d_indptr, const int32_t* d_keys, const float* d_vals,
+                             int64_t rows, int64_t nnz);
+/* update rows [row_begin, row_end); adds -sum v log(norm) into d_loss[0] (device double, may be NULL) */
+int bfl_plsi_update_device(bfl_plsi_t* h, int64_t row_begin, int64_t row_end, double* d_loss, void* stream);
+int bfl_plsi_normalize_device(bfl_plsi_t* h, float alpha1, float alpha2, void* stream);
+/* copy the new item factors into dQ and zero the accumulator for the next iteration (no separate reset) */
+int bfl_plsi_swap_device(bfl_plsi_t* h, void* stream);
 
 /* =====================================================================================
  * Evaluation top-k (SURVEY.md 8(f-2)); replaces the host quickselect behind Evaluable.get_topk /
