@@ -103,6 +103,17 @@ PROTOTYPES = {
     "bfl_csr_from_triples_host": (C.c_int, [_vp, _vp, _vp, _i64, _i32, _i32, C.c_int, _vp, _vp, _vp]),
     "bfl_popularity_table_device": (C.c_int, [_vp, _i64, _i32, C.c_int, _vp, _vp]),
     "bfl_popularity_table_host": (C.c_int, [_vp, _i64, _i32, C.c_int, _vp]),
+    # MatrixMarket ingest
+    "bfl_mm_ingest_create": (_vp, [_i32, _i32, _i64, _i64, _i64, _i64]),
+    "bfl_mm_ingest_destroy": (None, [_vp]),
+    "bfl_mm_ingest_staging": (C.c_int, [_vp, C.c_int, C.POINTER(_vp)]),
+    "bfl_mm_ingest_feed": (C.c_int, [_vp, C.c_int, _i64, C.c_int]),
+    "bfl_mm_ingest_finish": (C.c_int, [_vp, _pi64, C.POINTER(_i32), _pi64, _pi64, _pi64]),
+    "bfl_mm_ingest_slow_tokens": (C.c_int, [_vp, _i64, _vp, _vp, _vp]),
+    "bfl_mm_ingest_patch_values": (C.c_int, [_vp, _vp, _vp, _i64]),
+    "bfl_mm_ingest_split": (C.c_int, [_vp, _vp, _i64, _vp, _vp, _vp]),
+    "bfl_mm_ingest_build": (C.c_int, [_vp, C.c_int, _vp, _vp, _vp]),
+    "bfl_mm_ingest_stats": (C.c_int, [_vp, _pd, _pi64]),
 }
 
 

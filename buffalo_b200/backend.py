@@ -466,6 +466,92 @@ def csr_from_triples_host(major, minor, vals, num_major, num_minor, sort_minor=T
     return indptr, key[:n], val[:n]
 
 
+class MMIngest(object):
+    """Handle of the device MatrixMarket parser (csrc/mm_ingest.cu, bfl_mm_ingest_*): stream the text after the header
+    through two pinned staging buffers, then split and build both CSR orientations on the device."""
+
+    STAGES = ("h2d", "parse", "patch", "split", "csr_rowwise", "csr_colwise", "d2h")
+
+    def __init__(self, num_rows, num_cols, nnz_hint, block_bytes, header_lines, slow_cap):
+        self._lib = _cabi.lib()
+        self._h = self._lib.bfl_mm_ingest_create(int(num_rows), int(num_cols), int(nnz_hint), int(block_bytes),
+                                                 int(header_lines), int(slow_cap))
+        if not self._h:
+            raise _cabi.BackendError("bfl_mm_ingest_create failed: " +
+                                     self._lib.bfl_last_error().decode("utf-8", "replace"))
+        self.block_bytes = int(block_bytes)
+
+    def close(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            self._lib.bfl_mm_ingest_destroy(h)
+
+    __del__ = close
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def staging(self, slot):
+        """uint8 view of pinned staging buffer `slot`, free for writing (its previous upload has finished)."""
+        p = C.c_void_p()
+        _cabi.check(self._lib.bfl_mm_ingest_staging(self._h, int(slot), C.byref(p)), "bfl_mm_ingest_staging")
+        return np.ctypeslib.as_array((C.c_uint8 * self.block_bytes).from_address(p.value))
+
+    def feed(self, slot, n, is_last):
+        _cabi.check(self._lib.bfl_mm_ingest_feed(self._h, int(slot), int(n), int(bool(is_last))), "bfl_mm_ingest_feed")
+
+    def finish(self):
+        """-> dict(nnz, tokmask, reject_line, range_line, n_slow)"""
+        v = [C.c_int64(0), C.c_int32(0), C.c_int64(0), C.c_int64(0), C.c_int64(0)]
+        _cabi.check(self._lib.bfl_mm_ingest_finish(self._h, *[C.byref(x) for x in v]), "bfl_mm_ingest_finish")
+        return dict(zip(("nnz", "tokmask", "reject_line", "range_line", "n_slow"), [x.value for x in v]))
+
+    def slow_tokens(self, n):
+        """-> (ordinal int64, offset from the first fed byte int64, length int32) of n slow value tokens"""
+        o, off, ln = np.empty(n, np.int64), np.empty(n, np.int64), np.empty(n, np.int32)
+        _cabi.check(self._lib.bfl_mm_ingest_slow_tokens(self._h, int(n), o.ctypes.data, off.ctypes.data, ln.ctypes.data),
+                    "bfl_mm_ingest_slow_tokens")
+        return o, off, ln
+
+    def patch_values(self, ordinal, vals):
+        o = np.ascontiguousarray(ordinal, dtype=np.int64)
+        v = np.ascontiguousarray(vals, dtype=np.float32)
+        _cabi.check(self._lib.bfl_mm_ingest_patch_values(self._h, o.ctypes.data, v.ctypes.data, len(o)),
+                    "bfl_mm_ingest_patch_values")
+
+    def split(self, sample_idx):
+        """-> (row int32, col int32, val float32) of the sampled data-line ordinals (strictly increasing)"""
+        idx = np.ascontiguousarray(sample_idx, dtype=np.int64)
+        n = len(idx)
+        r, c, v = np.empty(n, np.int32), np.empty(n, np.int32), np.empty(n, np.float32)
+        _cabi.check(self._lib.bfl_mm_ingest_split(self._h, idx.ctypes.data, n, r.ctypes.data, c.ctypes.data,
+                                                  v.ctypes.data), "bfl_mm_ingest_split")
+        return r, c, v
+
+    def build(self, orientation, num_major, nnz):
+        """-> (indptr int64[num_major] END offsets, key int32[nnz], val float32[nnz]); 0 = rowwise, 1 = colwise"""
+        indptr = np.empty(int(num_major), np.int64)
+        key, val = np.empty(max(nnz, 1), np.int32), np.empty(max(nnz, 1), np.float32)
+        _cabi.check(self._lib.bfl_mm_ingest_build(self._h, int(orientation), indptr.ctypes.data, key.ctypes.data,
+                                                  val.ctypes.data), "bfl_mm_ingest_build")
+        return indptr, key[:nnz], val[:nnz]
+
+    def stats(self):
+        """-> ({stage: device ms}, peak device bytes of the default memory pool)"""
+        ms, peak = (C.c_double * len(self.STAGES))(), C.c_int64(0)
+        _cabi.check(self._lib.bfl_mm_ingest_stats(self._h, ms, C.byref(peak)), "bfl_mm_ingest_stats")
+        return dict(zip(self.STAGES, list(ms))), peak.value
+
+
+def device_free_bytes():
+    """Free device memory of the current device (cudaMemGetInfo)."""
+    import torch
+    return int(torch.cuda.mem_get_info()[0])
+
+
 def popularity_table_host(keys, n_items, power):
     """int64 cumulative table of count(item)**power (bpr.py:99-111) built on the device."""
     k = np.ascontiguousarray(keys, dtype=np.int32)

@@ -45,6 +45,9 @@ extern std::atomic<long long> g_launches;
 
 int require_device();  // BFL_OK iff a CUDA device of compute capability 10.x is current
 
+// out[i] = in[0] + ... + in[i] on `st` (in == out allowed); ingest.cu
+int inclusive_scan_i64(const long long* in, long long* out, long long n, cudaStream_t st);
+
 // ---------------------------------------------------------------------------------------
 // minimal JSON reader for the option file (the reference uses json11, lib/algo.cc:19-37).
 // Flat access to top-level scalars; nested objects/arrays are skipped.

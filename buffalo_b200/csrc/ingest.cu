@@ -72,6 +72,10 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_add_kernel(long long* __res
         if (base + i < n) out[base + i] += add;
 }
 
+}  // namespace
+
+namespace bfl {
+
 // out[i] = in[0] + ... + in[i]; in == out allowed; recursion over the tile sums
 int inclusive_scan_i64(const long long* in, long long* out, long long n, cudaStream_t st) {
     if (n <= 0) return BFL_OK;
@@ -89,6 +93,10 @@ int inclusive_scan_i64(const long long* in, long long* out, long long n, cudaStr
     BFL_CUDA(cudaFreeAsync(sums, st));
     return BFL_OK;
 }
+
+}  // namespace bfl
+
+namespace {
 
 // ---- histograms ----------------------------------------------------------------------------------
 __global__ void hist_i32_kernel(const int32_t* __restrict__ idx, long long n, long long* __restrict__ counts, int32_t nbins) {

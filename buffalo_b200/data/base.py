@@ -152,18 +152,28 @@ class Data(object):
 
     # ---- build side ----------------------------------------------------------------------------
     def _write_database(self, path, num_users, num_items, rows, cols, vals, uids, iids, vali,
-                        groups=("rowwise", "colwise"), keep_order=False):
-        """rows/cols: zero-based int arrays of the TRAINING entries; vali: None or dict(method, n, row, col, val)."""
+                        groups=("rowwise", "colwise"), keep_order=False, csr=None):
+        """rows/cols: zero-based int arrays of the TRAINING entries; vali: None or dict(method, n, row, col, val).
+        csr: None, or {group: (indptr, key, val)} already built from the training entries with raw values (the device
+        MatrixMarket parser); rows/cols/vals are then unused.  value_prepro is element-wise or uses the global min/max,
+        so applying it to each orientation's sorted values gives the bits of applying it before the sort."""
         if os.path.exists(path):
             self.logger.info(f"File {path} exists. To build new database, existing file {path} will be deleted.")
             os.remove(path)
         f = store.File(path, "w")
         self.path = path
-        vals = np.asarray(self.value_prepro(np.asarray(vals, dtype=np.float32).copy()), dtype=np.float32)
+        if csr is None:
+            vals = np.asarray(self.value_prepro(np.asarray(vals, dtype=np.float32).copy()), dtype=np.float32)
+            num_nnz = len(rows)
+        else:
+            num_nnz = len(csr["rowwise"][1])
         self.prepro.pre(f)
         for g, major, minor, nmajor in (("rowwise", rows, cols, num_users), ("colwise", cols, rows, num_items)):
             grp = f.create_group(g)
-            if g in groups:
+            if g in groups and csr is not None:
+                indptr, key, val = csr[g]
+                val = np.asarray(self.value_prepro(np.asarray(val, dtype=np.float32)), dtype=np.float32)
+            elif g in groups:
                 indptr, key, val = csr_from_triples(major, minor, vals, nmajor, stable_sort=not keep_order)
             else:
                 indptr, key, val = np.zeros(nmajor, np.int64), np.zeros(0, np.int32), np.zeros(0, np.float32)
@@ -190,7 +200,7 @@ class Data(object):
                 raise TypeError("id list for %s has %d entries, %d expected" % (name, len(ids), n))
             enc = [str(s).encode("utf-8") for s in ids]
             idmap.create_dataset(name, data=np.array(enc, dtype="S%d" % (max([len(e) for e in enc] + [1]) + 1)))
-        f.attrs.update(num_users=int(num_users), num_items=int(num_items), num_nnz=int(len(rows)), completed=1)
+        f.attrs.update(num_users=int(num_users), num_items=int(num_items), num_nnz=int(num_nnz), completed=1)
         f.close()
         self.handle = store.File(path, "r")
 

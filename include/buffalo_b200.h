@@ -302,6 +302,46 @@ int bfl_popularity_table_device(const int32_t* d_keys, int64_t nnz, int32_t n_it
                                 void* stream);
 int bfl_popularity_table_host(const int32_t* keys, int64_t nnz, int32_t n_items, int power, int64_t* cum);
 
+/* =====================================================================================
+ * MatrixMarket text -> database on the device (SURVEY.md 8(f-1); DESIGN.md 4.6).  The caller parses the header
+ * (banner, leading '%' lines, "U I nnz") and streams the rest of the file through the handle's two pinned staging
+ * buffers; the triples stay on the device through the validation split and both CSR builds.
+ *  - create: `nnz_hint` (the header's nnz) sizes the triple arrays; a file with more data lines than that reports
+ *    nnz > nnz_hint from finish and cannot be split.  `block_bytes` is the size of each staging buffer,
+ *    `header_lines` the number of lines before the first fed byte (for 1-based line numbers), `slow_cap` the number
+ *    of value tokens the handle can leave to the host parser.
+ *  - staging(slot): the pinned buffer of slot 0 or 1; waits until that buffer's previous upload has finished.
+ *  - feed(slot, n, is_last): uploads n bytes of the slot and parses them, asynchronously.  The CALLER carries partial
+ *    lines: a block that is not the last must end with '\n' (the bytes after the block's last '\n' start the next
+ *    block).  Lines longer than BFL_MM_MAX_LINE bytes (line end excluded) are grammar rejections.
+ *  - finish: waits for the parse; *nnz = data lines, *tokmask bit k set when some data line has k tokens,
+ *    *reject_line / *range_line = smallest 1-based file line the grammar rejected / with an index outside
+ *    [1, U] x [1, I] (-1: none), *n_slow = value tokens outside the exact fast path (compare with slow_cap).
+ *  - slow_tokens: their data-line ordinals, byte offsets from the first fed byte and lengths (any order);
+ *    patch_values writes the host-parsed values at those ordinals.
+ *  - split(sample_idx, n, ...): strictly increasing data-line ordinals move to the host vali arrays, the others keep
+ *    their order (n = 0 allowed, required before build).
+ *  - build(orientation 0 = rowwise, 1 = colwise): one CSR (exclusive END offsets) into host arrays of num_rows
+ *    resp. num_cols and nnz - n entries; each orientation once.
+ *  - stats: summed device time of H2D, parse, patch, split, rowwise CSR, colwise CSR and D2H (stage_ms[7]) and the
+ *    high-water mark of the device's default memory pool since create.
+ * ===================================================================================== */
+#define BFL_MM_MAX_LINE 1024
+typedef struct bfl_mm_ingest bfl_mm_ingest_t;
+bfl_mm_ingest_t* bfl_mm_ingest_create(int32_t num_rows, int32_t num_cols, int64_t nnz_hint, int64_t block_bytes,
+                                      int64_t header_lines, int64_t slow_cap);
+void bfl_mm_ingest_destroy(bfl_mm_ingest_t* h);
+int bfl_mm_ingest_staging(bfl_mm_ingest_t* h, int slot, void** host_ptr);
+int bfl_mm_ingest_feed(bfl_mm_ingest_t* h, int slot, int64_t n, int is_last);
+int bfl_mm_ingest_finish(bfl_mm_ingest_t* h, int64_t* nnz, int32_t* tokmask, int64_t* reject_line, int64_t* range_line,
+                         int64_t* n_slow);
+int bfl_mm_ingest_slow_tokens(bfl_mm_ingest_t* h, int64_t n, int64_t* ordinal, int64_t* offset, int32_t* length);
+int bfl_mm_ingest_patch_values(bfl_mm_ingest_t* h, const int64_t* ordinal, const float* val, int64_t n);
+int bfl_mm_ingest_split(bfl_mm_ingest_t* h, const int64_t* sample_idx, int64_t n, int32_t* out_row, int32_t* out_col,
+                        float* out_val);
+int bfl_mm_ingest_build(bfl_mm_ingest_t* h, int orientation, int64_t* indptr, int32_t* key, float* val);
+int bfl_mm_ingest_stats(bfl_mm_ingest_t* h, double* stage_ms, int64_t* peak_bytes);
+
 #ifdef __cplusplus
 }
 #endif
