@@ -5,8 +5,10 @@
 //           completion by cp.async.mbarrier.arrive.noinc
 //   mode 2: plain 128-bit loads into registers + st.shared (the synchronous baseline)
 // P producer warps share the ring (stage s belongs to warp s % P); one consumer warp releases a stage as soon as it is
-// full.  Persistent grid of one CTA per SM.  Prints GB/s per configuration.
+// full, so a configuration keeps up to `stages` tiles in flight per SM.  Persistent grid of one CTA per SM.  Prints
+// GB/s per configuration.
 //   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o gather_probe gather_probe.cu
+//   ./gather_probe [rows of Y, default 1e7] [mode, default all]
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -104,6 +106,7 @@ __global__ void __launch_bounds__(32 * (MAXP + 1), 1) probe(const float* __restr
 
 int main(int argc, char** argv) {
     const size_t rows = argc > 1 ? (size_t)atoll(argv[1]) : 10000000;
+    const int only_mode = argc > 2 ? atoi(argv[2]) : -1;   // -1: every mode
     int grid = 0, clk_khz = 0;
     CK(cudaDeviceGetAttribute(&grid, cudaDevAttrMultiProcessorCount, 0));
     CK(cudaDeviceGetAttribute(&clk_khz, cudaDevAttrClockRate, 0));
@@ -123,9 +126,9 @@ int main(int argc, char** argv) {
     cudaEventCreate(&e0); cudaEventCreate(&e1);
     const double bytes = (double)grid * tiles * TILE * ROWF * 4;
     for (int mode = 0; mode < 3; ++mode)
-        for (int NS : {4, 8, 12})
+        for (int NS : {2, 4, 6, 8, 12})
             for (int P : {1, 2, 4, 8}) {
-                if (P > NS) continue;
+                if (P > NS || (only_mode >= 0 && mode != only_mode)) continue;
                 const size_t smem = (size_t)NS * TILE * RAWP * 4 + 2 * NS * 8;
                 auto launch = [&]() {
                     if (mode == 0) { CK(cudaFuncSetAttribute(probe<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); probe<0><<<grid, 32 * (MAXP + 1), smem>>>(Y, dk, tiles, P, NS, sink); }

@@ -30,10 +30,12 @@
 //                     core matrices, conflict-free); accumulates b_m = sum w q_m (exact fp32) and the loss pieces in
 //                     registers; groups of two full tiles take a branch-free straight-line path;
 //   MMA warpgroup    : executes the generic -> async proxy fence for the group it has acquired, then issues wgmma
-//                     m64n128k16 (SASS HGMMA) for the two 64-row halves of the row's matrix, accumulating in registers
-//                     (128 fp32 per thread); entries with negative weight travel in their own tiles and are subtracted
-//                     with the negate-A immediate.  At a row's end it waits for the MMAs, stores 2^-2e x accumulator
-//                     into the shared-memory matrix of the epilogue and reloads 2^2e (G + reg I) for the next row;
+//                     (SASS HGMMA) for the two 64-row halves of the row's matrix, accumulating in registers: rows 64..127
+//                     over all 128 columns (m64n128k16), rows 0..63 only over columns 0..63 (m64n64k16; the matrix is
+//                     symmetric -- split-row chunks accumulate full blocks); entries with negative weight travel in
+//                     their own tiles and are subtracted with the negate-A immediate.  At a row's end it waits for the
+//                     MMAs, stores 2^-2e x accumulator (and the transpose of rows 64..127 x columns 0..63) into the
+//                     shared-memory matrix of the epilogue and reloads 2^2e (G + reg I) for the next row;
 //   4 epilogue warps : a systolic pipeline over the row's blocks.  Thread j owns matrix row j, warp q column block q:
 //                     h = M x - b from the shared matrix; then warp q folds the deltas of blocks 0..q-1 into its h as
 //                     they are published, runs the 3-step CG of its own 32 x 32 block and publishes its delta.  Nothing in
@@ -390,11 +392,19 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
         setmaxnreg_inc<REG_MMA>();
         // ================= MMA warpgroup =================
         // The accumulated block: feature rows [r0, r0 + 128) x feature columns [c0, c0 + 128); d0 holds rows r0 .. r0 + 63,
-        // d1 rows r0 + 64 .. r0 + 127 (fragment layout: sm90_ptx.cuh)
+        // d1 rows r0 + 64 .. r0 + 127 (fragment layout: sm90_ptx.cuh).  Fused mode: the row's matrix is symmetric, so d0
+        // only accumulates columns 0 .. 63 (m64n64: a quarter of the tensor-core work and of its shared-memory operand
+        // reads saved); its columns 64 .. 127 are the transpose of d1's columns 0 .. 63 and are stored from there.
         const int r0 = (D == 256 && ta.pass == 2) ? 128 : 0, c0 = (D == 256 && ta.pass > 0) ? 128 : 0;
         const int wq = warp - W_MMA;
         const int fr = 16 * wq + (lane >> 2), fc = 2 * (lane & 3);   // fragment row / column of register 0
-        float d0[64], d1[64];
+        constexpr int N0 = PARTIAL ? 128 : 64;                        // columns accumulated in d0
+        float d0[N0 / 2], d1[64];
+        auto mma0 = [&](auto neg, uint64_t adesc, uint64_t bdesc) {
+            constexpr bool NEG = decltype(neg)::value;
+            if constexpr (PARTIAL) wgmma_m64n128k16_f16<NEG>(d0, adesc, bdesc);
+            else wgmma_m64n64k16_f16<NEG>(d0, adesc, bdesc);
+        };
         // a new row's accumulator: 2^2e (G + reg I) in fused mode (so that the epilogue reads one matrix), 0 for chunks
         auto acc_init = [&]() {
             const float s2 = scale * scale;
@@ -405,14 +415,14 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                     const int r = fr + 8 * h, c = 8 * n + fc;
                     float2 g0 = make_float2(0.f, 0.f), g1 = make_float2(0.f, 0.f);
                     if (!PARTIAL) {
-                        g0 = __ldg(reinterpret_cast<const float2*>(a.G + (size_t)r * D + c));
+                        if (8 * n < N0) g0 = __ldg(reinterpret_cast<const float2*>(a.G + (size_t)r * D + c));
                         g1 = __ldg(reinterpret_cast<const float2*>(a.G + (size_t)(r + 64) * D + c));
                         g0.x += r == c ? a.reg : 0.f;
                         g0.y += r == c + 1 ? a.reg : 0.f;
                         g1.x += r + 64 == c ? a.reg : 0.f;
                         g1.y += r + 64 == c + 1 ? a.reg : 0.f;
                     }
-                    d0[4 * n + 2 * h] = g0.x * s2; d0[4 * n + 2 * h + 1] = g0.y * s2;
+                    if (8 * n < N0) { d0[4 * n + 2 * h] = g0.x * s2; d0[4 * n + 2 * h + 1] = g0.y * s2; }
                     d1[4 * n + 2 * h] = g1.x * s2; d1[4 * n + 2 * h + 1] = g1.y * s2;
                 }
         };
@@ -442,16 +452,16 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                     const uint64_t al0 = smem_desc(lo + k0 + r0 * 16, LBO, 128), al1 = smem_desc(lo + k0 + (r0 + 64) * 16, LBO, 128);
                     const uint64_t bh = smem_desc(hi + k0 + c0 * 16, LBO, 128), bl = smem_desc(lo + k0 + c0 * 16, LBO, 128);
                     if (meta & F_NEG) {
-                        wgmma_m64n128k16_f16<true>(d0, ah0, bh);
-                        wgmma_m64n128k16_f16<true>(d0, ah0, bl);
-                        wgmma_m64n128k16_f16<true>(d0, al0, bh);
+                        mma0(std::true_type{}, ah0, bh);
+                        mma0(std::true_type{}, ah0, bl);
+                        mma0(std::true_type{}, al0, bh);
                         wgmma_m64n128k16_f16<true>(d1, ah1, bh);
                         wgmma_m64n128k16_f16<true>(d1, ah1, bl);
                         wgmma_m64n128k16_f16<true>(d1, al1, bh);
                     } else {
-                        wgmma_m64n128k16_f16<false>(d0, ah0, bh);
-                        wgmma_m64n128k16_f16<false>(d0, ah0, bl);
-                        wgmma_m64n128k16_f16<false>(d0, al0, bh);
+                        mma0(std::false_type{}, ah0, bh);
+                        mma0(std::false_type{}, ah0, bl);
+                        mma0(std::false_type{}, al0, bh);
                         wgmma_m64n128k16_f16<false>(d1, ah1, bh);
                         wgmma_m64n128k16_f16<false>(d1, ah1, bl);
                         wgmma_m64n128k16_f16<false>(d1, al1, bh);
@@ -461,9 +471,9 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                 if (meta & F_LAST) {
                     wgmma_wait<0>();
 #pragma unroll
-                    for (int i = 0; i < 64; ++i) { acc_fence(d0[i]); acc_fence(d1[i]); }
+                    for (int i = 0; i < 64; ++i) { if (i < N0 / 2) acc_fence(d0[i]); acc_fence(d1[i]); }
                     mbar_wait_idle(&S.acc_empty, aph ^ 1u);   // the epilogue is done with the previous row
-                    if (PARTIAL) {
+                    if constexpr (PARTIAL) {
                         // the chunk of item my_first + seq * stride: float atomics (the chunks of one row are summed in
                         // arrival order); pass 1 of d = 256 also adds the transposed block
                         const int slot = ta.items[3 * (a.row_begin + my_first + seq * stride) + 2];
@@ -491,8 +501,12 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
 #pragma unroll
                                 for (int i = 0; i < 2; ++i) {
                                     const int r = fr + 8 * h, c = 8 * n + fc + i;
-                                    S.mat[c * 128 + (r ^ msw(c))] = d0[4 * n + 2 * h + i] * inv2;
-                                    S.mat[c * 128 + ((r + 64) ^ msw(c))] = d1[4 * n + 2 * h + i] * inv2;
+                                    const float v1 = d1[4 * n + 2 * h + i] * inv2;
+                                    S.mat[c * 128 + ((r + 64) ^ msw(c))] = v1;
+                                    if (8 * n < N0) {   // (r, c) from d0, and (c, r + 64) = (r + 64, c) by symmetry
+                                        S.mat[c * 128 + (r ^ msw(c))] = d0[4 * n + 2 * h + i] * inv2;
+                                        S.mat[(r + 64) * 128 + (c ^ msw(r + 64))] = v1;
+                                    }
                                 }
                     }
                     __syncwarp();
@@ -504,7 +518,7 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
             }
             wgmma_wait<0>();   // the group's operand reads are done
 #pragma unroll
-            for (int i = 0; i < 64; ++i) { acc_fence(d0[i]); acc_fence(d1[i]); }
+            for (int i = 0; i < 64; ++i) { if (i < N0 / 2) acc_fence(d0[i]); acc_fence(d1[i]); }
             __syncwarp();
             if (lane == 0) mbar_arrive(&S.op_empty[os]);   // (after a stop nobody waits for it any more)
             if (++os == NO) { os = 0; oph ^= 1u; }

@@ -103,8 +103,33 @@ __device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t ad
                      : "memory");
     }
 }
+// D[64 x 64] (+)= (+/-A)[64 x 16] B[16 x 64]^T: the first 64 columns of the above, same fragment layout (n < 8)
+#define BFL_WGMMA_ACC32(d)                                                                                              \
+    "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),         \
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),        \
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),       \
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+#define BFL_WGMMA_REGS32                                                                                                \
+    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "   \
+    "%24, %25, %26, %27, %28, %29, %30, %31}"
+template <bool NEG>
+__device__ __forceinline__ void wgmma_m64n64k16_f16(float (&d)[32], uint64_t adesc, uint64_t bdesc) {
+    if (NEG) {
+        asm volatile("wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 " BFL_WGMMA_REGS32 ", %32, %33, 1, -1, 1, 0, 0;"
+                     : BFL_WGMMA_ACC32(d)
+                     : "l"(adesc), "l"(bdesc)
+                     : "memory");
+    } else {
+        asm volatile("wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 " BFL_WGMMA_REGS32 ", %32, %33, 1, 1, 1, 0, 0;"
+                     : BFL_WGMMA_ACC32(d)
+                     : "l"(adesc), "l"(bdesc)
+                     : "memory");
+    }
+}
 #undef BFL_WGMMA_ACC64
 #undef BFL_WGMMA_REGS64
+#undef BFL_WGMMA_ACC32
+#undef BFL_WGMMA_REGS32
 
 // fp32 pairs (two FMULs / FFMAs: sm_90 has no packed fp32 arithmetic)
 __device__ __forceinline__ float2 f2mul(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
