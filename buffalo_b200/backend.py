@@ -234,6 +234,13 @@ class CuSGD(object):
 
     # --- device-resident path ---------------------------------------------------------------
     def bind_factors(self, P, Q, Qb, num_total_samples):
+        """P, Q: torch float32 CUDA tensors [rows, vdim] (padding columns zero), Qb: Q.shape[0] floats; updated in
+        place.  The kernels stride rows by vdim, so a narrower tensor would be read and written past its end."""
+        vdim = self.get_vdim()
+        if P.ndim != 2 or Q.ndim != 2 or P.shape[1] != vdim or Q.shape[1] != vdim:
+            raise ValueError("P and Q must be [rows, vdim=%d] (got %s, %s)" % (vdim, tuple(P.shape), tuple(Q.shape)))
+        if Qb.numel() != Q.shape[0]:
+            raise ValueError("Qb must hold %d elements (one per row of Q), got %s" % (Q.shape[0], tuple(Qb.shape)))
         self._keep = [P, Q, Qb]
         _cabi.check(self._lib.bfl_sgd_bind_factors_device(self._h, _dev(P, "float32", "P"), P.shape[0],
                                                           _dev(Q, "float32", "Q"), Q.shape[0],
