@@ -7,19 +7,16 @@ Two feeding modes, same results:
     obj.partial_update(start_x, next_x, indptr, keys, vals, axis) (als.py:115-142).
 The backend is GPU-only; `accelerator` is accepted and ignored (both values run the sm_90a kernels).
 """
-import json
 import time
 
 import numpy as np
 
-from buffalo_b200 import data as _data
 from buffalo_b200.algo.base import Algo, Serializable
 from buffalo_b200.algo.options import ALSOption
 from buffalo_b200.backend import CuALS
 from buffalo_b200.data.base import Data
 from buffalo_b200.data.buffered_data import BufferedDataMatrix
 from buffalo_b200.evaluate import Evaluable
-from buffalo_b200.misc import aux, log
 
 inited_CUALS = True
 
@@ -32,25 +29,8 @@ class ALS(Algo, ALSOption, Evaluable, Serializable):
         ALSOption.__init__(self, *args, **kwargs)
         Evaluable.__init__(self, *args, **kwargs)
         Serializable.__init__(self, *args, **kwargs)
-        if opt_path is None:
-            opt_path = ALSOption().get_default_option()
-        self.logger = log.get_logger("ALS")
-        self.opt, self.opt_path = self.get_option(opt_path)
-        self.obj = CuALS()
-        assert self.obj.init(bytes(self.opt_path, "utf-8")), \
-            "cannot parse option file: %s (%s)" % (opt_path, getattr(self.obj, "last_error", ""))
-        self.data = None
-        data = kwargs.get("data")
-        data_opt = kwargs.get("data_opt", self.opt.get("data_opt"))
-        if data_opt:
-            self.data = _data.load(data_opt)
-            self.data.create()
-        elif isinstance(data, Data):
-            self.data = data
-        self.logger.info("ALS(%s)" % json.dumps(self.opt, indent=2))
-        if self.data:
-            self.logger.info(self.data.show_info())
-            assert self.data.data_type in ["matrix"]
+        self._init_trainer("ALS", ALSOption, CuALS, opt_path,
+                           lambda path, err: "cannot parse option file: %s (%s)" % (path, err), kwargs)
 
     @staticmethod
     def new(path, data_fields=[]):
@@ -125,17 +105,8 @@ class ALS(Algo, ALSOption, Evaluable, Serializable):
         self.logger.debug(f"{group} updated: processed({updated}) elapsed({time.time() - t0:0.3f}s)")
         return nume, deno
 
-    def _resident_capable(self):
-        if self.opt.get("_b200_resident") is False:
-            return False
-        try:
-            import torch
-            free, _ = torch.cuda.mem_get_info()
-        except Exception:
-            return False
-        h = self.data.get_header()
-        need = 2 * h["num_nnz"] * 8 + (h["num_users"] + h["num_items"]) * (self.vdim * 4 + 8)
-        return need * 1.3 < free
+    def _rmse(self, nume, deno):
+        return (nume / (deno + self.opt.eps)) ** 0.5           # als.py:171
 
     def _train_resident(self, training_callback):
         import torch
@@ -145,11 +116,7 @@ class ALS(Algo, ALSOption, Evaluable, Serializable):
         tP, tQ = torch.from_numpy(self.P).to(dev), torch.from_numpy(self.Q).to(dev)
         self.obj.bind_factors(tP, tQ)
         for axis, G in enumerate(("rowwise", "colwise")):
-            grp = self.data.get_group(G)
-            n = int(grp["indptr"][-1]) if len(grp["indptr"]) else 0
-            t = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a, dtype=dt)).to(dev)  # noqa: E731
-            self.obj.bind_csr(axis, t(grp["indptr"][:], np.int64), t(grp["key"][:max(n, 1)] if n else np.zeros(1), np.int32),
-                              t(grp["val"][:max(n, 1)] if n else np.zeros(1), np.float32))
+            self.obj.bind_csr(axis, *self._csr_to_device(G, dev))
         loss = torch.zeros(2, dtype=torch.float64, device=dev)
 
         def sync_back():
@@ -161,9 +128,9 @@ class ALS(Algo, ALSOption, Evaluable, Serializable):
                 self.obj.precompute_device(axis)
                 self.obj.update_device(axis, 0, rows, loss)
             n_, d_ = loss.cpu().numpy()
-            return float(n_), float(d_)
+            return self._rmse(float(n_), float(d_))
         try:
-            return self._epoch_loop(one_iteration, sync_back, training_callback)
+            return self._timed_epochs(one_iteration, sync_back, training_callback)
         finally:
             sync_back()
             self.obj.initialize_model(self.P, self.Q)   # leave the holder on host-pointer semantics
@@ -176,33 +143,12 @@ class ALS(Algo, ALSOption, Evaluable, Serializable):
         def one_iteration():
             n1, d1 = self._iterate(buf, group="rowwise")
             n2, d2 = self._iterate(buf, group="colwise")
-            return n1 + n2, d1 + d2
-        return self._epoch_loop(one_iteration, lambda: None, training_callback)
+            return self._rmse(n1 + n2, d1 + d2)
+        return self._timed_epochs(one_iteration, lambda: None, training_callback)
 
-    def _epoch_loop(self, one_iteration, sync_back, training_callback):
-        best_loss, rmse, self.validation_result = float("inf"), None, {}
+    def _timed_epochs(self, one_iteration, sync_back, training_callback):
         t_all = time.time()
-        for i in range(self.opt.num_iters):
-            t0 = time.time()
-            nume, deno = one_iteration()
-            train_t = time.time() - t0
-            rmse = (nume / (deno + self.opt.eps)) ** 0.5           # als.py:171
-            metrics = {"train_loss": rmse}
-            if self.opt.validation and self.opt.evaluation_on_learning and self.periodical(self.opt.evaluation_period, i):
-                t0 = time.time()
-                sync_back()
-                self.validation_result = self.get_validation_results()
-                vals = " ".join(f"{k}:{v:0.5f}" for k, v in self.validation_result.items())
-                self.logger.info(f"Validation: {vals} Elapsed {time.time() - t0:0.3f} secs")
-                metrics.update({"val_%s" % k: v for k, v in self.validation_result.items()})
-                if callable(training_callback):
-                    training_callback(i, metrics)
-            self.logger.info("Iteration %d: RMSE %.3f Elapsed %.3f secs" % (i + 1, rmse, train_t))
-            if self.opt.save_best:
-                sync_back()
-            best_loss = self.save_best_only(rmse, best_loss, i)
-            if self.early_stopping(rmse):
-                break
+        rmse = self._epoch_loop(one_iteration, sync_back, training_callback, "RMSE", float("inf"))
         self.logger.info(f"elapsed for full epochs: {time.time() - t_all:.2f} sec")
         return rmse
 
@@ -214,7 +160,9 @@ class ALS(Algo, ALSOption, Evaluable, Serializable):
                 G[:, :self.opt.d] = F[:, :self.opt.d]
                 setattr(self, name, G)
         self.obj.initialize_model(self.P, self.Q)
-        rmse = self._train_resident(training_callback) if self._resident_capable() else self._train_chunked(training_callback)
+        h = self.data.get_header()
+        need = 2 * h["num_nnz"] * 8 + (h["num_users"] + h["num_items"]) * (self.vdim * 4 + 8)
+        rmse = self._train_resident(training_callback) if self._resident_capable(need) else self._train_chunked(training_callback)
         if self.opt.d < self.vdim:            # als.py:191-193
             self.P = np.ascontiguousarray(self.P[:, :self.opt.d])
             self.Q = np.ascontiguousarray(self.Q[:, :self.opt.d])

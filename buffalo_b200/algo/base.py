@@ -1,13 +1,17 @@
 """Host-side mixins shared by the trainers (buffalo/algo/base.py): id maps, top-k queries, similarity,
-early stopping / save-best bookkeeping and the length-prefixed pickle container of Serializable.
-Pure host glue around the factor matrices; nothing here is on the GPU hot path."""
+early stopping / save-best bookkeeping, the trainers' constructor body and epoch loop, and the length-prefixed pickle
+container of Serializable.  Pure host glue around the factor matrices; nothing here is on the GPU hot path."""
 import abc
+import json
 import pickle
 import struct
+import time
 
 import numpy as np
 
-from buffalo_b200.misc import aux
+from buffalo_b200 import data as _data
+from buffalo_b200.data.base import Data
+from buffalo_b200.misc import aux, log
 
 EPS = 1e-8
 
@@ -56,6 +60,81 @@ class Algo(abc.ABC):
             self.logger.info("Reached at early_stopping rounds, stopping train.")
             return True
         return False
+
+    # ---- training driver shared by the trainers -------------------------------------------------------
+    def _init_trainer(self, name, opt_cls, make_obj, opt_path, init_error, kwargs):
+        """Constructor body of a trainer: options, the backend holder make_obj(), data, logging.
+        init_error(opt_path, last_error) is the message of the assertion that the holder accepted the options."""
+        if opt_path is None:
+            opt_path = opt_cls().get_default_option()
+        self.logger = log.get_logger(name)
+        self.opt, self.opt_path = self.get_option(opt_path)
+        self.obj = make_obj()
+        assert self.obj.init(bytes(self.opt_path, "utf-8")), init_error(opt_path, getattr(self.obj, "last_error", ""))
+        self.data = None
+        data = kwargs.get("data")
+        data_opt = kwargs.get("data_opt", self.opt.get("data_opt"))
+        if data_opt:
+            self.data = _data.load(data_opt)
+            assert self.data.data_type == "matrix"
+            self.data.create()
+        elif isinstance(data, Data):
+            self.data = data
+        self.logger.info("%s(%s)" % (name, json.dumps(self.opt, indent=2)))
+        if self.data:
+            self.logger.info(self.data.show_info())
+            assert self.data.data_type in ["matrix"]
+
+    def _resident_capable(self, need_bytes):
+        """True when the device-resident path may run: not switched off by _b200_resident, and need_bytes fits in the
+        free device memory with 30% to spare."""
+        if self.opt.get("_b200_resident") is False:
+            return False
+        try:
+            import torch
+            free, _ = torch.cuda.mem_get_info()
+        except Exception:
+            return False
+        return need_bytes * 1.3 < free
+
+    def _csr_to_device(self, group, dev):
+        """(indptr int64, keys int32, vals float32) torch tensors on `dev` of one CSR group of self.data; an empty
+        group gets one-element key and value arrays."""
+        import torch
+        grp = self.data.get_group(group)
+        n = int(grp["indptr"][-1]) if len(grp["indptr"]) else 0
+
+        def t(a, dt):
+            return torch.from_numpy(np.ascontiguousarray(a, dtype=dt)).to(dev)
+        return (t(grp["indptr"][:], np.int64), t(grp["key"][:n] if n else np.zeros(1), np.int32),
+                t(grp["val"][:n] if n else np.zeros(1), np.float32))
+
+    def _epoch_loop(self, one_iteration, sync_back, training_callback, loss_label, best_loss):
+        """opt.num_iters epochs of one_iteration() -> training loss, with periodic validation and the training
+        callback, save-best and early stopping.  sync_back() brings device-resident factors to the host before they
+        are validated or saved; best_loss is what save-best compares the first loss against.  Returns the last loss."""
+        loss, self.validation_result = None, {}
+        for i in range(self.opt.num_iters):
+            t0 = time.time()
+            loss = one_iteration()
+            train_t = time.time() - t0
+            metrics = {"train_loss": loss}
+            if self.opt.validation and self.opt.evaluation_on_learning and self.periodical(self.opt.evaluation_period, i):
+                t0 = time.time()
+                sync_back()
+                self.validation_result = self.get_validation_results()
+                vals = " ".join(f"{k}:{v:0.5f}" for k, v in self.validation_result.items())
+                self.logger.info(f"Validation: {vals} Elapsed {time.time() - t0:0.3f} secs")
+                metrics.update({"val_%s" % k: v for k, v in self.validation_result.items()})
+                if callable(training_callback):
+                    training_callback(i, metrics)
+            self.logger.info("Iteration %d: %s %.3f Elapsed %.3f secs" % (i + 1, loss_label, loss, train_t))
+            if self.opt.save_best:
+                sync_back()
+            best_loss = self.save_best_only(loss, best_loss, i)
+            if self.early_stopping(loss):
+                break
+        return loss
 
     # ---- id maps ------------------------------------------------------------------------------
     def _build_map(self, field, count_key, ids_attr, map_attr, flag):

@@ -1,16 +1,13 @@
 """BPRMF trainer (buffalo/algo/bpr.py) on the H100 backend."""
-import json
 
 import numpy as np
 
-from buffalo_b200 import data as _data
 from buffalo_b200.algo.base import Algo, Serializable
 from buffalo_b200.algo.options import BPRMFOption
 from buffalo_b200.algo.sgd_common import SGDTrainerMixin
 from buffalo_b200.backend import CuSGD
 from buffalo_b200.data.base import Data
 from buffalo_b200.evaluate import Evaluable
-from buffalo_b200.misc import log
 
 inited_CUBPR = True
 
@@ -24,25 +21,8 @@ class BPRMF(SGDTrainerMixin, Algo, BPRMFOption, Evaluable, Serializable):
         self._OPT.__init__(self, *args, **kwargs)
         Evaluable.__init__(self, *args, **kwargs)
         Serializable.__init__(self, *args, **kwargs)
-        if opt_path is None:
-            opt_path = self._OPT().get_default_option()
-        self.logger = log.get_logger(self._NAME)
-        self.opt, self.opt_path = self.get_option(opt_path)
-        self.obj = CuSGD(self._KIND)
-        assert self.obj.init(bytes(self.opt_path, "utf-8")), \
-            "cannot parse option file: %s (%s)" % (opt_path, getattr(self.obj, "last_error", ""))
-        self.data = None
-        data = kwargs.get("data")
-        data_opt = kwargs.get("data_opt", self.opt.get("data_opt"))
-        if data_opt:
-            self.data = _data.load(data_opt)
-            self.data.create()
-        elif isinstance(data, Data):
-            self.data = data
-        self.logger.info("%s(%s)" % (self._NAME, json.dumps(self.opt, indent=2)))
-        if self.data:
-            self.logger.info(self.data.show_info())
-            assert self.data.data_type in ["matrix"]
+        self._init_trainer(self._NAME, self._OPT, lambda: CuSGD(self._KIND), opt_path,
+                           lambda path, err: "cannot parse option file: %s (%s)" % (path, err), kwargs)
 
     @staticmethod
     def new(path, data_fields=[]):

@@ -7,19 +7,16 @@ Two feeding modes, same results:
     BufferedDataMatrix chunk, normalize, swap (plsi.py:132-160).
 The factor arrays are [rows, d] (plsi.py:107-111: not padded).
 """
-import json
 import time
 
 import numpy as np
 
-from buffalo_b200 import data as _data
 from buffalo_b200.algo.base import Algo, Serializable
 from buffalo_b200.algo.options import PLSIOption
 from buffalo_b200.backend import CuPLSI
 from buffalo_b200.data.base import Data
 from buffalo_b200.data.buffered_data import BufferedDataMatrix
 from buffalo_b200.evaluate import Evaluable
-from buffalo_b200.misc import log
 
 
 class PLSI(Algo, PLSIOption, Evaluable, Serializable):
@@ -30,26 +27,8 @@ class PLSI(Algo, PLSIOption, Evaluable, Serializable):
         PLSIOption.__init__(self, *args, **kwargs)
         Evaluable.__init__(self, *args, **kwargs)
         Serializable.__init__(self, *args, **kwargs)
-        if opt_path is None:
-            opt_path = PLSIOption().get_default_option()
-        self.logger = log.get_logger("PLSI")
-        self.opt, self.opt_path = self.get_option(opt_path)
-        self.obj = CuPLSI()
-        assert self.obj.init(bytes(self.opt_path, "utf-8")), \
-            "putting parameter to cython object failed (%s)" % getattr(self.obj, "last_error", "")
-        self.data = None
-        data = kwargs.get("data")
-        data_opt = kwargs.get("data_opt", self.opt.get("data_opt"))
-        if data_opt:
-            self.data = _data.load(data_opt)
-            assert self.data.data_type == "matrix"
-            self.data.create()
-        elif isinstance(data, Data):
-            self.data = data
-        self.logger.info("PLSI ({})".format(json.dumps(self.opt, indent=2)))
-        if self.data:
-            self.logger.info(self.data.show_info())
-            assert self.data.data_type in ["matrix"]
+        self._init_trainer("PLSI", PLSIOption, CuPLSI, opt_path,
+                           lambda path, err: "putting parameter to cython object failed (%s)" % err, kwargs)
 
     @staticmethod
     def new(path, data_fields=[]):
@@ -155,19 +134,6 @@ class PLSI(Algo, PLSIOption, Evaluable, Serializable):
         self.logger.debug(f"updated processed({updated}) elapsed(data feed: {feed_t:0.5f} update: {update_t:0.5f})")
         return loss_nume, loss_deno
 
-    def _resident_capable(self):
-        if self.opt.get("_b200_resident") is False:
-            return False
-        try:
-            import torch
-            free, _ = torch.cuda.mem_get_info()
-        except Exception:
-            return False
-        h = self.data.get_header()
-        # rowwise CSR + factors + the item accumulator
-        need = h["num_nnz"] * 8 + h["num_users"] * (self.vdim * 4 + 9) + h["num_items"] * self.vdim * 8
-        return need * 1.3 < free
-
     def _train_resident(self, training_callback):
         import torch
         dev = torch.device("cuda", torch.cuda.current_device())
@@ -179,13 +145,9 @@ class PLSI(Algo, PLSIOption, Evaluable, Serializable):
             return T
         tP, tQ = padded(self.P), padded(self.Q)
         self.obj.bind_factors(tP, tQ)
-        grp = self.data.get_group("rowwise")
-        n = int(grp["indptr"][-1]) if len(grp["indptr"]) else 0
-        vals = np.ascontiguousarray(grp["val"][:n], dtype=np.float32)
-        t = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a, dtype=dt)).to(dev)  # noqa: E731
-        self.obj.bind_csr(t(grp["indptr"][:], np.int64), t(grp["key"][:n] if n else np.zeros(1), np.int32),
-                          t(vals if n else np.zeros(1), np.float32))
-        loss_deno = float(np.sum(vals, dtype=np.float64))
+        indptr, keys, vals = self._csr_to_device("rowwise", dev)
+        self.obj.bind_csr(indptr, keys, vals)
+        loss_deno = float(np.sum(vals.cpu().numpy(), dtype=np.float64))
         loss = torch.zeros(1, dtype=torch.float64, device=dev)
         rows = self.P.shape[0]
 
@@ -198,41 +160,18 @@ class PLSI(Algo, PLSIOption, Evaluable, Serializable):
             self.obj.update_device(0, rows, loss)
             self.obj.normalize_device(self.opt.alpha1, self.opt.alpha2)
             self.obj.swap_device()
-            return float(loss.cpu().numpy()[0]), loss_deno
+            return self._loss(float(loss.cpu().numpy()[0]), loss_deno)
         try:
-            return self._epoch_loop(one_iteration, sync_back, training_callback)
+            return self._epoch_loop(one_iteration, sync_back, training_callback, "Loss", 1e+10)
         finally:
             sync_back()
             self.obj.set_model(self.P, self.Q)   # leave the holder on host-pointer semantics
 
     def _train_chunked(self, training_callback):
-        return self._epoch_loop(self._iterate, lambda: None, training_callback)
+        return self._epoch_loop(lambda: self._loss(*self._iterate()), lambda: None, training_callback, "Loss", 1e+10)
 
-    def _epoch_loop(self, one_iteration, sync_back, training_callback):
-        best_loss, loss, self.validation_result = 1e+10, None, {}
-        for i in range(self.opt.num_iters):
-            start_t = time.time()
-            nume, deno = one_iteration()
-            train_t = time.time() - start_t
-            loss = nume / (deno + self.opt.eps)                              # plsi.py:171
-            metrics = {"train_loss": loss}
-            if self.opt.validation and self.opt.evaluation_on_learning and self.periodical(self.opt.evaluation_period, i):
-                start_t = time.time()
-                sync_back()
-                self.validation_result = self.get_validation_results()
-                vali_t = time.time() - start_t
-                val_str = " ".join([f"{k}:{v:0.5f}" for k, v in self.validation_result.items()])
-                self.logger.info(f"Validation: {val_str} Elapsed {vali_t:0.3f} secs")
-                metrics.update({"val_%s" % k: v for k, v in self.validation_result.items()})
-                if callable(training_callback):
-                    training_callback(i, metrics)
-            self.logger.info("Iteration %d: Loss %.3f Elapsed %.3f secs" % (i + 1, loss, train_t))
-            if self.opt.save_best:
-                sync_back()
-            best_loss = self.save_best_only(loss, best_loss, i)
-            if self.early_stopping(loss):
-                break
-        return loss
+    def _loss(self, nume, deno):
+        return nume / (deno + self.opt.eps)                              # plsi.py:171
 
     def train(self, training_callback=None):
         self.logger.info(f"Train pLSI, K: {self.opt.d}, alpha1: {self.opt.alpha1}, "
@@ -240,7 +179,10 @@ class PLSI(Algo, PLSIOption, Evaluable, Serializable):
         for name in ("P", "Q"):          # factors replaced or inherited by the user: the backend needs float32 [rows, d]
             setattr(self, name, np.ascontiguousarray(getattr(self, name), dtype=np.float32))
         self.obj.set_model(self.P, self.Q)
-        if self._resident_capable():
+        h = self.data.get_header()
+        # rowwise CSR + factors + the item accumulator
+        need = h["num_nnz"] * 8 + h["num_users"] * (self.vdim * 4 + 9) + h["num_items"] * self.vdim * 8
+        if self._resident_capable(need):
             loss = self._train_resident(training_callback)
         else:
             loss = self._train_chunked(training_callback)

@@ -74,26 +74,14 @@ class SGDTrainerMixin(object):
     def train(self, training_callback=None):
         self.validation_result = {}
         self.sampling_loss_samples()
-        best_loss = float("inf")
         self._prepare_train()
-        for i in range(self.opt.num_iters):
-            t0 = time.time()
+
+        def one_iteration():
             self._iterate()
             self.obj.wait_until_done()
-            loss = self.compute_loss() if self.opt.compute_loss_on_training else 0.0
-            metrics = {"train_loss": loss}
-            if self.opt.validation and self.opt.evaluation_on_learning and self.periodical(self.opt.evaluation_period, i):
-                tv = time.time()
-                self.validation_result = self.get_validation_results()
-                vals = " ".join(f"{k}:{v:0.5f}" for k, v in self.validation_result.items())
-                self.logger.info(f"Validation: {vals} Elased {time.time() - tv:0.3f}")
-                metrics.update({"val_%s" % k: v for k, v in self.validation_result.items()})
-                if callable(training_callback):
-                    training_callback(i, metrics)
-            self.logger.info("Iteration %s: PR-Loss %.3f Elapsed %.3f secs" % (i + 1, loss, time.time() - t0))
-            best_loss = self.save_best_only(loss, best_loss, i)
-            if self.early_stopping(loss):
-                break
+            return self.compute_loss() if self.opt.compute_loss_on_training else 0.0
+        # update_parameters() already copied the factors back to the host arrays: nothing to sync
+        self._epoch_loop(one_iteration, lambda: None, training_callback, "PR-Loss", float("inf"))
         ret = {"train_loss": self._finalize_train()}
         ret.update({"val_%s" % k: v for k, v in self.validation_result.items()})
         return ret

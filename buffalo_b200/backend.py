@@ -45,45 +45,71 @@ def _opt_bytes(opt):
     return json.dumps(dict(opt)).encode("utf-8"), False
 
 
-class CuALS(object):
-    """ALS backend (CyALS, _als.pyx:28-63; CUDA holder cuda/_als.pyx:25-67)."""
+def _device_view(ptr, shape, typestr):
+    """torch CUDA tensor over `ptr` (memory the library owns) through __cuda_array_interface__."""
+    import torch
 
-    def __init__(self):
+    class _Arr(object):
+        __cuda_array_interface__ = {"shape": tuple(shape), "typestr": typestr, "data": (ptr, False), "version": 2}
+    return torch.as_tensor(_Arr(), device="cuda")
+
+
+class _Holder(object):
+    """Lifecycle shared by the bfl_<prefix>_* handles: create/destroy, init, get_vdim and the tensors kept alive
+    while the native side holds their pointers."""
+
+    def __init__(self, prefix, *create_args):
         self._lib = _cabi.lib()
-        self._h = self._lib.bfl_als_create()
+        self._prefix = prefix
+        self._h = self._fn("create")(*create_args)
         if not self._h:
-            raise MemoryError("bfl_als_create")
+            raise MemoryError("bfl_%s_create" % prefix)
         self._keep = []
+
+    def _fn(self, name):
+        return getattr(self._lib, "bfl_%s_%s" % (self._prefix, name))
 
     def __del__(self):
         h, self._h = getattr(self, "_h", None), None
         if h:
-            self._lib.bfl_als_destroy(h)
+            self._fn("destroy")(h)
 
     # --- reference method set -------------------------------------------------------------
     def init(self, opt_path):
         """opt_path: bytes/str path of the JSON option file (als.py:43), or a dict."""
         data, is_path = _opt_bytes(opt_path)
-        rc = self._lib.bfl_als_init(self._h, data) if is_path else self._lib.bfl_als_init_json(self._h, data)
+        rc = self._fn("init")(self._h, data) if is_path else self._fn("init_json")(self._h, data)
         if rc == 1:  # BFL_ERR_OPTION: the reference's init returns False (algo.cc:22-34)
             self.last_error = self._lib.bfl_last_error().decode("utf-8", "replace")
             return False
-        _cabi.check(rc, "bfl_als_init")
+        _cabi.check(rc, "bfl_%s_init" % self._prefix)
         if is_path:
             with open(data.decode("utf-8")) as fin:
-                self._d = int(json.load(fin)["d"])
+                opt = json.load(fin)
         else:
-            self._d = int(json.loads(data.decode("utf-8"))["d"])
+            opt = json.loads(data.decode("utf-8"))
+        self._d = int(opt["d"]) if "d" in opt else None
         return True
 
     def get_vdim(self):
-        return self._lib.bfl_als_get_vdim(self._h)
+        return self._fn("get_vdim")(self._h)
+
+    def _check_vdim(self, P, Q):
+        # the kernels stride rows by vdim, so a narrower matrix would be read and written past its end
+        vdim = self.get_vdim()
+        if P.ndim != 2 or Q.ndim != 2 or P.shape[1] != vdim or Q.shape[1] != vdim:
+            raise ValueError("P and Q must be [rows, vdim=%d] (got %s, %s)" % (vdim, tuple(P.shape), tuple(Q.shape)))
+
+
+class CuALS(_Holder):
+    """ALS backend (CyALS, _als.pyx:28-63; CUDA holder cuda/_als.pyx:25-67)."""
+
+    def __init__(self):
+        super().__init__("als")
 
     def initialize_model(self, P, Q):
         pP, pQ = _host(P, np.float32, 2, "P"), _host(Q, np.float32, 2, "Q")
-        vdim = self.get_vdim()
-        if P.shape[1] != vdim or Q.shape[1] != vdim:
-            raise ValueError("factor matrices must have %d columns (get_vdim())" % vdim)
+        self._check_vdim(P, Q)
         self._keep = [P, Q]  # native side retains the pointers (als.cc:78-79)
         _cabi.check(self._lib.bfl_als_initialize_model(self._h, pP, P.shape[0], pQ, Q.shape[0]), "initialize_model")
 
@@ -107,8 +133,7 @@ class CuALS(object):
     # --- device-resident path ---------------------------------------------------------------
     def bind_factors(self, P, Q):
         """P, Q: torch float32 CUDA tensors [rows, vdim], updated in place."""
-        vdim = self.get_vdim()
-        assert P.shape[1] == vdim and Q.shape[1] == vdim, "factor tensors need vdim=%d columns" % vdim
+        self._check_vdim(P, Q)
         self._keep = [P, Q]
         _cabi.check(self._lib.bfl_als_bind_factors_device(self._h, _dev(P, "float32", "P"), P.shape[0],
                                                           _dev(Q, "float32", "Q"), Q.shape[0]), "bind_factors")
@@ -142,50 +167,21 @@ class CuALS(object):
 
     def gram_tensor(self):
         """View of the current d x d Gram matrix as a torch tensor (multi-GPU all-reduce, tests)."""
-        import torch
         ptr = self._lib.bfl_als_gram_device_mut(self._h)
-        n = self._d * self._d
-
-        class _Arr(object):
-            __cuda_array_interface__ = {"shape": (n,), "typestr": "<f4", "data": (ptr, False), "version": 2}
-        return torch.as_tensor(_Arr(), device="cuda").view(self._d, self._d)
+        return _device_view(ptr, (self._d * self._d,), "<f4").view(self._d, self._d)
 
 
-class CuSGD(object):
+class CuSGD(_Holder):
     """BPRMF / WARP backend (CyBPRMF _bpr.pyx:34-92, CyWARP _warp.pyx:34-92, CyBPR cuda/_bpr.pyx:27-80)."""
 
     KIND = {"bpr": 0, "warp": 1}
 
     def __init__(self, kind):
-        self._lib = _cabi.lib()
         self.kind = kind
-        self._h = self._lib.bfl_sgd_create(self.KIND[kind])
-        if not self._h:
-            raise MemoryError("bfl_sgd_create")
-        self._keep = []
-
-    def __del__(self):
-        h, self._h = getattr(self, "_h", None), None
-        if h:
-            self._lib.bfl_sgd_destroy(h)
-
-    def init(self, opt_path):
-        data, is_path = _opt_bytes(opt_path)
-        rc = self._lib.bfl_sgd_init(self._h, data) if is_path else self._lib.bfl_sgd_init_json(self._h, data)
-        if rc == 1:
-            self.last_error = self._lib.bfl_last_error().decode("utf-8", "replace")
-            return False
-        _cabi.check(rc, "bfl_sgd_init")
-        return True
-
-    def get_vdim(self):
-        return self._lib.bfl_sgd_get_vdim(self._h)
+        super().__init__("sgd", self.KIND[kind])
 
     def initialize_model(self, P, Q, Qb, num_nnz, set_gpu=True):
-        vdim = self.get_vdim()
-        if P.ndim != 2 or Q.ndim != 2 or P.shape[1] != vdim or Q.shape[1] != vdim:
-            raise ValueError("P and Q must be [rows, vdim=%d] (got %s, %s): the backend copies rows*vdim floats"
-                             % (vdim, P.shape, Q.shape))
+        self._check_vdim(P, Q)
         if Qb.shape != (Q.shape[0], 1):
             raise ValueError("Qb must be [%d, 1], got %s" % (Q.shape[0], Qb.shape))
         self._keep = [P, Q, Qb]
@@ -235,10 +231,8 @@ class CuSGD(object):
     # --- device-resident path ---------------------------------------------------------------
     def bind_factors(self, P, Q, Qb, num_total_samples):
         """P, Q: torch float32 CUDA tensors [rows, vdim] (padding columns zero), Qb: Q.shape[0] floats; updated in
-        place.  The kernels stride rows by vdim, so a narrower tensor would be read and written past its end."""
-        vdim = self.get_vdim()
-        if P.ndim != 2 or Q.ndim != 2 or P.shape[1] != vdim or Q.shape[1] != vdim:
-            raise ValueError("P and Q must be [rows, vdim=%d] (got %s, %s)" % (vdim, tuple(P.shape), tuple(Q.shape)))
+        place."""
+        self._check_vdim(P, Q)
         if Qb.numel() != Q.shape[0]:
             raise ValueError("Qb must hold %d elements (one per row of Q), got %s" % (Q.shape[0], tuple(Qb.shape)))
         self._keep = [P, Q, Qb]
@@ -273,26 +267,17 @@ class CuSGD(object):
                     "apply_triples_device")
 
     def grad_tensor(self, which, shape):
-        import torch
         ptr = self._lib.bfl_sgd_grad_device(self._h, int(which))
         if not ptr:
             return None
-        n = int(np.prod(shape))
-
-        class _Arr(object):
-            __cuda_array_interface__ = {"shape": (n,), "typestr": "<f4", "data": (ptr, False), "version": 2}
-        return torch.as_tensor(_Arr(), device="cuda").view(*shape)
+        return _device_view(ptr, (int(np.prod(shape)),), "<f4").view(*shape)
 
     def count_tensor(self, which, rows):
         """int32[rows] sample counters of per_coordinate_normalize (0: P rows, 1: Q rows); None if not allocated."""
-        import torch
         ptr = self._lib.bfl_sgd_count_device(self._h, int(which))
         if not ptr:
             return None
-
-        class _Arr(object):
-            __cuda_array_interface__ = {"shape": (int(rows),), "typestr": "<i4", "data": (ptr, False), "version": 2}
-        return torch.as_tensor(_Arr(), device="cuda")
+        return _device_view(ptr, (int(rows),), "<i4")
 
     def set_trace(self, trials, negs):
         self._keep += [trials, negs]
@@ -311,40 +296,12 @@ class CuSGD(object):
         return loss.value, n.value
 
 
-class CuPLSI(object):
+class CuPLSI(_Holder):
     """pLSI backend (CyPLSI, buffalo/algo/_plsi.pyx:13-57).  Holder methods take the [rows, d] host arrays of
     buffalo/algo/plsi.py:107-111; the device-resident path takes [rows, vdim] torch CUDA tensors."""
 
     def __init__(self):
-        self._lib = _cabi.lib()
-        self._h = self._lib.bfl_plsi_create()
-        if not self._h:
-            raise MemoryError("bfl_plsi_create")
-        self._keep = []
-
-    def __del__(self):
-        h, self._h = getattr(self, "_h", None), None
-        if h:
-            self._lib.bfl_plsi_destroy(h)
-
-    # --- reference method set -------------------------------------------------------------
-    def init(self, opt_path):
-        """opt_path: bytes/str path of the JSON option file (plsi.py:31), or a dict."""
-        data, is_path = _opt_bytes(opt_path)
-        rc = self._lib.bfl_plsi_init(self._h, data) if is_path else self._lib.bfl_plsi_init_json(self._h, data)
-        if rc == 1:  # BFL_ERR_OPTION
-            self.last_error = self._lib.bfl_last_error().decode("utf-8", "replace")
-            return False
-        _cabi.check(rc, "bfl_plsi_init")
-        if is_path:
-            with open(data.decode("utf-8")) as fin:
-                self._d = int(json.load(fin)["d"])
-        else:
-            self._d = int(json.loads(data.decode("utf-8"))["d"])
-        return True
-
-    def get_vdim(self):
-        return self._lib.bfl_plsi_get_vdim(self._h)
+        super().__init__("plsi")
 
     def _factors(self, P, Q):
         pP, pQ = _host(P, np.float32, 2, "P"), _host(Q, np.float32, 2, "Q")
@@ -388,8 +345,7 @@ class CuPLSI(object):
     # --- device-resident path ---------------------------------------------------------------
     def bind_factors(self, P, Q):
         """P, Q: torch float32 CUDA tensors [rows, vdim] (padding columns zero), updated in place."""
-        vdim = self.get_vdim()
-        assert P.shape[1] == vdim and Q.shape[1] == vdim, "factor tensors need vdim=%d columns" % vdim
+        self._check_vdim(P, Q)
         self._keep = [P, Q]
         _cabi.check(self._lib.bfl_plsi_bind_factors_device(self._h, _dev(P, "float32", "P"), P.shape[0],
                                                            _dev(Q, "float32", "Q"), Q.shape[0]), "bind_factors")

@@ -1,5 +1,5 @@
-// Host-side plumbing shared by the ALS and SGD backends: last-error slot, launch counter,
-// device check, and the flat JSON option reader.
+// Host-side plumbing shared by the ALS, SGD and pLSI backends: last-error slot, launch counter,
+// device check, the holder core and the flat JSON option reader.
 #include "bfl_common.cuh"
 
 #include <cctype>
@@ -30,6 +30,84 @@ int require_device() {
     if (major != 9 || minor != 0)   // sm_90a code (wgmma) runs on compute capability 9.0 only
         BFL_FAIL(BFL_ERR_CUDA, "buffalo_b200 kernels are compiled for sm_90a only; current device has compute capability " +
                                    std::to_string(major) + "." + std::to_string(minor));
+    return BFL_OK;
+}
+
+// ---- holder core ----------------------------------------------------------------------
+Holder::~Holder() {
+    if (stream) cudaStreamDestroy(stream);
+}
+
+int Holder::attach_device() {
+    if (BFL_OK != require_device()) return BFL_ERR_CUDA;
+    int dev = 0;
+    BFL_CUDA(cudaGetDevice(&dev));
+    BFL_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
+    if (!stream) BFL_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
+    return BFL_OK;
+}
+
+int Holder::borrow_factors(float* P, int64_t P_rows_, float* Q, int64_t Q_rows_) {
+    if (!P || !Q || P_rows_ <= 0 || Q_rows_ <= 0) BFL_FAIL(BFL_ERR_ARG, "bad factor arguments");
+    if (((uintptr_t)P | (uintptr_t)Q) & 15) BFL_FAIL(BFL_ERR_ARG, "device factor pointers must be 16-byte aligned");
+    hostP = hostQ = nullptr;
+    ownP.release();
+    ownQ.release();
+    dP = P;
+    dQ = Q;
+    P_rows = P_rows_;
+    Q_rows = Q_rows_;
+    return BFL_OK;
+}
+
+int Holder::mirror_factors(float* P, int64_t P_rows_, float* Q, int64_t Q_rows_) {
+    if (!P || !Q || P_rows_ <= 0 || Q_rows_ <= 0) BFL_FAIL(BFL_ERR_ARG, "bad factor arguments");
+    hostP = P;
+    hostQ = Q;
+    P_rows = P_rows_;
+    Q_rows = Q_rows_;
+    if (BFL_OK != ownP.reserve((size_t)P_rows * vdim)) return BFL_ERR_CUDA;
+    if (BFL_OK != ownQ.reserve((size_t)Q_rows * vdim)) return BFL_ERR_CUDA;
+    dP = ownP.p;
+    dQ = ownQ.p;
+    return BFL_OK;
+}
+
+int init_holder(Holder* h, const char* src, bool is_path) {
+    if (!h || !src) BFL_FAIL(BFL_ERR_ARG, "null argument");
+    JsonOpt j;
+    std::string err;
+    if (is_path ? !j.load(src, &err) : !j.parse(src, &err))
+        BFL_FAIL(BFL_ERR_OPTION, is_path ? err : "Failed to parse: " + err);
+    return h->apply_options(j);
+}
+
+int CsrBinding::bind(const int64_t* d_indptr, const int32_t* d_keys, const float* d_vals, int64_t n_rows,
+                     int64_t n_nnz, bool with_vals) {
+    if (!d_indptr || (n_nnz > 0 && (!d_keys || (with_vals && !d_vals))) || n_rows <= 0)
+        BFL_FAIL(BFL_ERR_ARG, "bad CSR arguments");
+    indptr = d_indptr;
+    keys = d_keys;
+    vals = d_vals;
+    rows = n_rows;
+    nnz = n_nnz;
+    return BFL_OK;
+}
+
+int CsrBinding::check_range(int64_t row_begin, int64_t row_end) const {
+    if (row_begin < 0 || row_end > rows || row_end < row_begin) BFL_FAIL(BFL_ERR_ARG, "bad row range");
+    return BFL_OK;
+}
+
+int read_row_span(const int64_t* indptr, int64_t row_begin, int64_t row_end, cudaStream_t st, int64_t* begin,
+                  int64_t* end) {
+    int64_t ends[2] = {0, 0};
+    if (row_begin > 0)
+        BFL_CUDA(cudaMemcpyAsync(&ends[0], indptr + row_begin - 1, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    BFL_CUDA(cudaMemcpyAsync(&ends[1], indptr + row_end - 1, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    BFL_CUDA(cudaStreamSynchronize(st));
+    *begin = ends[0];
+    *end = ends[1];
     return BFL_OK;
 }
 

@@ -43,7 +43,7 @@ extern std::atomic<long long> g_launches;
         return (code);                                                                       \
     } while (0)
 
-int require_device();  // BFL_OK iff a CUDA device of compute capability 10.x is current
+int require_device();  // BFL_OK iff a CUDA device of compute capability 9.0 is current
 
 // out[i] = in[0] + ... + in[i] on `st` (in == out allowed); ingest.cu
 int inclusive_scan_i64(const long long* in, long long* out, long long n, cudaStream_t st);
@@ -158,5 +158,51 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return (uint32_t)__cvta_generic_to_shared(p);
 }
 #endif  // __CUDACC__
+
+// ---------------------------------------------------------------------------------------
+// holder core shared by the ALS, SGD and pLSI handles: options state, device attach and the P/Q factor pointers
+// ---------------------------------------------------------------------------------------
+struct Holder {
+    bool opt_set = false;
+    int d = 0, vdim = 0;
+    int num_sms = 0;
+    cudaStream_t stream = nullptr;
+
+    // factors: either owned device mirrors of retained host pointers, or borrowed device memory
+    float *hostP = nullptr, *hostQ = nullptr;
+    DevBuf<float> ownP, ownQ;
+    float *dP = nullptr, *dQ = nullptr;
+    int64_t P_rows = 0, Q_rows = 0;
+    bool factors_ready = false;
+
+    virtual ~Holder();
+    // parses the handle's options; option errors (BFL_ERR_OPTION) come before attach_device()
+    virtual int apply_options(const JsonOpt& j) = 0;
+    // require_device(), the SM count and the non-blocking stream (created once)
+    int attach_device();
+    // caller-owned device factors of 16-byte aligned rows; releases the owned mirrors
+    int borrow_factors(float* P, int64_t P_rows, float* Q, int64_t Q_rows);
+    // retains the caller's host factors and points dP/dQ at owned mirrors of rows * vdim floats (not yet copied)
+    int mirror_factors(float* P, int64_t P_rows, float* Q, int64_t Q_rows);
+};
+
+// bfl_*_init (src is a file path) and bfl_*_init_json (src is the JSON text)
+int init_holder(Holder* h, const char* src, bool is_path);
+
+// a device CSR of END offsets: borrowed through bind_csr_device, or a holder's own upload of the caller's indptr
+struct CsrBinding {
+    const int64_t* indptr = nullptr;
+    const int32_t* keys = nullptr;
+    const float* vals = nullptr;
+    int64_t rows = 0, nnz = 0;
+    // borrows a device CSR; with_vals: the holder reads values as well as keys
+    int bind(const int64_t* d_indptr, const int32_t* d_keys, const float* d_vals, int64_t n_rows, int64_t n_nnz,
+             bool with_vals);
+    int check_range(int64_t row_begin, int64_t row_end) const;
+};
+
+// begin/end entry offsets of rows [row_begin, row_end) read from a device `indptr` of END offsets; synchronises `st`
+int read_row_span(const int64_t* indptr, int64_t row_begin, int64_t row_end, cudaStream_t st, int64_t* begin,
+                  int64_t* end);
 
 }  // namespace bfl

@@ -264,48 +264,35 @@ __global__ void __launch_bounds__(256) plsi_init_kernel(float* F, int64_t rows, 
 
 }  // namespace
 
-struct bfl_plsi {
-    bool opt_set = false;
-    int d = 0, vdim = 0;
+// the Holder's hostP/hostQ are the caller's [rows x d] arrays (holder path), ownP/ownQ the library's device copies
+struct bfl_plsi : Holder {
     uint32_t seed = 0;
 
-    float *hostP = nullptr, *hostQ = nullptr;   // caller's [rows x d] arrays (holder path)
-    DevBuf<float> ownP, ownQ;                   // holder path: the library's device copies
     DevBuf<float> Qacc;                         // new item factors of the running iteration
-    float *dP = nullptr, *dQ = nullptr;
-    int64_t P_rows = 0, Q_rows = 0;
-    bool factors_ready = false;
     DevBuf<uint8_t> visited;
     DevBuf<double> colpart, colsum, d_loss;
 
     DevBuf<int64_t> stage_ends;
     DevBuf<int32_t> stage_keys;
     DevBuf<float> stage_vals;
-    const int64_t* d_indptr = nullptr;
-    const int32_t* d_keys = nullptr;
-    const float* d_vals = nullptr;
-    int64_t csr_rows = 0, csr_nnz = 0;
+    CsrBinding csr;
 
-    cudaStream_t stream = nullptr;
-    int num_sms = 132;
+    int apply_options(const JsonOpt& j) override;
 };
 
-namespace {
-
-int plsi_apply_options(bfl_plsi* h, const JsonOpt& j) {
-    h->d = j.integer("d", 20);
-    if (h->d <= 0 || h->d > 512) BFL_FAIL(BFL_ERR_OPTION, "d must be in [1, 512]");
-    h->vdim = (h->d + 3) / 4 * 4;
-    h->seed = (uint32_t)j.integer("random_seed", 0);
-    if (BFL_OK != require_device()) return BFL_ERR_CUDA;
-    int dev = 0;
-    BFL_CUDA(cudaGetDevice(&dev));
-    BFL_CUDA(cudaDeviceGetAttribute(&h->num_sms, cudaDevAttrMultiProcessorCount, dev));
-    if (!h->stream) BFL_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-    if (BFL_OK != h->d_loss.reserve(1)) return BFL_ERR_CUDA;
-    h->opt_set = true;
+int bfl_plsi::apply_options(const JsonOpt& j) {
+    d = j.integer("d", 20);
+    if (d <= 0 || d > 512) BFL_FAIL(BFL_ERR_OPTION, "d must be in [1, 512]");
+    vdim = (d + 3) / 4 * 4;
+    seed = (uint32_t)j.integer("random_seed", 0);
+    int rc = attach_device();
+    if (rc != BFL_OK) return rc;
+    if (BFL_OK != d_loss.reserve(1)) return BFL_ERR_CUDA;
+    opt_set = true;
     return BFL_OK;
 }
+
+namespace {
 
 int grid_for(const bfl_plsi* h, int64_t work, int per_block, int blocks_per_sm) {
     return (int)std::max<int64_t>(1, std::min<int64_t>((work + per_block - 1) / per_block,
@@ -392,12 +379,8 @@ int copy_rows(float* dst, size_t dpitch, const float* src, size_t spitch, int64_
 // holder path: device copies of the caller's [rows x d] arrays, padding columns zeroed
 int adopt_host(bfl_plsi* h, float* P, int32_t P_rows, float* Q, int32_t Q_rows) {
     if (!h || !h->opt_set) BFL_FAIL(BFL_ERR_STATE, "init() must succeed before initialize_model()");
-    if (!P || !Q || P_rows <= 0 || Q_rows <= 0) BFL_FAIL(BFL_ERR_ARG, "bad factor arguments");
-    h->hostP = P; h->hostQ = Q;
-    h->P_rows = P_rows; h->Q_rows = Q_rows;
-    if (BFL_OK != h->ownP.reserve((size_t)P_rows * h->vdim)) return BFL_ERR_CUDA;
-    if (BFL_OK != h->ownQ.reserve((size_t)Q_rows * h->vdim)) return BFL_ERR_CUDA;
-    h->dP = h->ownP.p; h->dQ = h->ownQ.p;
+    int rc = h->mirror_factors(P, P_rows, Q, Q_rows);
+    if (rc != BFL_OK) return rc;
     h->factors_ready = false;
     return alloc_state(h);
 }
@@ -417,27 +400,11 @@ extern "C" {
 
 bfl_plsi_t* bfl_plsi_create(void) { return new (std::nothrow) bfl_plsi(); }
 
-void bfl_plsi_destroy(bfl_plsi_t* h) {
-    if (!h) return;
-    if (h->stream) cudaStreamDestroy(h->stream);
-    delete h;
-}
+void bfl_plsi_destroy(bfl_plsi_t* h) { delete h; }
 
-int bfl_plsi_init(bfl_plsi_t* h, const char* opt_path) {
-    if (!h || !opt_path) BFL_FAIL(BFL_ERR_ARG, "null argument");
-    JsonOpt j;
-    std::string err;
-    if (!j.load(opt_path, &err)) BFL_FAIL(BFL_ERR_OPTION, err);
-    return plsi_apply_options(h, j);
-}
+int bfl_plsi_init(bfl_plsi_t* h, const char* opt_path) { return init_holder(h, opt_path, true); }
 
-int bfl_plsi_init_json(bfl_plsi_t* h, const char* json_text) {
-    if (!h || !json_text) BFL_FAIL(BFL_ERR_ARG, "null argument");
-    JsonOpt j;
-    std::string err;
-    if (!j.parse(json_text, &err)) BFL_FAIL(BFL_ERR_OPTION, "Failed to parse: " + err);
-    return plsi_apply_options(h, j);
-}
+int bfl_plsi_init_json(bfl_plsi_t* h, const char* json_text) { return init_holder(h, json_text, false); }
 
 int bfl_plsi_get_vdim(bfl_plsi_t* h) { return h ? h->vdim : 0; }
 
@@ -546,13 +513,9 @@ int bfl_plsi_release(bfl_plsi_t* h) {
 
 int bfl_plsi_bind_factors_device(bfl_plsi_t* h, float* dP, int64_t P_rows, float* dQ, int64_t Q_rows) {
     if (!h || !h->opt_set) BFL_FAIL(BFL_ERR_STATE, "init() must succeed before binding factors");
-    if (!dP || !dQ || P_rows <= 0 || Q_rows <= 0) BFL_FAIL(BFL_ERR_ARG, "bad factor arguments");
-    if (((uintptr_t)dP | (uintptr_t)dQ) & 15) BFL_FAIL(BFL_ERR_ARG, "device factor pointers must be 16-byte aligned");
-    h->hostP = h->hostQ = nullptr;
-    h->ownP.release(); h->ownQ.release();
-    h->dP = dP; h->dQ = dQ;
-    h->P_rows = P_rows; h->Q_rows = Q_rows;
-    int rc = alloc_state(h);
+    int rc = h->borrow_factors(dP, P_rows, dQ, Q_rows);
+    if (rc != BFL_OK) return rc;
+    rc = alloc_state(h);
     if (rc != BFL_OK) return rc;
     BFL_CUDA(cudaStreamSynchronize(h->stream));
     h->factors_ready = true;
@@ -562,20 +525,18 @@ int bfl_plsi_bind_factors_device(bfl_plsi_t* h, float* dP, int64_t P_rows, float
 int bfl_plsi_bind_csr_device(bfl_plsi_t* h, const int64_t* d_indptr, const int32_t* d_keys, const float* d_vals,
                              int64_t rows, int64_t nnz) {
     if (!h || !h->opt_set) BFL_FAIL(BFL_ERR_STATE, "init() must precede bind_csr");
-    if (!d_indptr || (nnz > 0 && (!d_keys || !d_vals)) || rows <= 0) BFL_FAIL(BFL_ERR_ARG, "bad CSR arguments");
-    h->d_indptr = d_indptr; h->d_keys = d_keys; h->d_vals = d_vals;
-    h->csr_rows = rows; h->csr_nnz = nnz;
-    return BFL_OK;
+    return h->csr.bind(d_indptr, d_keys, d_vals, rows, nnz, true);
 }
 
 int bfl_plsi_update_device(bfl_plsi_t* h, int64_t row_begin, int64_t row_end, double* d_loss, void* stream) {
     if (!h || !h->factors_ready) BFL_FAIL(BFL_ERR_STATE, "factors not bound");
-    if (!h->d_indptr) BFL_FAIL(BFL_ERR_STATE, "no device CSR bound");
-    if (h->csr_rows != h->P_rows) BFL_FAIL(BFL_ERR_STATE, "the bound CSR and P disagree on the number of rows");
-    if (row_begin < 0 || row_end > h->csr_rows || row_end < row_begin) BFL_FAIL(BFL_ERR_ARG, "bad row range");
+    if (!h->csr.indptr) BFL_FAIL(BFL_ERR_STATE, "no device CSR bound");
+    if (h->csr.rows != h->P_rows) BFL_FAIL(BFL_ERR_STATE, "the bound CSR and P disagree on the number of rows");
+    int rc = h->csr.check_range(row_begin, row_end);
+    if (rc != BFL_OK) return rc;
     EmArgs a;
     a.P = h->dP; a.Q = h->dQ; a.Qacc = h->Qacc.p; a.visited = h->visited.p;
-    a.ends = h->d_indptr + row_begin; a.keys = h->d_keys; a.vals = h->d_vals; a.shift = 0;
+    a.ends = h->csr.indptr + row_begin; a.keys = h->csr.keys; a.vals = h->csr.vals; a.shift = 0;
     a.row_begin = row_begin; a.n_rows = row_end - row_begin; a.loss = d_loss; a.d = h->d; a.vdim = h->vdim;
     return launch_em(h, a, (cudaStream_t)stream);
 }

@@ -42,7 +42,7 @@ extern "C" {
 #define BFL_ERR_ARG 4      /* bad argument */
 
 const char* bfl_last_error(void);
-/* library/ABI version and the SM architecture the kernels were compiled for (100) */
+/* library/ABI version and the SM architecture the kernels were compiled for (90) */
 int bfl_abi_version(void);
 int bfl_compiled_sm(void);
 /* number of kernels this library launched since load (bench.py's gpu_launches claim) */

@@ -32,27 +32,46 @@ def test_library_is_sm90_only():
     assert lib.bfl_abi_version() == 1
 
 
+def _holders():
+    from buffalo_b200 import backend
+    return {"als": backend.CuALS, "bpr": lambda: backend.CuSGD("bpr"), "warp": lambda: backend.CuSGD("warp"),
+            "plsi": backend.CuPLSI}
+
+
 def test_no_cpu_fallback():
     import torch
     if torch.cuda.is_available():
         pytest.skip("GPU present")
-    from buffalo_b200 import _cabi, backend
-    obj = backend.CuALS()
-    with pytest.raises(_cabi.BackendError) as e:
-        obj.init({"d": 16})
-    assert "no CPU fallback" in str(e.value)
-    sgd = backend.CuSGD("bpr")
-    with pytest.raises(_cabi.BackendError):
-        sgd.init({"d": 16})
+    from buffalo_b200 import _cabi
+    for kind, make in _holders().items():
+        with pytest.raises(_cabi.BackendError) as e:
+            make().init({"d": 16})
+        assert "no CPU fallback" in str(e.value), kind
 
 
 def test_bad_option_file_returns_false_or_raises():
     # reference: init() returns False on a missing option file (lib/algo.cc:22-34) and the Python
     # layer asserts (buffalo/algo/als.py:43)
-    from buffalo_b200 import backend
-    obj = backend.CuALS()
-    assert obj.init(b"/nonexistent/option.json") is False
-    assert "File not exists" in obj.last_error
+    for kind, make in _holders().items():
+        obj = make()
+        assert obj.init(b"/nonexistent/option.json") is False, kind
+        assert "File not exists" in obj.last_error, kind
+
+
+@pytest.mark.parametrize("kind,opt,msg", [
+    ("als", {"d": 0}, "d must be in [1, 512], got 0"),
+    ("als", {"d": 513}, "d must be in [1, 512], got 513"),
+    ("als", {"d": 16, "optimizer": "eigen_cg"}, "optimizer 'eigen_cg' is not available on the H100 backend"),
+    ("bpr", {"d": 0}, "d must be in [1, 512]"),
+    ("warp", {"d": 600}, "d must be in [1, 512]"),
+    ("warp", {"d": 16, "optimizer": "sgd"}, "optimizer must be adagrad or adam"),
+    ("plsi", {"d": 0}, "d must be in [1, 512]"),
+])
+def test_option_errors_return_false_before_device_check(kind, opt, msg):
+    # option errors come before the device check: they return False with or without a GPU
+    obj = _holders()[kind]()
+    assert obj.init(opt) is False
+    assert msg in obj.last_error
 
 
 def test_product_never_imports_oracle():

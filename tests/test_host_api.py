@@ -260,6 +260,45 @@ def test_early_stopping_and_periodical():
     assert m.periodical(3, 2) and not m.periodical(3, 1) and m.periodical(0, 5)
 
 
+def test_epoch_loop_validation_save_best_and_early_stopping():
+    """The epoch loop every trainer runs: validation every evaluation_period epochs feeds the callback, factors are
+    synced before each validation and save, save-best keeps the lowest loss, early stopping ends the run."""
+    m = _Mock()
+    m.initialize()
+    m.opt.num_iters = 10
+    m.opt.validation = aux.Option({"topk": 5})
+    m.opt.evaluation_on_learning, m.opt.evaluation_period = True, 2
+    m.opt.save_best, m.opt.save_period, m.opt.model_path = True, 1, "best.bin"
+    m.opt.early_stopping_rounds = 2
+    events, calls = [], []
+    m.get_validation_results = lambda: events.append("val") or {"ndcg": 0.25}
+    m.save = lambda path: events.append("save " + path)
+    losses = iter([0.5, 0.4, 0.45, 0.3, 0.35, 0.38, 0.2])
+
+    def one_iteration():
+        events.append("iter")
+        return next(losses)
+    last = m._epoch_loop(one_iteration, lambda: events.append("sync"), lambda i, met: calls.append((i, met)),
+                         "Loss", 1e10)
+    # 0.35 and 0.38 rise twice in a row after 0.3: stop after the sixth epoch
+    assert last == 0.38
+    assert events == ["iter", "sync", "save best.bin",
+                      "iter", "sync", "val", "sync", "save best.bin",
+                      "iter", "sync",
+                      "iter", "sync", "val", "sync", "save best.bin",
+                      "iter", "sync",
+                      "iter", "sync", "val", "sync"]
+    assert calls == [(1, {"train_loss": 0.4, "val_ndcg": 0.25}), (3, {"train_loss": 0.3, "val_ndcg": 0.25}),
+                     (5, {"train_loss": 0.38, "val_ndcg": 0.25})]
+    assert m.validation_result == {"ndcg": 0.25}
+    # the start value of save-best is the trainer's: nothing below it is ever saved
+    events.clear()
+    m.initialize()
+    m.opt.num_iters, m.opt.validation = 2, None
+    assert m._epoch_loop(lambda: 2.0, lambda: None, None, "Loss", 1.0) == 2.0
+    assert events == []
+
+
 def test_ranking_metrics_match_bruteforce(tmp_path):
     rng = np.random.default_rng(0)
     M = scipy.sparse.random(60, 40, density=0.2, random_state=5)
