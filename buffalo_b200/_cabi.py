@@ -114,6 +114,17 @@ PROTOTYPES = {
     "bfl_mm_ingest_split": (C.c_int, [_vp, _vp, _i64, _vp, _vp, _vp]),
     "bfl_mm_ingest_build": (C.c_int, [_vp, C.c_int, _vp, _vp, _vp]),
     "bfl_mm_ingest_stats": (C.c_int, [_vp, _pd, _pi64]),
+    "bfl_stream_ingest_create": (_vp, [_i64, C.c_uint64, _vp, _i32, _i32]),
+    "bfl_stream_ingest_destroy": (None, [_vp]),
+    "bfl_stream_ingest_staging": (C.c_int, [_vp, C.c_int, C.POINTER(_vp)]),
+    "bfl_stream_ingest_load_iid": (C.c_int, [_vp, _vp, _vp, _i64]),
+    "bfl_stream_ingest_feed": (C.c_int, [_vp, C.c_int, _i64, C.c_int]),
+    "bfl_stream_ingest_finish": (C.c_int, [_vp, _pi64, _pi64, C.POINTER(_i32), C.POINTER(_i32), _pi64]),
+    "bfl_stream_ingest_names": (C.c_int, [_vp, _vp, _vp]),
+    "bfl_stream_ingest_split": (C.c_int, [_vp, _i32, C.c_int, _i64, _vp, _i64, C.c_int, _pi64, _pi64]),
+    "bfl_stream_ingest_vali": (C.c_int, [_vp, _vp, _vp, _vp]),
+    "bfl_stream_ingest_build": (C.c_int, [_vp, C.c_int, _vp, _vp, _vp]),
+    "bfl_stream_ingest_stats": (C.c_int, [_vp, _pd, _pi64]),
 }
 
 

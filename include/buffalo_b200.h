@@ -342,6 +342,47 @@ int bfl_mm_ingest_split(bfl_mm_ingest_t* h, const int64_t* sample_idx, int64_t n
 int bfl_mm_ingest_build(bfl_mm_ingest_t* h, int orientation, int64_t* indptr, int32_t* key, float* val);
 int bfl_mm_ingest_stats(bfl_mm_ingest_t* h, double* stage_ms, int64_t* peak_bytes);
 
+/* =====================================================================================
+ * Stream text -> database on the device (DESIGN.md 4.7).  One line per user of item tokens separated by whitespace;
+ * the caller streams the whole file through the handle's two pinned staging buffers.  Tokens are interned in a device
+ * hash table and numbered in first-appearance order (or by an iid list), the (user, item) pairs stay on the device
+ * through the validation split and the CSR builds.
+ *  - create: `block_bytes` per staging buffer; `ascii_ws` bit c set when byte c (< 64) separates tokens (must include
+ *    '\n'); `uspace[n_uspace]` multi-byte whitespace code points, which decline the file; `hash_bits` < 64 truncates
+ *    the token hash (tests: distinct tokens then share keys and the byte comparison must decline the file).
+ *  - load_iid(names, offsets[n + 1], n): the UTF-8 item names, before the first block; a repeated name takes its last
+ *    index, the table is frozen and a token it does not hold declines the file.
+ *  - staging(slot) / feed(slot, n, is_last): as bfl_mm_ingest_*; every block but the last ends with '\n'.  Parsing is
+ *    synchronous; after a decline the remaining blocks are skipped.
+ *  - finish: *num_tokens, *num_lines ('\n' bytes), *num_items, *decline = reason bits (1 bare '\r', 2 invalid UTF-8,
+ *    4 multi-byte whitespace, 8 token missing from the iid list, 16 hash collision, 32 device memory, 64 more than
+ *    2^31 - 2 lines or items; 0: accepted) and *decline_line (smallest 1-based line with reason 1, 2, 4, 8 or 16; -1).
+ *  - names: byte offset from the first fed byte and length of each item's first occurrence (no iid list).
+ *  - split(num_users, method 0 none / 1 newest / 2 sample, newest_n, sample ordinals, as_matrix): holds out the last
+ *    min(newest_n, len - 1) tokens of each session, or the given token ordinals; *n_vali = Counter(held) triples of
+ *    all users, *n_train = distinct (user, item) pairs (as_matrix) or kept tokens; vali copies the triples out.
+ *  - build(orientation): one CSR (END offsets, int32 key, float32 value) into host arrays of num_users resp. num_items
+ *    and n_train entries; matrix: rowwise by (user, item) and colwise by (item, user) with counts as values; stream:
+ *    rowwise only, in session order, value 1.
+ *  - stats: summed device time of H2D, parse, intern, number, split, rowwise CSR, colwise CSR and D2H (stage_ms[8])
+ *    and the high-water mark of the device's default memory pool since create.
+ * ===================================================================================== */
+typedef struct bfl_stream_ingest bfl_stream_ingest_t;
+bfl_stream_ingest_t* bfl_stream_ingest_create(int64_t block_bytes, uint64_t ascii_ws, const int32_t* uspace, int32_t n_uspace,
+                                              int32_t hash_bits);
+void bfl_stream_ingest_destroy(bfl_stream_ingest_t* h);
+int bfl_stream_ingest_staging(bfl_stream_ingest_t* h, int slot, void** host_ptr);
+int bfl_stream_ingest_load_iid(bfl_stream_ingest_t* h, const char* names, const int64_t* offsets, int64_t n);
+int bfl_stream_ingest_feed(bfl_stream_ingest_t* h, int slot, int64_t n, int is_last);
+int bfl_stream_ingest_finish(bfl_stream_ingest_t* h, int64_t* num_tokens, int64_t* num_lines, int32_t* num_items,
+                             int32_t* decline, int64_t* decline_line);
+int bfl_stream_ingest_names(bfl_stream_ingest_t* h, int64_t* offset, int32_t* length);
+int bfl_stream_ingest_split(bfl_stream_ingest_t* h, int32_t num_users, int method, int64_t newest_n, const int64_t* sample_idx,
+                            int64_t n_sample, int as_matrix, int64_t* n_vali, int64_t* n_train);
+int bfl_stream_ingest_vali(bfl_stream_ingest_t* h, int32_t* row, int32_t* col, float* val);
+int bfl_stream_ingest_build(bfl_stream_ingest_t* h, int orientation, int64_t* indptr, int32_t* key, float* val);
+int bfl_stream_ingest_stats(bfl_stream_ingest_t* h, double* stage_ms, int64_t* peak_bytes);
+
 #ifdef __cplusplus
 }
 #endif
