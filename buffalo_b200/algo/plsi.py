@@ -6,6 +6,10 @@ Two feeding modes, same results:
   * chunked: the reference's own protocol -- reset, obj.partial_update(start_x, next_x, indptr, keys, vals) per
     BufferedDataMatrix chunk, normalize, swap (plsi.py:132-160).
 The factor arrays are [rows, d] (plsi.py:107-111: not padded).
+
+With the option `deterministic` (a backend key, false when absent) the new item rows are built by an item pass over
+the colwise CSR before the row pass, without atomics, so a fixed random_seed gives bitwise the same model in either
+feeding mode.  The resident mode then also holds the colwise CSR and the segment partial rows of long items.
 """
 import time
 
@@ -115,11 +119,25 @@ class PLSI(Algo, PLSIOption, Evaluable, Serializable):
         return None
 
     # ---- training -----------------------------------------------------------------------------
+    def _deterministic(self):
+        return bool(self.opt.get("deterministic", False))
+
     def _iterate(self):
-        """The reference protocol: reset, partial_update per rowwise chunk, normalize, swap (plsi.py:132-160)."""
+        """The reference protocol: reset, partial_update per rowwise chunk, normalize, swap (plsi.py:132-160).
+        Deterministic mode sends the colwise chunks through partial_update_items first."""
         self.obj.reset()
         loss_nume, loss_deno = 0.0, 0.0
         feed_t, update_t, updated = 0.0, 0.0, 0
+        if self._deterministic():
+            self.buf.set_group("colwise")
+            for sz in self.buf.fetch_batch():
+                st = time.time()
+                start_x, next_x, indptr, keys, vals = self.buf.get()
+                feed_t += time.time() - st
+                st = time.time()
+                self.obj.partial_update_items(start_x, next_x, indptr, keys, vals)
+                update_t += time.time() - st
+            self.buf.set_group("rowwise")
         for sz in self.buf.fetch_batch():
             st = time.time()
             start_x, next_x, indptr, keys, vals = self.buf.get()
@@ -147,9 +165,12 @@ class PLSI(Algo, PLSIOption, Evaluable, Serializable):
         self.obj.bind_factors(tP, tQ)
         indptr, keys, vals = self._csr_to_device("rowwise", dev)
         self.obj.bind_csr(indptr, keys, vals)
+        deterministic = self._deterministic()
+        if deterministic:
+            self.obj.bind_colwise_csr(*self._csr_to_device("colwise", dev))
         loss_deno = float(np.sum(vals.cpu().numpy(), dtype=np.float64))
         loss = torch.zeros(1, dtype=torch.float64, device=dev)
-        rows = self.P.shape[0]
+        rows, items = self.P.shape[0], self.Q.shape[0]
 
         def sync_back():
             self.P[:] = tP[:, :d].cpu().numpy()
@@ -157,6 +178,8 @@ class PLSI(Algo, PLSIOption, Evaluable, Serializable):
 
         def one_iteration():
             loss.zero_()
+            if deterministic:
+                self.obj.update_items_device(0, items)
             self.obj.update_device(0, rows, loss)
             self.obj.normalize_device(self.opt.alpha1, self.opt.alpha2)
             self.obj.swap_device()
@@ -179,16 +202,30 @@ class PLSI(Algo, PLSIOption, Evaluable, Serializable):
         for name in ("P", "Q"):          # factors replaced or inherited by the user: the backend needs float32 [rows, d]
             setattr(self, name, np.ascontiguousarray(getattr(self, name), dtype=np.float32))
         self.obj.set_model(self.P, self.Q)
-        h = self.data.get_header()
-        # rowwise CSR + factors + the item accumulator
-        need = h["num_nnz"] * 8 + h["num_users"] * (self.vdim * 4 + 9) + h["num_items"] * self.vdim * 8
-        if self._resident_capable(need):
+        deterministic = self._deterministic()
+        resident = self._resident_capable(self._resident_bytes())
+        self.logger.info("pLSI feeding: %s, item rows: %s" % ("resident" if resident else "chunked",
+                                                               "deterministic item pass" if deterministic else "atomics"))
+        if resident:
             loss = self._train_resident(training_callback)
         else:
             loss = self._train_chunked(training_callback)
         ret = {"train_loss": loss}
         ret.update({"val_%s" % k: v for k, v in self.validation_result.items()})
         return ret
+
+    def _resident_bytes(self):
+        """Device bytes of the resident mode: the rowwise CSR, the factors and the item accumulator; in deterministic
+        mode also the colwise CSR, the per-row losses and the partial rows of the segments of long items."""
+        h = self.data.get_header()
+        need = h["num_nnz"] * 8 + h["num_users"] * (self.vdim * 4 + 9) + h["num_items"] * self.vdim * 8
+        if self._deterministic():
+            seg = self.obj.item_segment_len()
+            cind = np.asarray(self.data.get_group("colwise")["indptr"][:], dtype=np.int64)
+            lens = np.diff(cind, prepend=0)
+            segments = int(np.sum((lens[lens > seg] + seg - 1) // seg))
+            need += h["num_nnz"] * 8 + h["num_items"] * 8 + h["num_users"] * 8 + segments * self.vdim * 4
+        return need
 
     def _get_data(self):
         return super()._get_data() + [("opt", self.opt), ("Q", self.Q), ("P", self.P)]

@@ -332,6 +332,19 @@ class CuPLSI(_Holder):
                     "partial_update")
         return loss.value
 
+    def partial_update_items(self, start_x, next_x, indptr, keys, vals):
+        """Deterministic mode: the item pass over one colwise chunk (items [start_x, next_x)), before the rowwise
+        chunks of the same iteration.  Same conventions as partial_update."""
+        _cabi.check(self._lib.bfl_plsi_partial_update_items(self._h, int(start_x), int(next_x),
+                                                            _host(indptr, np.int64, 1, "indptr"),
+                                                            _host(keys, np.int32, 1, "keys"),
+                                                            _host(vals, np.float32, 1, "vals")),
+                    "partial_update_items")
+
+    def item_segment_len(self):
+        """Entries per segment of a long item row in the deterministic item pass."""
+        return self._lib.bfl_plsi_item_segment_len()
+
     def normalize(self, alpha1, alpha2):
         _cabi.check(self._lib.bfl_plsi_normalize(self._h, float(alpha1), float(alpha2)), "normalize")
 
@@ -356,6 +369,20 @@ class CuPLSI(_Holder):
         _cabi.check(self._lib.bfl_plsi_bind_csr_device(self._h, _dev(indptr, "int64", "indptr"),
                                                        _dev(keys, "int32", "keys"), _dev(vals, "float32", "vals"),
                                                        indptr.shape[0], keys.shape[0]), "bind_csr")
+
+    def bind_colwise_csr(self, indptr, keys, vals):
+        """Deterministic mode: the colwise CSR (indptr int64[items] END offsets, keys int32[nnz] user rows,
+        vals float32[nnz]) as torch CUDA tensors, bound after the factors."""
+        self._keep += [indptr, keys, vals]
+        _cabi.check(self._lib.bfl_plsi_bind_colwise_csr_device(self._h, _dev(indptr, "int64", "indptr"),
+                                                               _dev(keys, "int32", "keys"),
+                                                               _dev(vals, "float32", "vals"),
+                                                               indptr.shape[0], keys.shape[0]), "bind_colwise_csr")
+
+    def update_items_device(self, item_begin, item_end, stream=None):
+        """Deterministic mode: the item pass over items [item_begin, item_end), before update_device."""
+        _cabi.check(self._lib.bfl_plsi_update_items_device(self._h, int(item_begin), int(item_end),
+                                                           _stream_ptr(stream)), "update_items_device")
 
     def update_device(self, row_begin, row_end, loss=None, stream=None):
         """loss: optional torch float64 CUDA tensor[1] receiving (+=) -sum v log(norm)."""

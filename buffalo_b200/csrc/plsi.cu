@@ -9,6 +9,11 @@
 // which user rows the pass wrote: a row the pass never reached counts as zero in normalize, as the reference's
 // zeroed accumulator would.
 //
+// Deterministic mode (option `deterministic`): the atomics go.  An item pass over the colwise CSR runs first and
+// builds every new item row with plain stores from the current P and Q (one warp per item, or per fixed segment of a
+// long item, whose partial rows a second kernel adds in segment order); the row pass then runs without the item
+// accumulation, and the loss is per-row fp64 partials summed by a fixed tree.  The same inputs give the same bits.
+//
 // Layout: factor rows have pitch vdim = ceil4(d) on the device; padding columns stay zero.  The holder entry points
 // take the caller's [rows x d] host arrays (plsi.py:107-111 does not pad) and copy with a pitch conversion.
 #include <algorithm>
@@ -24,6 +29,10 @@ namespace {
 
 constexpr float kLatentFloor = 1e-10f;   // plsi.cc:95
 constexpr int kColsumBlocks = 512;       // fixed partial count: the column sums do not depend on the device
+// Entries per segment of a long item row in the deterministic item pass.  A compile-time constant, so the order of
+// every item sum depends on the data only, not on the grid, the SM count or the chunking.
+constexpr int64_t kItemSegment = 4096;
+constexpr int kLossRows = 4096;          // rows per fixed partial of the deterministic loss
 
 __device__ __forceinline__ void red4(float* p, float4 v) { atomicAdd(reinterpret_cast<float4*>(p), v); }
 
@@ -51,12 +60,14 @@ struct EmArgs {
     int64_t row_begin, n_rows;
     double* loss;            // += -sum v * log(norm) (nullable)
     int d, vdim;
+    double* row_loss;        // kDet: row_loss[i] = -sum v * log(norm) of row row_begin + i (nullable)
 };
 
 // One warp per user row.  A row is split into float4 slices; G lanes (a group) cover one entry's slices, NV slices
 // per lane when a row has more than 32 slices, and the 32 / G groups of the warp take different entries.  Keys and
 // values are loaded 32 at a time, coalesced, and broadcast by shuffles; each group keeps U item rows in flight.
-template <int G, int NV, int U>
+// kDet: no item accumulation (the item pass built Qacc) and the loss goes to row_loss instead of an atomic.
+template <int G, int NV, int U, bool kDet = false>
 __global__ void __launch_bounds__(256) plsi_em_kernel(const EmArgs a) {
     constexpr int NG = 32 / G;
     __shared__ double s_loss[8];
@@ -66,6 +77,7 @@ __global__ void __launch_bounds__(256) plsi_em_kernel(const EmArgs a) {
     const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     double lacc = 0.0;
     for (int64_t i = warp0; i < a.n_rows; i += nwarps) {
+        if constexpr (kDet) lacc = 0.0;
         const int64_t x = a.row_begin + i;
         const int64_t beg = (x == 0) ? 0 : a.ends[i - 1];
         const int64_t end = a.ends[i];
@@ -113,13 +125,25 @@ __global__ void __launch_bounds__(256) plsi_em_kernel(const EmArgs a) {
                     // lanes past the chunk's end add zeros to acc and skip the atomics
                     const float w = ok[u] ? v[u] / ps : 0.f;
                     if (ok[u] && gl == 0) lacc -= (double)v[u] * (double)logf(ps);
-                    float* qrow = a.Qacc + (int64_t)c[u] * a.vdim;
+                    if constexpr (kDet) {
+                        // the rounding of the default instantiation (a product, then a sum: its product also
+                        // feeds the atomic, so it is not contracted), spelled out so that no FMA forms here
 #pragma unroll
-                    for (int k = 0; k < NV; ++k) {
-                        const int s = gl + G * k;
-                        const float4 ctb = make_float4(l[k].x * w, l[k].y * w, l[k].z * w, l[k].w * w);
-                        acc[k].x += ctb.x; acc[k].y += ctb.y; acc[k].z += ctb.z; acc[k].w += ctb.w;
-                        if (ok[u] && s < nv4) red4(qrow + 4 * s, ctb);
+                        for (int k = 0; k < NV; ++k) {
+                            acc[k].x = __fadd_rn(acc[k].x, __fmul_rn(l[k].x, w));
+                            acc[k].y = __fadd_rn(acc[k].y, __fmul_rn(l[k].y, w));
+                            acc[k].z = __fadd_rn(acc[k].z, __fmul_rn(l[k].z, w));
+                            acc[k].w = __fadd_rn(acc[k].w, __fmul_rn(l[k].w, w));
+                        }
+                    } else {
+                        float* qrow = a.Qacc + (int64_t)c[u] * a.vdim;
+#pragma unroll
+                        for (int k = 0; k < NV; ++k) {
+                            const int s = gl + G * k;
+                            const float4 ctb = make_float4(l[k].x * w, l[k].y * w, l[k].z * w, l[k].w * w);
+                            acc[k].x += ctb.x; acc[k].y += ctb.y; acc[k].z += ctb.z; acc[k].w += ctb.w;
+                            if (ok[u] && s < nv4) red4(qrow + 4 * s, ctb);
+                        }
                     }
                 }
             }
@@ -138,17 +162,181 @@ __global__ void __launch_bounds__(256) plsi_em_kernel(const EmArgs a) {
             if (g == 0 && s < nv4) *reinterpret_cast<float4*>(prow + 4 * s) = acc[k];
         }
         if (lane == 0) a.visited[x] = 1;
-    }
-    if (a.loss) {
-        lacc = warp_sum_d(lacc);
-        if (lane == 0) s_loss[threadIdx.x >> 5] = lacc;
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            double s = 0.0;
-            for (int w = 0; w < (int)(blockDim.x >> 5); ++w) s += s_loss[w];
-            if (s != 0.0) atomicAdd(a.loss, s);
+        if constexpr (kDet) {
+            if (a.row_loss) {
+                const double r = warp_sum_d(lacc);
+                if (lane == 0) a.row_loss[i] = r;
+            }
         }
     }
+    if constexpr (!kDet) {
+        if (a.loss) {
+            lacc = warp_sum_d(lacc);
+            if (lane == 0) s_loss[threadIdx.x >> 5] = lacc;
+            __syncthreads();
+            if (threadIdx.x == 0) {
+                double s = 0.0;
+                for (int w = 0; w < (int)(blockDim.x >> 5); ++w) s += s_loss[w];
+                if (s != 0.0) atomicAdd(a.loss, s);
+            }
+        }
+    }
+}
+
+struct ItemArgs {
+    const float* P;          // [P_rows x vdim] current user rows (read only during the pass)
+    const float* Q;          // [Q_rows x vdim] current item rows (read only)
+    float* Qacc;             // [Q_rows x vdim] new item rows, written with plain stores
+    float* part;             // [n_segs x vdim] partial rows of the long items' segments
+    const int64_t* ends;     // ends[i] = end offset of item item_begin + i; ends[-1] is valid when item_begin > 0
+    const int32_t* keys;     // entry j (a user row) at keys[j - shift]
+    const float* vals;
+    int64_t shift;
+    int64_t item_begin, n_items;
+    const int32_t* seg;      // segment tasks: seg[2s] = item, seg[2s + 1] = segment index within the item
+    int64_t n_segs;
+    int d, vdim;
+};
+
+// Deterministic item pass: one warp per item of at most kItemSegment entries (tasks [0, n_items)) and one per segment
+// of a longer item (tasks [n_items, n_items + n_segs)).  The lane layout, latent4 and the norm reduction are those of
+// plsi_em_kernel, with Q[item] held in registers and the user rows gathered, so every norm is bitwise the one the row
+// pass computes for the same entry.  Each group sums its entries in order, the groups fold by a fixed butterfly, and
+// the row goes out with plain stores: to Qacc, or to the segment's partial row.
+template <int G, int NV, int U>
+__global__ void __launch_bounds__(256) plsi_item_kernel(const ItemArgs a) {
+    constexpr int NG = 32 / G;
+    const int lane = threadIdx.x & 31, g = lane / G, gl = lane % G;
+    const int nv4 = a.vdim >> 2;
+    const int64_t warp0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t task = warp0; task < a.n_items + a.n_segs; task += nwarps) {
+        int64_t item, beg, end;
+        float* out;
+        if (task < a.n_items) {
+            item = a.item_begin + task;
+            beg = (item == 0) ? 0 : a.ends[task - 1];
+            end = a.ends[task];
+            if (end - beg > kItemSegment) continue;          // its segments write partial rows
+            out = a.Qacc + item * a.vdim;
+        } else {
+            const int64_t s = task - a.n_items;
+            item = a.seg[2 * s];
+            const int64_t t = item - a.item_begin;
+            beg = ((item == 0) ? 0 : a.ends[t - 1]) + (int64_t)a.seg[2 * s + 1] * kItemSegment;
+            end = min(a.ends[t], beg + kItemSegment);
+            out = a.part + s * a.vdim;
+        }
+        const float* qrow = a.Q + item * a.vdim;
+        float4 q[NV], acc[NV];
+#pragma unroll
+        for (int k = 0; k < NV; ++k) {
+            const int s = gl + G * k;
+            q[k] = s < nv4 ? ld4(qrow + 4 * s) : make_float4(0.f, 0.f, 0.f, 0.f);
+            acc[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+        for (int64_t base = beg; base < end; base += 32) {
+            const int cnt = (int)min((int64_t)32, end - base);
+            const int my_key = lane < cnt ? __ldg(a.keys + (base + lane - a.shift)) : 0;
+            const float my_val = lane < cnt ? __ldg(a.vals + (base + lane - a.shift)) : 0.f;
+            for (int t = 0; t < cnt; t += NG * U) {
+                int r[U];
+                float v[U];
+                bool ok[U];
+                float4 p[U][NV];
+#pragma unroll
+                for (int u = 0; u < U; ++u) {
+                    const int e = t + u * NG + g;
+                    ok[u] = e < cnt;
+                    r[u] = __shfl_sync(FULL, my_key, e & 31);
+                    v[u] = __shfl_sync(FULL, my_val, e & 31);
+#pragma unroll
+                    for (int k = 0; k < NV; ++k) {
+                        const int s = gl + G * k;
+                        p[u][k] = (ok[u] && s < nv4) ? ld4(a.P + (int64_t)r[u] * a.vdim + 4 * s)
+                                                     : make_float4(0.f, 0.f, 0.f, 0.f);
+                    }
+                }
+#pragma unroll
+                for (int u = 0; u < U; ++u) {
+                    float4 l[NV];
+                    float ps = 0.f;
+#pragma unroll
+                    for (int k = 0; k < NV; ++k) {
+                        l[k] = latent4(p[u][k], q[k], 4 * (gl + G * k), a.d);
+                        ps += (l[k].x + l[k].y) + (l[k].z + l[k].w);
+                    }
+#pragma unroll
+                    for (int o = G / 2; o > 0; o >>= 1) ps += __shfl_xor_sync(FULL, ps, o);
+                    const float w = ok[u] ? v[u] / ps : 0.f;
+#pragma unroll
+                    for (int k = 0; k < NV; ++k) {
+                        acc[k].x = __fadd_rn(acc[k].x, __fmul_rn(l[k].x, w));
+                        acc[k].y = __fadd_rn(acc[k].y, __fmul_rn(l[k].y, w));
+                        acc[k].z = __fadd_rn(acc[k].z, __fmul_rn(l[k].z, w));
+                        acc[k].w = __fadd_rn(acc[k].w, __fmul_rn(l[k].w, w));
+                    }
+                }
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < NV; ++k) {
+#pragma unroll
+            for (int o = G; o < 32; o <<= 1) {
+                acc[k].x += __shfl_xor_sync(FULL, acc[k].x, o);
+                acc[k].y += __shfl_xor_sync(FULL, acc[k].y, o);
+                acc[k].z += __shfl_xor_sync(FULL, acc[k].z, o);
+                acc[k].w += __shfl_xor_sync(FULL, acc[k].w, o);
+            }
+            const int s = gl + G * k;
+            if (g == 0 && s < nv4) *reinterpret_cast<float4*>(out + 4 * s) = acc[k];
+        }
+    }
+}
+
+// Long items: Qacc[item] = the item's segment partial rows added in segment order.  One thread per (item, column);
+// long_off[L] .. long_off[L + 1] are item long_items[L]'s rows of `part`.
+__global__ void __launch_bounds__(256) plsi_item_combine_kernel(const float* part, const int32_t* long_items,
+                                                                const int64_t* long_off, int64_t n_long, int vdim,
+                                                                float* Qacc) {
+    const int64_t n = n_long * vdim;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t L = e / vdim;
+        const int col = (int)(e % vdim);
+        const int64_t s0 = long_off[L], s1 = long_off[L + 1];
+        float t = part[s0 * vdim + col];
+        for (int64_t s = s0 + 1; s < s1; ++s) t += part[s * vdim + col];
+        Qacc[(int64_t)long_items[L] * vdim + col] = t;
+    }
+}
+
+// Deterministic loss, stage 1: the row losses of fixed ranges of kLossRows rows, each summed by a fixed tree.
+__global__ void __launch_bounds__(256) plsi_loss_partial_kernel(const double* row_loss, int64_t n, double* part) {
+    __shared__ double s[256];
+    const int64_t lo = (int64_t)blockIdx.x * kLossRows, hi = min(n, lo + kLossRows);
+    double t = 0.0;
+    for (int64_t i = lo + threadIdx.x; i < hi; i += 256) t += row_loss[i];
+    s[threadIdx.x] = t;
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+        if ((int)threadIdx.x < o) s[threadIdx.x] += s[threadIdx.x + o];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) part[blockIdx.x] = s[0];
+}
+
+// Deterministic loss, stage 2 (one CTA of 256 threads): the partials by the same tree, added into *loss.
+__global__ void __launch_bounds__(256) plsi_loss_final_kernel(const double* part, int64_t nblk, double* loss) {
+    __shared__ double s[256];
+    double t = 0.0;
+    for (int64_t i = threadIdx.x; i < nblk; i += 256) t += part[i];
+    s[threadIdx.x] = t;
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+        if ((int)threadIdx.x < o) s[threadIdx.x] += s[threadIdx.x + o];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) *loss += s[0];
 }
 
 // P rows: (row + alpha1) / sum(row + alpha1) over the d real columns (plsi.cc:115-119).  A row the last pass did not
@@ -264,6 +452,30 @@ __global__ void __launch_bounds__(256) plsi_init_kernel(float* F, int64_t rows, 
 
 }  // namespace
 
+// The items of a colwise CSR longer than one segment, ascending: items[L] owns segments off[L] .. off[L + 1] - 1, and
+// seg holds the (item, segment index) pair of every segment.
+struct LongItems {
+    std::vector<int32_t> items;
+    std::vector<int64_t> off{0};
+    std::vector<int32_t> seg;
+    // indptr: HOST global END offsets; items [item_begin, item_end)
+    void build(const int64_t* indptr, int64_t item_begin, int64_t item_end) {
+        items.clear(); seg.clear(); off.assign(1, 0);
+        for (int64_t x = item_begin; x < item_end; ++x) {
+            const int64_t len = indptr[x] - (x == 0 ? 0 : indptr[x - 1]);
+            if (len <= kItemSegment) continue;
+            const int64_t n = (len + kItemSegment - 1) / kItemSegment;
+            items.push_back((int32_t)x);
+            for (int64_t k = 0; k < n; ++k) {
+                seg.push_back((int32_t)x);
+                seg.push_back((int32_t)k);
+            }
+            off.push_back(off.back() + n);
+        }
+    }
+    int64_t n_segs() const { return off.back(); }
+};
+
 // the Holder's hostP/hostQ are the caller's [rows x d] arrays (holder path), ownP/ownQ the library's device copies
 struct bfl_plsi : Holder {
     uint32_t seed = 0;
@@ -277,6 +489,17 @@ struct bfl_plsi : Holder {
     DevBuf<float> stage_vals;
     CsrBinding csr;
 
+    // deterministic mode
+    bool deterministic = false;
+    bool rows_done = false;                     // a row pass ran since the last reset / swap: P is overwritten
+    DevBuf<double> row_loss, loss_part;
+    DevBuf<float> seg_part;                     // partial rows of the long items' segments
+    CsrBinding ccsr;                            // the bound colwise CSR (rows == Q_rows)
+    LongItems bound_long;                       // its long items, built once per binding
+    DevBuf<int32_t> d_seg, d_long_items;        // the long-item table on the device (bound or the chunk's)
+    DevBuf<int64_t> d_long_off;
+    bool long_bound = false;                    // the device table is bound_long (a chunk's replaces it)
+
     int apply_options(const JsonOpt& j) override;
 };
 
@@ -285,6 +508,7 @@ int bfl_plsi::apply_options(const JsonOpt& j) {
     if (d <= 0 || d > 512) BFL_FAIL(BFL_ERR_OPTION, "d must be in [1, 512]");
     vdim = (d + 3) / 4 * 4;
     seed = (uint32_t)j.integer("random_seed", 0);
+    deterministic = j.flag("deterministic", false);
     int rc = attach_device();
     if (rc != BFL_OK) return rc;
     if (BFL_OK != d_loss.reserve(1)) return BFL_ERR_CUDA;
@@ -303,6 +527,7 @@ int grid_for(const bfl_plsi* h, int64_t work, int per_block, int blocks_per_sm) 
 int reset_acc(bfl_plsi* h, cudaStream_t st) {
     BFL_CUDA(cudaMemsetAsync(h->Qacc.p, 0, sizeof(float) * (size_t)h->Q_rows * h->vdim, st));
     BFL_CUDA(cudaMemsetAsync(h->visited.p, 0, (size_t)h->P_rows, st));
+    h->rows_done = false;
     return BFL_OK;
 }
 
@@ -311,22 +536,97 @@ int alloc_state(bfl_plsi* h) {
     if (BFL_OK != h->visited.reserve((size_t)h->P_rows)) return BFL_ERR_CUDA;
     if (BFL_OK != h->colpart.reserve((size_t)kColsumBlocks * h->vdim)) return BFL_ERR_CUDA;
     if (BFL_OK != h->colsum.reserve((size_t)h->vdim)) return BFL_ERR_CUDA;
+    if (h->deterministic) {
+        if (BFL_OK != h->row_loss.reserve((size_t)std::max<int64_t>(1, h->P_rows))) return BFL_ERR_CUDA;
+        if (BFL_OK != h->loss_part.reserve((size_t)std::max<int64_t>(1, (h->P_rows + kLossRows - 1) / kLossRows)))
+            return BFL_ERR_CUDA;
+    }
     return reset_acc(h, h->stream);
 }
 
-int launch_em(bfl_plsi* h, const EmArgs& a, cudaStream_t st) {
+// The deterministic row pass at 64 < d <= 128 keeps 3 item rows in flight, not 4: with 4, ptxas holds that
+// instantiation to 64 registers and spills.  U does not change any sum: group g still takes entries g, g + NG, ...
+// in order, so the rows and the loss are those of U = 4 bit for bit.
+template <bool kDet>
+void launch_em_kernel(int nv4, int grid, const EmArgs& a, cudaStream_t st) {
+    if (nv4 <= 1) plsi_em_kernel<1, 1, 2, kDet><<<grid, 256, 0, st>>>(a);
+    else if (nv4 <= 2) plsi_em_kernel<2, 1, 2, kDet><<<grid, 256, 0, st>>>(a);
+    else if (nv4 <= 4) plsi_em_kernel<4, 1, 2, kDet><<<grid, 256, 0, st>>>(a);
+    else if (nv4 <= 8) plsi_em_kernel<8, 1, 2, kDet><<<grid, 256, 0, st>>>(a);
+    else if (nv4 <= 16) plsi_em_kernel<16, 1, 4, kDet><<<grid, 256, 0, st>>>(a);
+    else if (nv4 <= 32) plsi_em_kernel<32, 1, kDet ? 3 : 4, kDet><<<grid, 256, 0, st>>>(a);
+    else if (nv4 <= 64) plsi_em_kernel<32, 2, 4, kDet><<<grid, 256, 0, st>>>(a);
+    else plsi_em_kernel<32, 4, 2, kDet><<<grid, 256, 0, st>>>(a);
+}
+
+// The row pass.  Deterministic mode: no item accumulation, and the loss (when a.loss is set) is the row losses of
+// the range summed by the fixed tree of plsi_loss_*_kernel, added into a.loss[0] by one thread.
+int launch_em(bfl_plsi* h, EmArgs a, cudaStream_t st) {
+    h->rows_done = true;
     if (a.n_rows <= 0) return BFL_OK;
     const int grid = grid_for(h, a.n_rows, 8, 16);
     const int nv4 = h->vdim / 4;
-    if (nv4 <= 1) plsi_em_kernel<1, 1, 2><<<grid, 256, 0, st>>>(a);
-    else if (nv4 <= 2) plsi_em_kernel<2, 1, 2><<<grid, 256, 0, st>>>(a);
-    else if (nv4 <= 4) plsi_em_kernel<4, 1, 2><<<grid, 256, 0, st>>>(a);
-    else if (nv4 <= 8) plsi_em_kernel<8, 1, 2><<<grid, 256, 0, st>>>(a);
-    else if (nv4 <= 16) plsi_em_kernel<16, 1, 4><<<grid, 256, 0, st>>>(a);
-    else if (nv4 <= 32) plsi_em_kernel<32, 1, 4><<<grid, 256, 0, st>>>(a);
-    else if (nv4 <= 64) plsi_em_kernel<32, 2, 4><<<grid, 256, 0, st>>>(a);
-    else plsi_em_kernel<32, 4, 2><<<grid, 256, 0, st>>>(a);
+    if (!h->deterministic) {
+        a.row_loss = nullptr;
+        launch_em_kernel<false>(nv4, grid, a, st);
+        BFL_LAUNCHED();
+        return BFL_OK;
+    }
+    a.row_loss = a.loss ? h->row_loss.p : nullptr;
+    launch_em_kernel<true>(nv4, grid, a, st);
     BFL_LAUNCHED();
+    if (a.loss) {
+        const int64_t nblk = (a.n_rows + kLossRows - 1) / kLossRows;
+        plsi_loss_partial_kernel<<<(unsigned)nblk, 256, 0, st>>>(h->row_loss.p, a.n_rows, h->loss_part.p);
+        BFL_LAUNCHED();
+        plsi_loss_final_kernel<<<1, 256, 0, st>>>(h->loss_part.p, nblk, a.loss);
+        BFL_LAUNCHED();
+    }
+    return BFL_OK;
+}
+
+// uploads a long-item table and sizes the segment partial rows for it
+int upload_long(bfl_plsi* h, const LongItems& t, cudaStream_t st) {
+    const size_t n_long = t.items.size();
+    if (BFL_OK != h->d_long_off.reserve(n_long + 1)) return BFL_ERR_CUDA;
+    BFL_CUDA(cudaMemcpyAsync(h->d_long_off.p, t.off.data(), sizeof(int64_t) * (n_long + 1), cudaMemcpyHostToDevice, st));
+    if (n_long == 0) return BFL_OK;
+    if (BFL_OK != h->d_long_items.reserve(n_long)) return BFL_ERR_CUDA;
+    if (BFL_OK != h->d_seg.reserve(t.seg.size())) return BFL_ERR_CUDA;
+    if (BFL_OK != h->seg_part.reserve((size_t)t.n_segs() * h->vdim)) return BFL_ERR_CUDA;
+    BFL_CUDA(cudaMemcpyAsync(h->d_long_items.p, t.items.data(), sizeof(int32_t) * n_long, cudaMemcpyHostToDevice, st));
+    BFL_CUDA(cudaMemcpyAsync(h->d_seg.p, t.seg.data(), sizeof(int32_t) * t.seg.size(), cudaMemcpyHostToDevice, st));
+    return BFL_OK;
+}
+
+// The item pass over items [a.item_begin, a.item_begin + a.n_items); long items la .. lb - 1 of the uploaded table t
+// are the range's.
+int launch_items(bfl_plsi* h, ItemArgs a, const LongItems& t, int64_t la, int64_t lb, cudaStream_t st) {
+    if (h->rows_done)
+        BFL_FAIL(BFL_ERR_STATE, "the item pass must run before the row pass of the same iteration (P is overwritten)");
+    if (a.n_items <= 0) return BFL_OK;
+    const int64_t s0 = t.off[la], s1 = t.off[lb];
+    a.seg = h->d_seg.p + 2 * s0;
+    a.n_segs = s1 - s0;
+    a.part = h->seg_part.p + s0 * h->vdim;
+    a.d = h->d;
+    a.vdim = h->vdim;
+    const int grid = grid_for(h, a.n_items + a.n_segs, 8, 16);
+    const int nv4 = h->vdim / 4;
+    if (nv4 <= 1) plsi_item_kernel<1, 1, 2><<<grid, 256, 0, st>>>(a);
+    else if (nv4 <= 2) plsi_item_kernel<2, 1, 2><<<grid, 256, 0, st>>>(a);
+    else if (nv4 <= 4) plsi_item_kernel<4, 1, 2><<<grid, 256, 0, st>>>(a);
+    else if (nv4 <= 8) plsi_item_kernel<8, 1, 2><<<grid, 256, 0, st>>>(a);
+    else if (nv4 <= 16) plsi_item_kernel<16, 1, 4><<<grid, 256, 0, st>>>(a);
+    else if (nv4 <= 32) plsi_item_kernel<32, 1, 4><<<grid, 256, 0, st>>>(a);
+    else if (nv4 <= 64) plsi_item_kernel<32, 2, 4><<<grid, 256, 0, st>>>(a);
+    else plsi_item_kernel<32, 4, 2><<<grid, 256, 0, st>>>(a);
+    BFL_LAUNCHED();
+    if (lb > la) {
+        plsi_item_combine_kernel<<<grid_for(h, (lb - la) * h->vdim, 256, 16), 256, 0, st>>>(
+            h->seg_part.p, h->d_long_items.p + la, h->d_long_off.p + la, lb - la, h->vdim, a.Qacc);
+        BFL_LAUNCHED();
+    }
     return BFL_OK;
 }
 
@@ -383,6 +683,29 @@ int adopt_host(bfl_plsi* h, float* P, int32_t P_rows, float* Q, int32_t Q_rows) 
     if (rc != BFL_OK) return rc;
     h->factors_ready = false;
     return alloc_state(h);
+}
+
+// Copies one host chunk, major rows [start_x, next_x) of a CSR with global END offsets `indptr`, into the staging
+// buffers: the chunk's end offsets preceded by the previous row's end when start_x > 0 (*lead = 1), its keys and
+// values.  *beg is the chunk's first global entry.
+int stage_chunk(bfl_plsi* h, int64_t start_x, int64_t next_x, const int64_t* indptr, const int32_t* keys,
+                const float* vals, int64_t* beg, int64_t* lead) {
+    *beg = start_x == 0 ? 0 : indptr[start_x - 1];
+    const int64_t n = indptr[next_x - 1] - *beg;
+    if (n > 0 && (!keys || !vals)) BFL_FAIL(BFL_ERR_ARG, "null keys / vals");
+    cudaStream_t st = h->stream;
+    *lead = start_x > 0 ? 1 : 0;
+    const int64_t n_ends = next_x - start_x + *lead;
+    if (BFL_OK != h->stage_ends.reserve((size_t)n_ends)) return BFL_ERR_CUDA;
+    BFL_CUDA(cudaMemcpyAsync(h->stage_ends.p, indptr + start_x - *lead, sizeof(int64_t) * n_ends, cudaMemcpyHostToDevice,
+                             st));
+    if (n > 0) {
+        if (BFL_OK != h->stage_keys.reserve((size_t)n)) return BFL_ERR_CUDA;
+        if (BFL_OK != h->stage_vals.reserve((size_t)n)) return BFL_ERR_CUDA;
+        BFL_CUDA(cudaMemcpyAsync(h->stage_keys.p, keys, sizeof(int32_t) * n, cudaMemcpyHostToDevice, st));
+        BFL_CUDA(cudaMemcpyAsync(h->stage_vals.p, vals, sizeof(float) * n, cudaMemcpyHostToDevice, st));
+    }
+    return BFL_OK;
 }
 
 int download(bfl_plsi* h) {
@@ -452,27 +775,16 @@ int bfl_plsi_partial_update(bfl_plsi_t* h, int32_t start_x, int32_t next_x, cons
     if (!h || !h->factors_ready || !h->hostP) BFL_FAIL(BFL_ERR_STATE, "initialize_model() must precede partial_update()");
     if (next_x == start_x) return BFL_OK;
     if (start_x < 0 || next_x > h->P_rows || next_x < start_x || !indptr) BFL_FAIL(BFL_ERR_ARG, "bad chunk arguments");
-    const int64_t beg = start_x == 0 ? 0 : indptr[start_x - 1];
-    const int64_t n = indptr[next_x - 1] - beg;
-    if (n > 0 && (!keys || !vals)) BFL_FAIL(BFL_ERR_ARG, "null keys / vals");
+    int64_t beg = 0, lead = 0;
+    int rc = stage_chunk(h, start_x, next_x, indptr, keys, vals, &beg, &lead);
+    if (rc != BFL_OK) return rc;
     cudaStream_t st = h->stream;
-    // the chunk's end offsets, preceded by the previous row's end when start_x > 0
-    const int64_t lead = start_x > 0 ? 1 : 0;
-    const int64_t n_ends = next_x - start_x + lead;
-    if (BFL_OK != h->stage_ends.reserve((size_t)n_ends)) return BFL_ERR_CUDA;
-    BFL_CUDA(cudaMemcpyAsync(h->stage_ends.p, indptr + start_x - lead, sizeof(int64_t) * n_ends, cudaMemcpyHostToDevice, st));
-    if (n > 0) {
-        if (BFL_OK != h->stage_keys.reserve((size_t)n)) return BFL_ERR_CUDA;
-        if (BFL_OK != h->stage_vals.reserve((size_t)n)) return BFL_ERR_CUDA;
-        BFL_CUDA(cudaMemcpyAsync(h->stage_keys.p, keys, sizeof(int32_t) * n, cudaMemcpyHostToDevice, st));
-        BFL_CUDA(cudaMemcpyAsync(h->stage_vals.p, vals, sizeof(float) * n, cudaMemcpyHostToDevice, st));
-    }
     BFL_CUDA(cudaMemsetAsync(h->d_loss.p, 0, sizeof(double), st));
     EmArgs a;
     a.P = h->dP; a.Q = h->dQ; a.Qacc = h->Qacc.p; a.visited = h->visited.p;
     a.ends = h->stage_ends.p + lead; a.keys = h->stage_keys.p; a.vals = h->stage_vals.p; a.shift = beg;
     a.row_begin = start_x; a.n_rows = next_x - start_x; a.loss = h->d_loss.p; a.d = h->d; a.vdim = h->vdim;
-    int rc = launch_em(h, a, st);
+    rc = launch_em(h, a, st);
     if (rc != BFL_OK) return rc;
     double out = 0.0;
     BFL_CUDA(cudaMemcpyAsync(&out, h->d_loss.p, sizeof(double), cudaMemcpyDeviceToHost, st));
@@ -480,6 +792,34 @@ int bfl_plsi_partial_update(bfl_plsi_t* h, int32_t start_x, int32_t next_x, cons
     if (loss) *loss = out;
     return BFL_OK;
 }
+
+int bfl_plsi_partial_update_items(bfl_plsi_t* h, int32_t start_x, int32_t next_x, const int64_t* indptr,
+                                  const int32_t* keys, const float* vals) {
+    if (!h || !h->factors_ready || !h->hostP)
+        BFL_FAIL(BFL_ERR_STATE, "initialize_model() must precede partial_update_items()");
+    if (!h->deterministic) BFL_FAIL(BFL_ERR_STATE, "the item pass needs the deterministic option");
+    if (h->rows_done)
+        BFL_FAIL(BFL_ERR_STATE, "the item pass must run before the row pass of the same iteration (P is overwritten)");
+    if (next_x == start_x) return BFL_OK;
+    if (start_x < 0 || next_x > h->Q_rows || next_x < start_x || !indptr) BFL_FAIL(BFL_ERR_ARG, "bad chunk arguments");
+    int64_t beg = 0, lead = 0;
+    int rc = stage_chunk(h, start_x, next_x, indptr, keys, vals, &beg, &lead);
+    if (rc != BFL_OK) return rc;
+    cudaStream_t st = h->stream;
+    LongItems t;
+    t.build(indptr, start_x, next_x);
+    if (BFL_OK != (rc = upload_long(h, t, st))) return rc;
+    h->long_bound = false;
+    ItemArgs a;
+    a.P = h->dP; a.Q = h->dQ; a.Qacc = h->Qacc.p;
+    a.ends = h->stage_ends.p + lead; a.keys = h->stage_keys.p; a.vals = h->stage_vals.p; a.shift = beg;
+    a.item_begin = start_x; a.n_items = next_x - start_x;
+    if (BFL_OK != (rc = launch_items(h, a, t, 0, (int64_t)t.items.size(), st))) return rc;
+    BFL_CUDA(cudaStreamSynchronize(st));   // the staging buffers are reused by the next chunk
+    return BFL_OK;
+}
+
+int bfl_plsi_item_segment_len(void) { return (int)kItemSegment; }
 
 int bfl_plsi_normalize(bfl_plsi_t* h, float alpha1, float alpha2) {
     if (!h || !h->factors_ready) BFL_FAIL(BFL_ERR_STATE, "initialize_model() must precede normalize()");
@@ -495,6 +835,7 @@ int bfl_plsi_swap(bfl_plsi_t* h) {
     std::swap(h->ownQ.p, h->Qacc.p);
     std::swap(h->ownQ.cap, h->Qacc.cap);
     h->dQ = h->ownQ.p;
+    h->rows_done = false;
     return download(h);
 }
 
@@ -504,6 +845,12 @@ int bfl_plsi_release(bfl_plsi_t* h) {
     h->ownP.release(); h->ownQ.release(); h->Qacc.release(); h->visited.release();
     h->colpart.release(); h->colsum.release();
     h->stage_ends.release(); h->stage_keys.release(); h->stage_vals.release();
+    h->row_loss.release(); h->loss_part.release(); h->seg_part.release();
+    h->d_seg.release(); h->d_long_items.release(); h->d_long_off.release();
+    h->ccsr = CsrBinding();
+    h->bound_long = LongItems();
+    h->long_bound = false;
+    h->rows_done = false;
     h->hostP = h->hostQ = nullptr;
     h->dP = h->dQ = nullptr;
     h->P_rows = h->Q_rows = 0;
@@ -551,6 +898,46 @@ int bfl_plsi_swap_device(bfl_plsi_t* h, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     BFL_CUDA(cudaMemcpyAsync(h->dQ, h->Qacc.p, sizeof(float) * (size_t)h->Q_rows * h->vdim, cudaMemcpyDeviceToDevice, st));
     return reset_acc(h, st);
+}
+
+int bfl_plsi_bind_colwise_csr_device(bfl_plsi_t* h, const int64_t* d_indptr, const int32_t* d_keys,
+                                     const float* d_vals, int64_t rows, int64_t nnz) {
+    if (!h || !h->factors_ready) BFL_FAIL(BFL_ERR_STATE, "factors must be bound before the colwise CSR");
+    if (!h->deterministic) BFL_FAIL(BFL_ERR_STATE, "the colwise CSR serves the deterministic option only");
+    if (rows != h->Q_rows) BFL_FAIL(BFL_ERR_ARG, "the colwise CSR must have Q_rows rows");
+    int rc = h->ccsr.bind(d_indptr, d_keys, d_vals, rows, nnz, true);
+    if (rc != BFL_OK) return rc;
+    // the long-item table, from a host copy of the END offsets
+    std::vector<int64_t> ends((size_t)rows);
+    BFL_CUDA(cudaMemcpyAsync(ends.data(), d_indptr, sizeof(int64_t) * (size_t)rows, cudaMemcpyDeviceToHost, h->stream));
+    BFL_CUDA(cudaStreamSynchronize(h->stream));
+    h->bound_long.build(ends.data(), 0, rows);
+    if (BFL_OK != (rc = upload_long(h, h->bound_long, h->stream))) return rc;
+    BFL_CUDA(cudaStreamSynchronize(h->stream));
+    h->long_bound = true;
+    return BFL_OK;
+}
+
+int bfl_plsi_update_items_device(bfl_plsi_t* h, int64_t item_begin, int64_t item_end, void* stream) {
+    if (!h || !h->factors_ready) BFL_FAIL(BFL_ERR_STATE, "factors not bound");
+    if (!h->deterministic) BFL_FAIL(BFL_ERR_STATE, "the item pass needs the deterministic option");
+    if (!h->ccsr.indptr) BFL_FAIL(BFL_ERR_STATE, "no colwise CSR bound");
+    if (h->ccsr.rows != h->Q_rows) BFL_FAIL(BFL_ERR_STATE, "the bound colwise CSR and Q disagree on the number of rows");
+    int rc = h->ccsr.check_range(item_begin, item_end);
+    if (rc != BFL_OK) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (!h->long_bound) {
+        if (BFL_OK != (rc = upload_long(h, h->bound_long, st))) return rc;
+        h->long_bound = true;
+    }
+    const std::vector<int32_t>& li = h->bound_long.items;
+    const int64_t la = std::lower_bound(li.begin(), li.end(), (int32_t)item_begin) - li.begin();
+    const int64_t lb = std::lower_bound(li.begin(), li.end(), (int32_t)item_end) - li.begin();
+    ItemArgs a;
+    a.P = h->dP; a.Q = h->dQ; a.Qacc = h->Qacc.p;
+    a.ends = h->ccsr.indptr + item_begin; a.keys = h->ccsr.keys; a.vals = h->ccsr.vals; a.shift = 0;
+    a.item_begin = item_begin; a.n_items = item_end - item_begin;
+    return launch_items(h, a, h->bound_long, la, lb, st);
 }
 
 }  // extern "C"

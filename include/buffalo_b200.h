@@ -250,6 +250,16 @@ int bfl_plsi_reset(bfl_plsi_t* h);
  * the chunk (fp64). */
 int bfl_plsi_partial_update(bfl_plsi_t* h, int32_t start_x, int32_t next_x, const int64_t* indptr,
                             const int32_t* keys, const float* vals, double* loss);
+/* Deterministic mode (option "deterministic": true): the same inputs give bitwise the same factors and loss.  An
+ * iteration is reset -> partial_update_items per colwise chunk -> partial_update per rowwise chunk -> normalize ->
+ * swap.  The item pass builds the new item rows from the colwise CSR and the CURRENT P and Q, so it must come before
+ * the row pass of its iteration (after it: BFL_ERR_STATE); partial_update then leaves the item rows alone, and its
+ * *loss is a fixed-order sum.  HOST buffers with the conventions of partial_update: `indptr` is the global colwise
+ * end-offset array, `keys` (user rows) / `vals` the chunk starting at item start_x.  Without the option: BFL_ERR_STATE. */
+int bfl_plsi_partial_update_items(bfl_plsi_t* h, int32_t start_x, int32_t next_x, const int64_t* indptr,
+                                  const int32_t* keys, const float* vals);
+/* entries per segment of a long item row in the deterministic item pass (a compile-time constant) */
+int bfl_plsi_item_segment_len(void);
 /* CPLSI::normalize(alpha1, alpha2) (plsi.cc:108-125): alpha1 /= d, alpha2 /= num_items, then every P row
  * (+alpha1) and every Q column (+alpha2) is divided by its sum.  Column sums are fp64 and deterministic. */
 int bfl_plsi_normalize(bfl_plsi_t* h, float alpha1, float alpha2);
@@ -263,8 +273,16 @@ int bfl_plsi_bind_factors_device(bfl_plsi_t* h, float* dP, int64_t P_rows, float
 /* the rowwise CSR (rows == P_rows) */
 int bfl_plsi_bind_csr_device(bfl_plsi_t* h, const int64_t* d_indptr, const int32_t* d_keys, const float* d_vals,
                              int64_t rows, int64_t nnz);
-/* update rows [row_begin, row_end); adds -sum v log(norm) into d_loss[0] (device double, may be NULL) */
+/* update rows [row_begin, row_end); adds -sum v log(norm) into d_loss[0] (device double, may be NULL).  In
+ * deterministic mode the row pass leaves the item rows alone and the loss is a fixed-order sum over the range. */
 int bfl_plsi_update_device(bfl_plsi_t* h, int64_t row_begin, int64_t row_end, double* d_loss, void* stream);
+/* deterministic mode: the colwise CSR (rows == Q_rows, else BFL_ERR_ARG), bound after the factors.  Its END offsets
+ * are read once here to list the items longer than one segment and to size their partial rows. */
+int bfl_plsi_bind_colwise_csr_device(bfl_plsi_t* h, const int64_t* d_indptr, const int32_t* d_keys,
+                                     const float* d_vals, int64_t rows, int64_t nnz);
+/* deterministic mode: the item pass over items [item_begin, item_end) of the colwise CSR; runs before
+ * bfl_plsi_update_device in each iteration (after it: BFL_ERR_STATE until swap_device) */
+int bfl_plsi_update_items_device(bfl_plsi_t* h, int64_t item_begin, int64_t item_end, void* stream);
 int bfl_plsi_normalize_device(bfl_plsi_t* h, float alpha1, float alpha2, void* stream);
 /* copy the new item factors into dQ and zero the accumulator for the next iteration (no separate reset) */
 int bfl_plsi_swap_device(bfl_plsi_t* h, void* stream);
