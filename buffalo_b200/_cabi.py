@@ -77,6 +77,8 @@ PROTOTYPES = {
     "bfl_sgd_epoch": (C.c_int, [_vp]),
     "bfl_sgd_current_lr": (_d, [_vp]),
     "bfl_sgd_read_stats": (C.c_int, [_vp, _pd, _pi64]),
+    "bfl_sgd_reduce_items_device": (C.c_int, [_vp, _vp]),
+    "bfl_sgd_segment_len": (C.c_int, []),
     # PLSI
     "bfl_plsi_create": (_vp, []),
     "bfl_plsi_destroy": (None, [_vp]),

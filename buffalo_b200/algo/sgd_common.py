@@ -54,6 +54,9 @@ class SGDTrainerMixin(object):
 
     def _prepare_train(self):
         indptr, _, batch_size = self.buf.get_indptrs()
+        # option `deterministic` (a backend key, false when absent): gradient sums in a fixed order, bitwise repeatable
+        self.logger.info("gradient accumulation: %s" % ("deterministic (fixed-order user and item passes)"
+                                                        if self.opt.get("deterministic", False) else "atomics"))
         # a second train() (or user-replaced factors) arrives at width d: re-pad to vdim like bpr.py's _prepare_train,
         # the native side copies rows * vdim floats in and out
         self.P, self.Q = self._pad(self.P), self._pad(self.Q)

@@ -295,6 +295,17 @@ class CuSGD(_Holder):
         _cabi.check(self._lib.bfl_sgd_read_stats(self._h, C.byref(loss), C.byref(n)), "read_stats")
         return loss.value, n.value
 
+    def reduce_items_device(self, stream=None):
+        """Deterministic mode: adds the item sums of the samples recorded since the last call to the Q / Qb gradient
+        accumulators and the WARP loss terms to the running loss.  update_parameters does it first; call it to read
+        (or all-reduce) an epoch's accumulators before the optimizer step."""
+        _cabi.check(self._lib.bfl_sgd_reduce_items_device(self._h, _stream_ptr(stream)), "reduce_items_device")
+
+    @staticmethod
+    def segment_len():
+        """Samples / item entries per segment of the deterministic user and item sums."""
+        return _cabi.lib().bfl_sgd_segment_len()
+
 
 class CuPLSI(_Holder):
     """pLSI backend (CyPLSI, buffalo/algo/_plsi.pyx:13-57).  Holder methods take the [rows, d] host arrays of

@@ -215,6 +215,13 @@ int bfl_sgd_set_trace_device(bfl_sgd_t* h, int32_t* d_trials, int32_t* d_negs);
 int bfl_sgd_epoch(bfl_sgd_t* h);
 double bfl_sgd_current_lr(bfl_sgd_t* h);
 int bfl_sgd_read_stats(bfl_sgd_t* h, double* loss_sum, int64_t* num_updates);
+/* Deterministic mode (option `deterministic`): the item pass over the samples recorded since the last one -- adds every
+ * item's gradient sum to the Q / Qb accumulators in the fixed order and the WARP loss terms to the running loss sum.
+ * update_parameters runs it first, so it is only needed to read the epoch's accumulators before the optimizer step
+ * (or to all-reduce them across ranks).  BFL_ERR_STATE without the option. */
+int bfl_sgd_reduce_items_device(bfl_sgd_t* h, void* stream);
+/* samples / item entries per segment of the deterministic user and item sums */
+int bfl_sgd_segment_len(void);
 
 /* ======================================================================================
  * PLSI -- replaces CyPLSI (buffalo/algo/_plsi.pyx:13-57 -> plsi::CPLSI, lib/algo_impl/plsi/plsi.cc)
