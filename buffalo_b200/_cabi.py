@@ -104,6 +104,13 @@ PROTOTYPES = {
     # evaluation top-k
     "bfl_topk_device": (C.c_int, [_vp, _i64, C.c_int, _vp, _i64, C.c_int, _vp, C.c_int, C.c_int, _vp, _vp, _vp]),
     "bfl_topk_host": (C.c_int, [_vp, _i64, C.c_int, _vp, _i64, C.c_int, _vp, C.c_int, C.c_int, _vp, _vp]),
+    # validation metrics
+    "bfl_eval_unsorted_rows_device": (C.c_int, [_vp, _vp, _i64, _vp, _vp]),
+    "bfl_eval_topk_masked_device": (C.c_int, [_vp, _i64, C.c_int, _vp, _i64, C.c_int, _vp, C.c_int, C.c_int, _vp, _vp,
+                                              _vp, _vp, _vp]),
+    "bfl_eval_ranking_terms_device": (C.c_int, [_vp, _i64, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp]),
+    "bfl_eval_score_terms_device": (C.c_int, [_vp, _vp, _vp, C.c_int, C.c_int, _vp, _vp, _vp, _i64, _vp, _vp]),
+    "bfl_eval_sum_device": (C.c_int, [_vp, _i64, C.c_int, _vp, _vp]),
     # ingest helpers
     "bfl_csr_from_triples_device": (C.c_int, [_vp, _vp, _vp, _i64, _i32, _i32, C.c_int, _vp, _vp, _vp, _vp]),
     "bfl_csr_from_triples_host": (C.c_int, [_vp, _vp, _vp, _i64, _i32, _i32, C.c_int, _vp, _vp, _vp]),

@@ -17,6 +17,7 @@ from buffalo_b200.backend import CuALS
 from buffalo_b200.data.base import Data
 from buffalo_b200.data.buffered_data import BufferedDataMatrix
 from buffalo_b200.evaluate import Evaluable
+from buffalo_b200.evaluate.device import EvalModel
 
 inited_CUALS = True
 
@@ -81,6 +82,9 @@ class ALS(Algo, ALSOption, Evaluable, Serializable):
 
     def _get_feature(self, index, group="item"):
         return {"item": self.Q, "user": self.P}[group][index] if group in ("item", "user") else None
+
+    def _device_eval_model(self):
+        return EvalModel(self.P, self.Q, None, None, False)
 
     # ---- training -----------------------------------------------------------------------------
     def _get_buffer(self):

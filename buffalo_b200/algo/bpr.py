@@ -8,6 +8,7 @@ from buffalo_b200.algo.sgd_common import SGDTrainerMixin
 from buffalo_b200.backend import CuSGD
 from buffalo_b200.data.base import Data
 from buffalo_b200.evaluate import Evaluable
+from buffalo_b200.evaluate.device import EvalModel
 
 inited_CUBPR = True
 
@@ -96,6 +97,10 @@ class BPRMF(SGDTrainerMixin, Algo, BPRMFOption, Evaluable, Serializable):
 
     def _get_feature(self, index, group="item"):
         return {"item": self.Q, "user": self.P}[group][index] if group in ("item", "user") else None
+
+    def _device_eval_model(self):
+        # ranking adds Qb only with use_bias (_get_topk_recommendation); _get_scores always adds it
+        return EvalModel(self.P, self.Q, self.Qb if self.opt.get("use_bias") else None, self.Qb, False)
 
     def _get_data(self):
         return super()._get_data() + [("opt", self.opt), ("Q", self.Q), ("Qb", self.Qb), ("P", self.P)]

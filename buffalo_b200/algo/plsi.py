@@ -21,6 +21,7 @@ from buffalo_b200.backend import CuPLSI
 from buffalo_b200.data.base import Data
 from buffalo_b200.data.buffered_data import BufferedDataMatrix
 from buffalo_b200.evaluate import Evaluable
+from buffalo_b200.evaluate.device import EvalModel
 
 
 class PLSI(Algo, PLSIOption, Evaluable, Serializable):
@@ -117,6 +118,9 @@ class PLSI(Algo, PLSIOption, Evaluable, Serializable):
         elif group == "user":
             return self.P[index]
         return None
+
+    def _device_eval_model(self):
+        return EvalModel(self.P, self.Q, None, None, False)
 
     # ---- training -----------------------------------------------------------------------------
     def _deterministic(self):

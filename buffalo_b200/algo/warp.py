@@ -4,6 +4,7 @@ import numpy as np
 
 from buffalo_b200.algo.bpr import BPRMF
 from buffalo_b200.algo.options import _WARP, WARPOption
+from buffalo_b200.evaluate.device import EvalModel
 
 
 class WARP(BPRMF):
@@ -67,6 +68,9 @@ class WARP(BPRMF):
         if self._l2():
             return {(r, c): -((self.P[r] - self.Q[c]) ** 2).sum() for r, c in row_col_pairs}
         return {(r, c): self.P[r].dot(self.Q[c]) for r, c in row_col_pairs}
+
+    def _device_eval_model(self):
+        return EvalModel(self.P, self.Q, None, None, self._l2())
 
     def _get_scores(self, row, col):
         if self._l2():

@@ -451,6 +451,87 @@ def topk_device(queries, items, item_bias, k, stream=None):
     return idx, val
 
 
+def csr_from_triples_device(major, minor, vals, num_major, num_minor, sort_minor=True, stream=None):
+    """(indptr_end int64, key int32, val float32) torch CUDA tensors of one orientation from int32 major / minor and
+    float32 vals CUDA tensors, through the device radix sort (bfl_csr_from_triples_device)."""
+    import torch
+    n, dev = int(major.shape[0]), major.device
+    indptr = torch.empty(int(num_major), dtype=torch.int64, device=dev)
+    key = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
+    val = torch.empty(max(n, 1), dtype=torch.float32, device=dev)
+    _cabi.check(_cabi.lib().bfl_csr_from_triples_device(
+        _dev(major, "int32", "major") if n else None, _dev(minor, "int32", "minor") if n else None,
+        _dev(vals, "float32", "vals") if n else None, n, int(num_major), int(max(num_minor, 1)), int(bool(sort_minor)),
+        indptr.data_ptr(), key.data_ptr(), val.data_ptr(), _stream_ptr(stream)), "bfl_csr_from_triples_device")
+    return indptr, key[:n], val[:n]
+
+
+def eval_unsorted_rows(indptr, keys, stream=None):
+    """Number of rows of a device CSR (END offsets) whose keys are not non-decreasing; synchronises."""
+    import torch
+    count = torch.zeros(1, dtype=torch.int64, device=indptr.device)
+    _cabi.check(_cabi.lib().bfl_eval_unsorted_rows_device(_dev(indptr, "int64", "indptr"), _dev(keys, "int32", "keys"),
+                                                          indptr.shape[0], count.data_ptr(), _stream_ptr(stream)),
+                "bfl_eval_unsorted_rows_device")
+    return int(count.item())
+
+
+def eval_topk_masked(queries, items, item_bias, k, seen_indptr, seen_keys, seen_row, stream=None):
+    """int32 [nq, k] device tensor: per query, the k best items (scores of bfl_topk_device) outside seen row
+    seen_row[q] of the device CSR (seen_indptr END offsets, sorted seen_keys); -1 pads."""
+    import torch
+    nq = queries.shape[0]
+    idx = torch.empty((nq, int(k)), dtype=torch.int32, device=queries.device)
+    _cabi.check(_cabi.lib().bfl_eval_topk_masked_device(
+        _dev(queries, "float32", "queries"), nq, queries.stride(0), _dev(items, "float32", "items"), items.shape[0],
+        items.stride(0), None if item_bias is None else _dev(item_bias, "float32", "bias"),
+        int(min(queries.shape[1], items.shape[1])), int(k), _dev(seen_indptr, "int64", "seen_indptr"),
+        _dev(seen_keys, "int32", "seen_keys"), _dev(seen_row, "int32", "seen_row"), idx.data_ptr(), _stream_ptr(stream)),
+        "bfl_eval_topk_masked_device")
+    return idx
+
+
+def eval_ranking_terms(ranked, users, seen_indptr, seen_row, gt_indptr, gt_keys, gains, ideal, num_items, terms,
+                       stream=None):
+    """Fills the float64 [nq, 6] device tensor `terms` with the per-row ranking terms of bfl_eval_ranking_terms_device."""
+    nq, k = ranked.shape
+    if terms.shape != (nq, 6):
+        raise ValueError("terms must be [%d, 6], got %s" % (nq, tuple(terms.shape)))
+    _cabi.check(_cabi.lib().bfl_eval_ranking_terms_device(
+        _dev(ranked, "int32", "ranked"), nq, k, _dev(users, "int32", "users"), _dev(seen_indptr, "int64", "seen_indptr"),
+        _dev(seen_row, "int32", "seen_row"), _dev(gt_indptr, "int64", "gt_indptr"), _dev(gt_keys, "int32", "gt_keys"),
+        _dev(gains, "float64", "gains"), _dev(ideal, "float64", "ideal"), int(num_items), _dev(terms, "float64", "terms"),
+        _stream_ptr(stream)), "bfl_eval_ranking_terms_device")
+
+
+EVAL_SCORE_MODES = {"dot": 0, "dot_bias": 1, "l2": 2}
+
+
+def eval_score_terms(P, Q, Qb, mode, rows, cols, vals, stream=None):
+    """float64 [n, 2] device tensor of (err^2, |err|) per held-out triple (bfl_eval_score_terms_device); P, Q rows of
+    the same width, mode one of EVAL_SCORE_MODES."""
+    import torch
+    if P.shape[1] != Q.shape[1]:
+        raise ValueError("P and Q must have the same width (got %d, %d)" % (P.shape[1], Q.shape[1]))
+    n = rows.shape[0]
+    terms = torch.empty((n, 2), dtype=torch.float64, device=P.device)
+    _cabi.check(_cabi.lib().bfl_eval_score_terms_device(
+        _dev(P, "float32", "P"), _dev(Q, "float32", "Q"), None if Qb is None else _dev(Qb, "float32", "Qb"), P.shape[1],
+        EVAL_SCORE_MODES[mode], _dev(rows, "int32", "rows"), _dev(cols, "int32", "cols"), _dev(vals, "float32", "vals"), n,
+        terms.data_ptr(), _stream_ptr(stream)), "bfl_eval_score_terms_device")
+    return terms
+
+
+def eval_sum(terms, stream=None):
+    """Column sums (float64 numpy array) of a float64 [n, width <= 8] device tensor, in a fixed order."""
+    import torch
+    out = torch.empty(terms.shape[1], dtype=torch.float64, device=terms.device)
+    _cabi.check(_cabi.lib().bfl_eval_sum_device(_dev(terms, "float64", "terms") if terms.shape[0] else None,
+                                                terms.shape[0], terms.shape[1], out.data_ptr(), _stream_ptr(stream)),
+                "bfl_eval_sum_device")
+    return out.cpu().numpy()
+
+
 def csr_from_triples_host(major, minor, vals, num_major, num_minor, sort_minor=True):
     """(indptr_end int64, key int32, val float32) of one orientation through the hand-written device radix sort
     (csrc/ingest.cu: bfl_csr_from_triples_host)."""

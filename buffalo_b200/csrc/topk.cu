@@ -5,21 +5,13 @@
 //                       keeps the scores in shared memory and radix-selects the slice's k best per query;
 //   topk_merge_kernel : per query, radix-selects the k best of the slices' candidates and orders them with a
 //                       shared-memory bitonic sort on (score descending, item index ascending) -- deterministic ties.
-#include "bfl_common.cuh"
+#include "topk_common.cuh"
 
 using namespace bfl;
 
 namespace {
 
-constexpr int TK_THREADS = 256;
-constexpr int TK_SLICE = 4096;
 constexpr int TK_QB = 4;
-constexpr int TK_KMAX = 4096;
-
-__device__ __forceinline__ uint32_t ord_of(float f) {
-    const uint32_t u = __float_as_uint(f);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);   // larger float <=> larger unsigned
-}
 
 struct SelScratch {
     unsigned int hist[256];
@@ -113,49 +105,12 @@ __global__ void __launch_bounds__(TK_THREADS) topk_slice_kernel(const float* __r
     float* scores = tk_smem;                       // [TK_QB][TK_SLICE]
     float* qv = scores + TK_QB * TK_SLICE;         // [TK_QB][dpad]
     __shared__ SelScratch sc;
-    const int dpad = (d + 3) & ~3;
-    const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
     const int slice = blockIdx.x;
     const int64_t q0 = (int64_t)blockIdx.y * TK_QB;
     const int nqb = (int)min((long long)TK_QB, (long long)(nq - q0));
     const int64_t i0 = (int64_t)slice * TK_SLICE;
     const int ni = (int)min((long long)TK_SLICE, (long long)(n_items - i0));
-    for (int e = tid; e < TK_QB * dpad; e += TK_THREADS) {
-        const int qi = e / dpad, c = e - qi * dpad;
-        qv[e] = (qi < nqb && c < d) ? Qr[(q0 + qi) * ldq + c] : 0.f;
-    }
-    __syncthreads();
-    const bool vec = (ldi & 3) == 0 && (d & 3) == 0;
-    for (int it = w; it < ni; it += TK_THREADS / 32) {
-        const float* row = It + (i0 + it) * ldi;
-        float acc[TK_QB];
-#pragma unroll
-        for (int qi = 0; qi < TK_QB; ++qi) acc[qi] = 0.f;
-        if (vec) {
-            for (int c = lane * 4; c < d; c += 128) {
-                const float4 v = __ldg(reinterpret_cast<const float4*>(row + c));
-#pragma unroll
-                for (int qi = 0; qi < TK_QB; ++qi) {
-                    const float4 x = *reinterpret_cast<const float4*>(qv + qi * dpad + c);
-                    acc[qi] = fmaf(v.x, x.x, fmaf(v.y, x.y, fmaf(v.z, x.z, fmaf(v.w, x.w, acc[qi]))));
-                }
-            }
-        } else {
-            for (int c = lane; c < d; c += 32) {
-                const float v = __ldg(row + c);
-#pragma unroll
-                for (int qi = 0; qi < TK_QB; ++qi) acc[qi] = fmaf(v, qv[qi * dpad + c], acc[qi]);
-            }
-        }
-#pragma unroll
-        for (int qi = 0; qi < TK_QB; ++qi) acc[qi] = warp_sum(acc[qi]);
-        if (lane == 0) {
-            const float b = bias ? bias[i0 + it] : 0.f;
-#pragma unroll
-            for (int qi = 0; qi < TK_QB; ++qi) scores[qi * TK_SLICE + it] = acc[qi] + b;
-        }
-    }
-    __syncthreads();
+    topk_score_slice<TK_QB>(Qr, q0, nqb, ldq, It, i0, ni, ldi, bias, d, qv, scores);
     for (int qi = 0; qi < nqb; ++qi) {
         const size_t o = ((size_t)(q0 + qi) * nslices + slice) * k;
         block_select(scores + qi * TK_SLICE, nullptr, (int)i0, ni, k, cand_v + o, cand_i + o, sc);

@@ -34,10 +34,34 @@ class Evaluable(object):
     def get_validation_results(self):
         if not self.opt.validation or not self.data.has_group("vali"):
             return
+        model = self._device_eval_route()
         res = {}
-        res.update(self._evaluate_ranking_metrics())
-        res.update(self._evaluate_score_metrics())
+        if model is None:
+            res.update(self._evaluate_ranking_metrics())
+            res.update(self._evaluate_score_metrics())
+            return res
+        from buffalo_b200.evaluate.device import Evaluation
+        if model.l2:   # ranking by 1 - |p - q|^2 has no device top-k: host ranking, device score metrics
+            res.update(self._evaluate_ranking_metrics())
+        ev = Evaluation(self.data, model, max_users=self.opt.get("_b200_eval_batch"))
+        if not model.l2:
+            res.update(ev.ranking(self.opt.validation.topk, self.opt.validation.eval_samples))
+        res.update(ev.scores())
         return res
+
+    def _device_eval_route(self):
+        """The EvalModel of the device path (evaluate/device.py), or None for the host path: the device path needs a
+        trainer that provides _device_eval_model, 0 < topk <= 4096, a GPU, and the private option _b200_device_eval
+        not False."""
+        hook = getattr(self, "_device_eval_model", None)
+        topk = self.opt.validation.get("topk")
+        if hook is None or self.opt.get("_b200_device_eval") is False or not isinstance(topk, (int, np.integer)) \
+                or not 0 < topk <= 4096:
+            return None
+        from buffalo_b200 import backend
+        if not backend.device_available():
+            return None
+        return hook()
 
     def get_topk(self, scores, k, sorted=True, num_threads=4):
         scores = np.asarray(scores)

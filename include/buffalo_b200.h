@@ -309,6 +309,36 @@ int bfl_topk_host(const float* queries, int64_t nq, int ldq, const float* items,
                   const float* item_bias /* nullable */, int d, int k, int32_t* out_idx, float* out_val);
 
 /* =====================================================================================
+ * Validation metrics on the device (DESIGN.md 4.8): the device path of Evaluable.get_validation_results
+ * (buffalo/evaluate/base.py:44-148).  Device pointers, stream-ordered.  A "seen" CSR (END offsets, int32 keys, every
+ * row non-decreasing) holds training rows; seen_row[q] names the row of query q.  The held-out CSR is indexed by user.
+ *  - unsorted_rows: *d_count (device u64) = number of rows whose keys are not non-decreasing.
+ *  - topk_masked: per query q, the k best items (score = queries[q] . items^T (+ item_bias), bitwise the scores of
+ *    bfl_topk_device for the same arguments) among the items not in seen row seen_row[q]; score descending, then item
+ *    ascending; -1 pads when fewer than k such items exist.  k <= 4096, n_items < 2^31.
+ *  - ranking_terms: per query, from its ranked list (d_ranked [nq x k]) and held-out row of user d_users[q], the fp64
+ *    terms (ndcg, ap / min(n_pos, k), accuracy, auc / (n_pos * n_neg), counted, no-negative) into d_terms [nq x 6];
+ *    a query whose seen row is empty gets zeros.  d_gains / d_ideal: the host's 1 / log2(j + 2) and its prefix sums.
+ *  - score_terms: per held-out triple, score = mode 0 (P[r] * Q[c]).sum(), 1 the same + Qb[c], 2 1 - ((P[r] - Q[c])^2).sum()
+ *    in NumPy's float32 order (rows of `width` floats), err = score - val in fp64: d_terms [n x 2] = (err^2, |err|).
+ *  - sum: column sums of d_terms [n x width] (width <= 8) into d_out[width], in a fixed order.
+ * ===================================================================================== */
+int bfl_eval_unsorted_rows_device(const int64_t* d_indptr, const int32_t* d_keys, int64_t rows,
+                                  unsigned long long* d_count, void* stream);
+int bfl_eval_topk_masked_device(const float* d_queries, int64_t nq, int ldq, const float* d_items, int64_t n_items,
+                                int ldi, const float* d_item_bias /* nullable */, int d, int k,
+                                const int64_t* d_seen_indptr, const int32_t* d_seen_keys, const int32_t* d_seen_row,
+                                int32_t* d_out_idx, void* stream);
+int bfl_eval_ranking_terms_device(const int32_t* d_ranked, int64_t nq, int k, const int32_t* d_users,
+                                  const int64_t* d_seen_indptr, const int32_t* d_seen_row, const int64_t* d_gt_indptr,
+                                  const int32_t* d_gt_keys, const double* d_gains, const double* d_ideal,
+                                  int64_t num_items, double* d_terms, void* stream);
+int bfl_eval_score_terms_device(const float* d_P, const float* d_Q, const float* d_Qb /* mode 1 */, int width, int mode,
+                                const int32_t* d_rows, const int32_t* d_cols, const float* d_vals, int64_t n,
+                                double* d_terms, void* stream);
+int bfl_eval_sum_device(const double* d_terms, int64_t n, int width, double* d_out, void* stream);
+
+/* =====================================================================================
  * Ingest helpers (SURVEY.md 8(f-1), 8(f-4)).
  * CSR of one orientation from (major, minor, value) triples, the sort/compress stage of
  * MatrixMarket.create -> _sort_and_compressed_binarization (buffalo/data/mm.py:236-279,
