@@ -165,7 +165,12 @@ class ALS(Algo, ALSOption, Evaluable, Serializable):
                 setattr(self, name, G)
         self.obj.initialize_model(self.P, self.Q)
         h = self.data.get_header()
+        # option `deterministic` (a backend key, false when absent): bitwise repeatable factors and loss on one GPU
+        det = bool(self.opt.get("deterministic", False))
+        self.logger.info("split rows and loss: %s" % ("deterministic (ordered chunk sums)" if det else "atomics"))
         need = 2 * h["num_nnz"] * 8 + (h["num_users"] + h["num_items"]) * (self.vdim * 4 + 8)
+        if det:
+            need += self.deterministic_bytes(h["num_users"], h["num_items"], self.opt.get("_b200_det_scratch_mb", 0))
         rmse = self._train_resident(training_callback) if self._resident_capable(need) else self._train_chunked(training_callback)
         if self.opt.d < self.vdim:            # als.py:191-193
             self.P = np.ascontiguousarray(self.P[:, :self.opt.d])
@@ -173,6 +178,14 @@ class ALS(Algo, ALSOption, Evaluable, Serializable):
         ret = {"train_loss": rmse}
         ret.update({"val_%s" % k: v for k, v in self.validation_result.items()})
         return ret
+
+    @staticmethod
+    def deterministic_bytes(num_users, num_items, scratch_mb=0):
+        """Upper bound of the device memory the deterministic mode adds: 16 B of loss terms per row of the longer axis,
+        and the scratch budget of one batch of split rows (scratch_mb, fractions allowed, or when 0 the backend's cap
+        of 2 GiB).  The backend takes min(free / 4, 2 GiB) and allocates only what the split rows need (0.97 GB at C2),
+        so near the residency limit this bound can choose the chunked feed where the resident one would have fitted."""
+        return 16 * max(num_users, num_items) + (int(scratch_mb * (1 << 20)) if scratch_mb else 2 << 30)
 
     def _get_data(self):
         return super()._get_data() + [("opt", self.opt), ("Q", self.Q), ("P", self.P)]

@@ -19,6 +19,9 @@ struct bfl_als : Holder {
     int tc_min_class = 2; // first row-length class (als_fast.cuh) solved by the tensor-core kernel (rows of <= 64 nnz stay on
                           // the SIMT classes 0, 1: an epilogue per row costs more than their whole SIMT solve; measured 400 vs 411 ms)
     int64_t sub_chunk_nnz = 16ll << 20;   // host-pointer path: entries per pipelined sub-chunk of one partial_update call
+    // split-row chunk matrices and the training loss summed in a fixed order instead of with atomics: the same factors,
+    // CSR, options and feed give bitwise the same P, Q and loss on every run (one GPU)
+    bool deterministic = false;
 
     // CSR per axis: bound device CSR (device path), or just own_indptr (host-pointer path)
     DevBuf<int64_t> own_indptr[2];
@@ -34,6 +37,8 @@ struct bfl_als : Holder {
     DevBuf<float> gram_part;  // partials of the two-stage Gram
     DevBuf<float> yui;        // generic ialspp scratch
     DevBuf<double> d_loss;    // 2 doubles
+    DevBuf<double> loss_rows; // deterministic: (numerator, denominator) terms per row of the axis being updated
+    DevBuf<double> loss_part; // deterministic: the loss tree's partials, one pair per kLossRows rows
     FastCache fast_cache;     // row-length bins of the tuned path, keyed by (indptr, row range)
     // tensor-core path (als_tc.cuh): max|Y| (noted by precompute, which reads the whole opposite factor anyway) and
     // max|v| of the launch -> power-of-two operand scale, all on the device
@@ -76,6 +81,11 @@ int bfl_als::apply_options(const JsonOpt& j) {
     tc_min_class = std::max(0, std::min(7, j.integer("_b200_tc_min_class", 2)));
     sub_chunk_nnz = (int64_t)j.number("_b200_sub_chunk_nnz", (double)(16ll << 20));
     if (sub_chunk_nnz < 1) BFL_FAIL(BFL_ERR_OPTION, "_b200_sub_chunk_nnz must be positive");
+    deterministic = j.flag("deterministic", false);
+    // deterministic split rows: scratch budget of one batch of long rows (0: from the free device memory)
+    const double det_mb = j.number("_b200_det_scratch_mb", 0.0);
+    if (det_mb < 0) BFL_FAIL(BFL_ERR_OPTION, "_b200_det_scratch_mb must not be negative");
+    fast_cache.det_budget = (size_t)(det_mb * (double)(1 << 20));
     std::string optimizer = j.string("optimizer", "manual_cg");
     if (d >= 128) optimizer = "ialspp";  // als.cc:46
     if (optimizer == "llt") optimizer_code = 0;
@@ -131,23 +141,27 @@ int gram(bfl_als* h, const float* F, int64_t rows, cudaStream_t st) {
     return BFL_OK;
 }
 
+// det_loss: a.loss takes per-row terms (the kernels' DET instantiations)
 template <int NC>
-int launch_generic(bfl_als* h, const AlsArgs& a, int64_t nrows, cudaStream_t st) {
+int launch_generic(bfl_als* h, const AlsArgs& a, int64_t nrows, bool det_loss, cudaStream_t st) {
     int grid = (int)std::min<int64_t>((nrows + GEN_WARPS - 1) / GEN_WARPS, (int64_t)h->num_sms * 8);
     if (grid < 1) grid = 1;
-    if (h->optimizer_code == 8)
-        als_ialspp_warp_kernel<NC><<<grid, GEN_WARPS * 32, 0, st>>>(a);
-    else
-        als_cg_warp_kernel<NC><<<grid, GEN_WARPS * 32, 0, st>>>(a);
+    if (h->optimizer_code == 8) {
+        if (det_loss) als_ialspp_warp_kernel<NC, true><<<grid, GEN_WARPS * 32, 0, st>>>(a);
+        else als_ialspp_warp_kernel<NC><<<grid, GEN_WARPS * 32, 0, st>>>(a);
+    } else {
+        if (det_loss) als_cg_warp_kernel<NC, true><<<grid, GEN_WARPS * 32, 0, st>>>(a);
+        else als_cg_warp_kernel<NC><<<grid, GEN_WARPS * 32, 0, st>>>(a);
+    }
     BFL_LAUNCHED();
     return BFL_OK;
 }
 
 // Solve rows [row_begin,row_end) of axis with keys/vals device buffers whose element 0 is global
-// offset `shift`.  chunk_nnz = number of entries those rows span.
-int solve_rows(bfl_als* h, int axis, int64_t row_begin, int64_t row_end, const int32_t* keys, const float* vals,
-               int64_t shift, int64_t chunk_nnz, double* d_loss, cudaStream_t st) {
-    if (row_end <= row_begin) return BFL_OK;
+// offset `shift`.  chunk_nnz = number of entries those rows span.  d_loss: the two sums, or (deterministic mode) the
+// per-row terms indexed by absolute row.
+int launch_row_solves(bfl_als* h, int axis, int64_t row_begin, int64_t row_end, const int32_t* keys, const float* vals,
+                      int64_t shift, int64_t chunk_nnz, double* d_loss, cudaStream_t st) {
     AlsArgs a;
     a.X = axis == 0 ? h->dP : h->dQ;
     a.Y = axis == 0 ? h->dQ : h->dP;
@@ -176,6 +190,7 @@ int solve_rows(bfl_als* h, int axis, int64_t row_begin, int64_t row_end, const i
     a.n_peer = h->n_peer[axis];
     for (int i = 0; i < BFL_MAX_PEERS; ++i) a.peerX[i] = i < a.n_peer ? h->peers[axis][i] : nullptr;
     a.tc_scales = nullptr;
+    const bool det_loss = h->deterministic && a.loss && a.compute_loss;
     int64_t nrows = row_end - row_begin;
     if (h->tc_on) {
         // max|v| of this launch's values (a resident array is scanned once), then the operand scale -- device only
@@ -204,7 +219,8 @@ int solve_rows(bfl_als* h, int axis, int64_t row_begin, int64_t row_end, const i
             // the split-row mode reads it once and pays 2 x 256 KB of scratch traffic per row instead
             splitmin = 6;
         }
-        int rc = fast_als_launch(a, h->fast_cache, h->num_sms, st, &left, &nleft, tcmin, splitmin, h->kernel_mode == 4 ? 1 : 0);
+        int rc = fast_als_launch(a, h->fast_cache, h->num_sms, st, &left, &nleft, tcmin, splitmin, h->kernel_mode == 4 ? 1 : 0,
+                                 h->deterministic);
         if (rc != BFL_OK || nleft == 0) return rc;
         // rows longer than the tuned kernels accept go through the generic kernel
         a.row_list = left;
@@ -216,9 +232,14 @@ int solve_rows(bfl_als* h, int axis, int64_t row_begin, int64_t row_end, const i
     if (h->optimizer_code == 0 || h->optimizer_code == 1) {
         const size_t smem = ((size_t)h->d * (h->d + 1) + 2 * h->d + (size_t)DIRECT_NB * h->d) * sizeof(float);
         if (smem > 220 * 1024) BFL_FAIL(BFL_ERR_OPTION, "llt/ldlt needs d <= 224 on this backend");
-        BFL_CUDA(cudaFuncSetAttribute(als_direct_cta_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         int grid = (int)std::min<int64_t>(nrows, (int64_t)h->num_sms * 4);
-        als_direct_cta_kernel<<<grid, DIRECT_THREADS, smem, st>>>(a);
+        if (det_loss) {
+            BFL_CUDA(cudaFuncSetAttribute(als_direct_cta_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            als_direct_cta_kernel<true><<<grid, DIRECT_THREADS, smem, st>>>(a);
+        } else {
+            BFL_CUDA(cudaFuncSetAttribute(als_direct_cta_kernel<>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            als_direct_cta_kernel<><<<grid, DIRECT_THREADS, smem, st>>>(a);
+        }
         BFL_LAUNCHED();
         return BFL_OK;
     }
@@ -227,11 +248,35 @@ int solve_rows(bfl_als* h, int axis, int64_t row_begin, int64_t row_end, const i
         a.yui = h->yui.p;
     }
     const int nc = (h->d + 31) / 32;
-    if (nc <= 1) return launch_generic<1>(h, a, nrows, st);
-    if (nc <= 2) return launch_generic<2>(h, a, nrows, st);
-    if (nc <= 4) return launch_generic<4>(h, a, nrows, st);
-    if (nc <= 8) return launch_generic<8>(h, a, nrows, st);
-    return launch_generic<16>(h, a, nrows, st);
+    if (nc <= 1) return launch_generic<1>(h, a, nrows, det_loss, st);
+    if (nc <= 2) return launch_generic<2>(h, a, nrows, det_loss, st);
+    if (nc <= 4) return launch_generic<4>(h, a, nrows, det_loss, st);
+    if (nc <= 8) return launch_generic<8>(h, a, nrows, det_loss, st);
+    return launch_generic<16>(h, a, nrows, det_loss, st);
+}
+
+// launch_row_solves with the loss added into d_loss[0 .. 2).  Deterministic mode: every row of the range stores its
+// terms (rows without entries keep the zeros written here) and a fixed tree over the range sums them, so the loss does
+// not depend on which warp solved which rows.
+int solve_rows(bfl_als* h, int axis, int64_t row_begin, int64_t row_end, const int32_t* keys, const float* vals,
+               int64_t shift, int64_t chunk_nnz, double* d_loss, cudaStream_t st) {
+    if (row_end <= row_begin) return BFL_OK;
+    if (!(h->deterministic && h->compute_loss && d_loss))
+        return launch_row_solves(h, axis, row_begin, row_end, keys, vals, shift, chunk_nnz, d_loss, st);
+    const int64_t n = row_end - row_begin, nblk = (n + kLossRows - 1) / kLossRows;
+    const int64_t max_rows = std::max(h->P_rows, h->Q_rows);
+    if (BFL_OK != h->loss_rows.reserve(2 * (size_t)max_rows) ||
+        BFL_OK != h->loss_part.reserve(2 * (size_t)((max_rows + kLossRows - 1) / kLossRows)))
+        return BFL_ERR_CUDA;
+    double* terms = h->loss_rows.p + 2 * row_begin;
+    BFL_CUDA(cudaMemsetAsync(terms, 0, 2 * sizeof(double) * (size_t)n, st));
+    int rc = launch_row_solves(h, axis, row_begin, row_end, keys, vals, shift, chunk_nnz, h->loss_rows.p, st);
+    if (rc != BFL_OK) return rc;
+    loss_tree_partial_kernel<2><<<(unsigned)nblk, 256, 0, st>>>(terms, n, h->loss_part.p);
+    BFL_LAUNCHED();
+    loss_tree_final_kernel<2><<<1, 256, 0, st>>>(h->loss_part.p, nblk, d_loss);
+    BFL_LAUNCHED();
+    return BFL_OK;
 }
 
 }  // namespace

@@ -5,6 +5,8 @@
 //   h[later] -= M[later, B] delta.
 // One CTA of D threads per row; thread j owns column j of the (symmetric) matrix, so every global read of a matrix
 // row is coalesced across the CTA.
+// DET: the row's loss terms are reduced inside each warp, added across the CTA's warps in warp order and stored at
+// loss[2 row] (AlsArgs::loss) instead of being added to loss[0 .. 2) with atomics.
 #pragma once
 #include "als_generic.cuh"
 #include "bfl_common.cuh"
@@ -16,7 +18,7 @@ struct ExplicitArgs {
     const float* scratch;   // per slot: D*D matrix, D (b), D (sum q), 4 (sum w, pad)
 };
 
-template <int D>
+template <int D, bool DET = false>
 __global__ void __launch_bounds__(D) als_explicit_solve_kernel(ExplicitArgs ea) {
     static_assert(D % 32 == 0 && D <= 256, "d % 32 == 0, d <= 256");
     const AlsArgs& a = ea.a;
@@ -24,6 +26,7 @@ __global__ void __launch_bounds__(D) als_explicit_solve_kernel(ExplicitArgs ea) 
     __shared__ float pv[32];
     __shared__ float dl[2][32];
     __shared__ int badf[D / 32];
+    __shared__ double lred[DET ? D / 32 : 1][2];
     const int j = threadIdx.x, lane = j & 31, q = j >> 5;
     const size_t SF = (size_t)D * D + 2 * D + 4;
     double l_nume = 0.0, l_deno = 0.0;
@@ -58,6 +61,15 @@ __global__ void __launch_bounds__(D) als_explicit_solve_kernel(ExplicitArgs ea) 
                 }
             }
             l_nume += t;
+            if (DET) {
+                l_nume = warp_sum_d(l_nume);
+                l_deno = warp_sum_d(l_deno);
+                if (lane == 0) {
+                    lred[q][0] = l_nume;
+                    lred[q][1] = l_deno;
+                }
+                l_nume = l_deno = 0.0;
+            }
         }
         float h = hG + hD - bj;
         const float tol = a.tol;
@@ -113,10 +125,20 @@ __global__ void __launch_bounds__(D) als_explicit_solve_kernel(ExplicitArgs ea) 
 #pragma unroll
         for (int w = 0; w < D / 32; ++w) bad |= badf[w] != 0;
         v = bad ? 0.f : v;
+        if (DET && a.loss && a.compute_loss && j == 0) {   // lred: written before the block loop's barriers
+            double sn = lred[0][0], sd = lred[0][1];
+#pragma unroll
+            for (int w = 1; w < D / 32; ++w) {
+                sn += lred[w][0];
+                sd += lred[w][1];
+            }
+            a.loss[2 * (int64_t)row] = sn;
+            a.loss[2 * (int64_t)row + 1] = sd;
+        }
         a.X[(int64_t)row * a.ld + j] = v;
         for (int pr = 0; pr < a.n_peer; ++pr) a.peerX[pr][(int64_t)row * a.ld + j] = v;
     }
-    if (a.loss && a.compute_loss) {
+    if (!DET && a.loss && a.compute_loss) {
         l_nume = warp_sum_d(l_nume);
         l_deno = warp_sum_d(l_deno);
         if (lane == 0 && (l_nume != 0.0 || l_deno != 0.0)) {

@@ -190,7 +190,9 @@ __host__ __device__ inline size_t fast_smem_bytes(int D, int W, int K, int KS, b
 
 // W warps per row, K register-resident tiles per warp, KS extra tiles per warp kept in shared memory,
 // RES=false: nothing resident, every pass re-gathers (rows longer than 32*W*(K+KS)); GSM: Gram matrix in smem.
-template <int W, int K, int KS, bool RES, bool GSM>
+// DET: a row's loss terms are reduced inside each warp of the team (the lanes' terms come from a fixed tile -> lane map),
+// added across the team's warps in warp order and stored at loss[2 row] (AlsArgs::loss), instead of atomics on loss[0 .. 2).
+template <int W, int K, int KS, bool RES, bool GSM, bool DET = false>
 __global__ void __launch_bounds__(FAST_THREADS, 1) als_ialspp_team_kernel(AlsArgs a, int cap) {
     extern __shared__ __align__(16) float smem[];
     constexpr int TEAMS = FAST_WARPS / W;
@@ -360,8 +362,34 @@ __global__ void __launch_bounds__(FAST_THREADS, 1) als_ialspp_team_kernel(AlsArg
                     if (wt == 0) l_deno += (double)a.Y_rows;
                 }
             }
+            if (DET && a.loss) {
+                l_nume = warp_sum_d(l_nume);
+                l_deno = warp_sum_d(l_deno);
+                if (lane == 0) {
+                    if (W == 1) {
+                        a.loss[2 * (int64_t)row] = l_nume;
+                        a.loss[2 * (int64_t)row + 1] = l_deno;
+                    } else {   // [W][2] doubles in the half of `red` that no partial uses
+                        double* lred = reinterpret_cast<double*>(red + 32 * W);
+                        lred[2 * wt] = l_nume;
+                        lred[2 * wt + 1] = l_deno;
+                    }
+                }
+            }
+            if (DET) l_nume = l_deno = 0.0;
         }
         team_sync<W>(team);
+        if (DET && W > 1 && a.compute_loss && a.loss && wt == 0 && lane == 0) {   // rewritten only after this row's later barriers
+            const double* lred = reinterpret_cast<const double*>(red + 32 * W);
+            double sn = lred[0], sd = lred[1];
+#pragma unroll
+            for (int w = 1; w < W; ++w) {
+                sn += lred[2 * w];
+                sd += lred[2 * w + 1];
+            }
+            a.loss[2 * (int64_t)row] = sn;
+            a.loss[2 * (int64_t)row + 1] = sd;
+        }
 
         // ---- column blocks (als.cc:268-352) ----
         for (int B = 0; B < NB; ++B) {
@@ -515,7 +543,7 @@ __global__ void __launch_bounds__(FAST_THREADS, 1) als_ialspp_team_kernel(AlsArg
             for (int pr = 0; pr < a.n_peer; ++pr) a.peerX[pr][(int64_t)row * ld + j] = v;
         }
     }
-    if (a.loss && a.compute_loss) {
+    if (!DET && a.loss && a.compute_loss) {
         l_nume = warp_sum_d(l_nume);
         l_deno = warp_sum_d(l_deno);
         if (lane == 0 && (l_nume != 0.0 || l_deno != 0.0)) {
@@ -536,6 +564,13 @@ struct FastBins {
     DevBuf<unsigned long long> item_counter;
     int64_t n_items = -1;
     int items_split_class = -1;
+    // deterministic mode: items in list order; END offsets of the list rows' chunks (device and host) and the batches
+    // (list row bounds) of the last scratch budget
+    bool items_det = false;
+    DevBuf<long long> chunk_end;
+    std::vector<long long> h_chunk_end;
+    std::vector<int64_t> det_batches;
+    size_t det_batches_budget = 0;
 };
 // nnz per chunk of a split row.  The tensor core's fp32 accumulator truncates (measured: -0.5 ulp per accumulating MMA on
 // average, 3 MMAs per 8 entries => ~1.1e-5 relative after 1000 entries), so no accumulator is allowed to run longer
@@ -551,7 +586,11 @@ struct FastBinKey {
 };
 struct FastCache {
     std::map<FastBinKey, FastBins*> bins;
-    DevBuf<float> scratch;   // partial matrices of the split rows (als_tc.cuh PARTIAL mode)
+    DevBuf<float> scratch;   // partial matrices of the split rows (als_tc.cuh PARTIAL mode), one slot per row
+    // deterministic mode: one slot per chunk of the batch in flight; budget in bytes for a batch's chunk + row slots
+    // (0: a quarter of the free device memory at first use, at most 2 GiB)
+    DevBuf<float> chunk_scratch;
+    size_t det_budget = 0;
     void clear() {
         for (auto& kv : bins) delete kv.second;
         bins.clear();
@@ -564,19 +603,125 @@ inline bool fast_als_applicable(int optimizer_code, int d, int vdim, int block_s
     return optimizer_code == 8 && d % 32 == 0 && d <= 256 && vdim == d && block_size == 32;
 }
 
-template <int W, int K, int KS, bool RES, bool GSM>
+template <int W, int K, int KS, bool RES, bool GSM, bool DET = false>
 int fast_launch_class(const AlsArgs& a, int cap, int num_sms, cudaStream_t st) {
     const size_t smem = fast_smem_bytes(a.D, W, K, KS, RES, GSM, cap);
     constexpr int SMEM_MAX = 227 * 1024;
     // per device/context attribute: set it on every launch (a process may drive several GPUs)
-    BFL_CUDA(cudaFuncSetAttribute(als_ialspp_team_kernel<W, K, KS, RES, GSM>,
+    BFL_CUDA(cudaFuncSetAttribute(als_ialspp_team_kernel<W, K, KS, RES, GSM, DET>,
                                   cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX));
     if (smem > (size_t)SMEM_MAX) BFL_FAIL(BFL_ERR_STATE, "tuned ALS kernel: shared memory budget exceeded");
     const int64_t nrows = a.row_end - a.row_begin;
     constexpr int TEAMS = FAST_WARPS / W;
     const int grid = (int)std::min<int64_t>((nrows + TEAMS - 1) / TEAMS, (int64_t)num_sms);
-    als_ialspp_team_kernel<W, K, KS, RES, GSM><<<grid, FAST_THREADS, smem, st>>>(a, cap);
+    als_ialspp_team_kernel<W, K, KS, RES, GSM, DET><<<grid, FAST_THREADS, smem, st>>>(a, cap);
     BFL_LAUNCHED();
+    return BFL_OK;
+}
+// det_loss: a.loss takes per-row terms (the DET instantiation)
+template <int W, int K, int KS, bool RES, bool GSM>
+int fast_launch_class(const AlsArgs& a, int cap, int num_sms, cudaStream_t st, bool det_loss) {
+    return det_loss ? fast_launch_class<W, K, KS, RES, GSM, true>(a, cap, num_sms, st)
+                    : fast_launch_class<W, K, KS, RES, GSM>(a, cap, num_sms, st);
+}
+
+// explicit-matrix solve of the rows list[0 .. nrows) from their row slots scratch[0 .. nrows); det_loss: a0.loss takes
+// per-row terms (the DET instantiation)
+inline int launch_explicit_solve(const AlsArgs& a0, const int32_t* list, int64_t nrows, const float* scratch, bool det_loss,
+                                 int num_sms, cudaStream_t st) {
+    ExplicitArgs ea;
+    ea.a = a0;
+    ea.a.row_list = list;
+    ea.a.row_begin = 0;
+    ea.a.row_end = nrows;
+    ea.scratch = scratch;
+    const int ge = (int)std::min<int64_t>(nrows, (int64_t)num_sms * 4);
+    if (a0.D == 128) {
+        if (det_loss) als_explicit_solve_kernel<128, true><<<ge, 128, 0, st>>>(ea);
+        else als_explicit_solve_kernel<128><<<ge, 128, 0, st>>>(ea);
+    } else {
+        if (det_loss) als_explicit_solve_kernel<256, true><<<ge, 256, 0, st>>>(ea);
+        else als_explicit_solve_kernel<256><<<ge, 256, 0, st>>>(ea);
+    }
+    BFL_LAUNCHED();
+    return BFL_OK;
+}
+
+// Deterministic split rows: the long rows list7[0 .. n7) in batches of whole rows whose chunk and row slots fit the
+// budget (a batch always takes at least one row).  Per batch: chunk matrices by plain stores, the ordered sum of each
+// row's chunks, the explicit-matrix solve.  The items follow list7, so the chunks of list row i are the items
+// first[i] .. first[i] + nc_i of an exclusive scan; list7 itself is filled through fast_fill_kernel's atomic cursor, so
+// the item order, the slot of a chunk and the batch bounds differ between handles.  No bit depends on them: a row is
+// summed on its own in chunk order and its loss terms are stored by row.  Scratch that cannot be allocated is an error.
+template <int D>
+int fast_split_rows_det(const AlsArgs& a0, FastCache& cache, FastBins* fb, const int32_t* list7, int64_t n7,
+                        int split_min_class, bool det_loss, int num_sms, cudaStream_t st) {
+    if (fb->n_items < 0 || fb->items_split_class != split_min_class || !fb->items_det) {
+        const int g7 = (int)std::min<int64_t>((n7 + 127) / 128, 1024);
+        if (BFL_OK != fb->chunk_end.reserve((size_t)n7)) return BFL_ERR_CUDA;
+        tc::tc_chunk_counts_kernel<<<g7, 128, 0, st>>>(a0.indptr, list7, n7, TC_SPLIT, fb->chunk_end.p);
+        BFL_LAUNCHED();
+        int rc = inclusive_scan_i64(fb->chunk_end.p, fb->chunk_end.p, n7, st);
+        if (rc != BFL_OK) return rc;
+        fb->h_chunk_end.resize((size_t)n7);
+        BFL_CUDA(cudaMemcpyAsync(fb->h_chunk_end.data(), fb->chunk_end.p, sizeof(long long) * (size_t)n7, cudaMemcpyDeviceToHost, st));
+        BFL_CUDA(cudaStreamSynchronize(st));
+        const long long total = fb->h_chunk_end.back();
+        if (BFL_OK != fb->items.reserve(3 * (size_t)total)) return BFL_ERR_CUDA;
+        tc::tc_fill_items_scanned_kernel<<<g7, 128, 0, st>>>(list7, n7, fb->chunk_end.p, fb->items.p);
+        BFL_LAUNCHED();
+        fb->n_items = (int64_t)total;
+        fb->items_split_class = split_min_class;
+        fb->items_det = true;
+        fb->det_batches.clear();
+    }
+    const size_t sf = tc::scratch_floats<D>(), sfb = sf * sizeof(float);
+    if (!cache.det_budget) {
+        size_t free_b = 0, total_b = 0;
+        BFL_CUDA(cudaMemGetInfo(&free_b, &total_b));
+        cache.det_budget = std::max<size_t>(std::min<size_t>(free_b / 4, (size_t)2 << 30), 2 * sfb);
+    }
+    const long long* ce = fb->h_chunk_end.data();
+    if (fb->det_batches.empty() || fb->det_batches_budget != cache.det_budget) {
+        fb->det_batches.assign(1, 0);
+        size_t used = 0;
+        for (int64_t i = 0; i < n7; ++i) {
+            const size_t cost = (size_t)(ce[i] - (i ? ce[i - 1] : 0) + 1) * sfb;
+            if (used && used + cost > cache.det_budget) {
+                fb->det_batches.push_back(i);
+                used = 0;
+            }
+            used += cost;
+        }
+        fb->det_batches.push_back(n7);
+        fb->det_batches_budget = cache.det_budget;
+    }
+    int64_t max_rows = 0, max_chunks = 0;
+    for (size_t b = 0; b + 1 < fb->det_batches.size(); ++b) {
+        const int64_t i = fb->det_batches[b], j = fb->det_batches[b + 1];
+        max_rows = std::max(max_rows, j - i);
+        max_chunks = std::max<int64_t>(max_chunks, ce[j - 1] - (i ? ce[i - 1] : 0));
+    }
+    if (BFL_OK != cache.scratch.reserve(sf * (size_t)max_rows) || BFL_OK != cache.chunk_scratch.reserve(sf * (size_t)max_chunks))
+        BFL_FAIL(BFL_ERR_CUDA, "deterministic ALS: cannot allocate the split-row scratch (" +
+                                   std::to_string((sfb * (size_t)(max_rows + max_chunks)) >> 20) +
+                                   " MB); lower _b200_det_scratch_mb or free device memory");
+    const int nf4 = (int)((a0.compute_loss && a0.axis == 1 ? sf : (size_t)D * D + D) / 4);
+    for (size_t b = 0; b + 1 < fb->det_batches.size(); ++b) {
+        const int64_t i = fb->det_batches[b], j = fb->det_batches[b + 1];
+        const int64_t chunk0 = i ? ce[i - 1] : 0, nchunks = ce[j - 1] - chunk0;
+        int rc = tc::tc_launch_partial<D>(a0, fb->items.p + 3 * chunk0, nchunks, cache.chunk_scratch.p, nchunks, TC_SPLIT,
+                                          num_sms, st, true);
+        if (rc != BFL_OK) return rc;
+        for (int64_t r = i; r < j; r += 65535) {   // grid.y limit
+            const dim3 grid((nf4 + 255) / 256, (unsigned)std::min<int64_t>(65535, j - r));
+            tc::tc_chunk_reduce_kernel<<<grid, 256, 0, st>>>(cache.chunk_scratch.p, fb->chunk_end.p, r, chunk0, sf, nf4,
+                                                             cache.scratch.p + (size_t)(r - i) * sf);
+            BFL_LAUNCHED();
+        }
+        rc = launch_explicit_solve(a0, list7 + i, j - i, cache.scratch.p, det_loss, num_sms, st);
+        if (rc != BFL_OK) return rc;
+    }
     return BFL_OK;
 }
 
@@ -587,7 +732,9 @@ int fast_launch_class(const AlsArgs& a, int cap, int num_sms, cudaStream_t st) {
 // (chunk matrices summed in global memory + explicit-matrix solve).  FAST_NCLASS disables either.
 inline int fast_als_launch(const AlsArgs& a0, FastCache& cache, int num_sms, cudaStream_t st,
                            const int32_t** leftover_rows, int64_t* leftover_count, int tc_min_class, int split_min_class,
-                           int long_regather = 0) {
+                           int long_regather = 0, bool det = false) {
+    // deterministic mode: split rows through fast_split_rows_det, and the kernels that store per-row loss terms
+    const bool det_loss = det && a0.loss && a0.compute_loss;
     *leftover_rows = nullptr;
     *leftover_count = 0;
     const int64_t nrows = a0.row_end - a0.row_begin;
@@ -619,7 +766,16 @@ inline int fast_als_launch(const AlsArgs& a0, FastCache& cache, int num_sms, cud
         fb = it->second;
     }
     tc_min_class = std::min(tc_min_class, split_min_class);
-    if (split_min_class < FAST_NCLASS && fb->offset[FAST_NCLASS] > fb->offset[split_min_class]) {
+    const bool has_split = split_min_class < FAST_NCLASS && fb->offset[FAST_NCLASS] > fb->offset[split_min_class];
+    if (has_split && det) {
+        const int64_t n7 = fb->offset[FAST_NCLASS] - fb->offset[split_min_class];
+        const int32_t* list7 = fb->lists.p + fb->offset[split_min_class];
+        const int rc = a0.D == 128
+                           ? fast_split_rows_det<128>(a0, cache, fb, list7, n7, split_min_class, det_loss, num_sms, st)
+                           : fast_split_rows_det<256>(a0, cache, fb, list7, n7, split_min_class, det_loss, num_sms, st);
+        if (rc != BFL_OK) return rc;
+    }
+    if (has_split && !det) {
         // long rows (any length): cut into chunks spread over the SMs, partial matrices summed in global memory, then the
         // explicit-matrix solve
         const int64_t n7 = fb->offset[FAST_NCLASS] - fb->offset[split_min_class];
@@ -645,23 +801,15 @@ inline int fast_als_launch(const AlsArgs& a0, FastCache& cache, int num_sms, cud
                      ? tc::tc_launch_partial<128>(a0, fb->items.p, fb->n_items, cache.scratch.p, n7, TC_SPLIT, num_sms, st)
                      : tc::tc_launch_partial<256>(a0, fb->items.p, fb->n_items, cache.scratch.p, n7, TC_SPLIT, num_sms, st);
         if (rc != BFL_OK) return rc;
-        ExplicitArgs ea;
-        ea.a = a0;
-        ea.a.row_list = list7;
-        ea.a.row_begin = 0;
-        ea.a.row_end = n7;
-        ea.scratch = cache.scratch.p;
-        const int ge = (int)std::min<int64_t>(n7, (int64_t)num_sms * 4);
-        if (a0.D == 128) als_explicit_solve_kernel<128><<<ge, 128, 0, st>>>(ea);
-        else als_explicit_solve_kernel<256><<<ge, 256, 0, st>>>(ea);
-        BFL_LAUNCHED();
+        rc = launch_explicit_solve(a0, list7, n7, cache.scratch.p, false, num_sms, st);
+        if (rc != BFL_OK) return rc;
     }
     if (tc_min_class < split_min_class && fb->offset[split_min_class] > fb->offset[tc_min_class]) {
         AlsArgs a = a0;
         a.row_list = fb->lists.p;
         a.row_begin = fb->offset[tc_min_class];
         a.row_end = fb->offset[split_min_class];
-        const int rc = tc::tc_launch(a, num_sms, st);
+        const int rc = tc::tc_launch(a, num_sms, st, det_loss);
         if (rc != BFL_OK) return rc;
     }
     for (int c = 0; c < std::min(FAST_NCLASS - 1, tc_min_class); ++c) {
@@ -674,19 +822,19 @@ inline int fast_als_launch(const AlsArgs& a0, FastCache& cache, int num_sms, cud
         int rc = BFL_OK;
         const bool gsm = a.D <= 128;   // d x (d+4) floats of Gram fit next to the staging buffers only up to d = 128
         switch (c) {
-            case 0: rc = gsm ? fast_launch_class<1, 1, 0, true, true>(a, fc.cap, num_sms, st)
-                             : fast_launch_class<1, 1, 0, true, false>(a, fc.cap, num_sms, st); break;
-            case 1: rc = gsm ? fast_launch_class<1, 2, 0, true, true>(a, fc.cap, num_sms, st)
-                             : fast_launch_class<1, 2, 0, true, false>(a, fc.cap, num_sms, st); break;
-            case 2: rc = gsm ? fast_launch_class<2, 2, 0, true, true>(a, fc.cap, num_sms, st)
-                             : fast_launch_class<2, 2, 0, true, false>(a, fc.cap, num_sms, st); break;
-            case 3: rc = gsm ? fast_launch_class<4, 2, 0, true, true>(a, fc.cap, num_sms, st)
-                             : fast_launch_class<4, 2, 0, true, false>(a, fc.cap, num_sms, st); break;
-            case 4: rc = gsm ? fast_launch_class<8, 2, 0, true, true>(a, fc.cap, num_sms, st)
-                             : fast_launch_class<8, 2, 0, true, false>(a, fc.cap, num_sms, st); break;
-            case 5: rc = fast_launch_class<16, 2, 1, true, false>(a, fc.cap, num_sms, st); break;
-            case 6: rc = gsm ? fast_launch_class<16, 1, 0, false, true>(a, fc.cap, num_sms, st)
-                             : fast_launch_class<16, 1, 0, false, false>(a, fc.cap, num_sms, st); break;
+            case 0: rc = gsm ? fast_launch_class<1, 1, 0, true, true>(a, fc.cap, num_sms, st, det_loss)
+                             : fast_launch_class<1, 1, 0, true, false>(a, fc.cap, num_sms, st, det_loss); break;
+            case 1: rc = gsm ? fast_launch_class<1, 2, 0, true, true>(a, fc.cap, num_sms, st, det_loss)
+                             : fast_launch_class<1, 2, 0, true, false>(a, fc.cap, num_sms, st, det_loss); break;
+            case 2: rc = gsm ? fast_launch_class<2, 2, 0, true, true>(a, fc.cap, num_sms, st, det_loss)
+                             : fast_launch_class<2, 2, 0, true, false>(a, fc.cap, num_sms, st, det_loss); break;
+            case 3: rc = gsm ? fast_launch_class<4, 2, 0, true, true>(a, fc.cap, num_sms, st, det_loss)
+                             : fast_launch_class<4, 2, 0, true, false>(a, fc.cap, num_sms, st, det_loss); break;
+            case 4: rc = gsm ? fast_launch_class<8, 2, 0, true, true>(a, fc.cap, num_sms, st, det_loss)
+                             : fast_launch_class<8, 2, 0, true, false>(a, fc.cap, num_sms, st, det_loss); break;
+            case 5: rc = fast_launch_class<16, 2, 1, true, false>(a, fc.cap, num_sms, st, det_loss); break;
+            case 6: rc = gsm ? fast_launch_class<16, 1, 0, false, true>(a, fc.cap, num_sms, st, det_loss)
+                             : fast_launch_class<16, 1, 0, false, false>(a, fc.cap, num_sms, st, det_loss); break;
         }
         if (rc != BFL_OK) return rc;
     }

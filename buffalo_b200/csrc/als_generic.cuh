@@ -19,7 +19,8 @@ struct AlsArgs {
     const int32_t* keys;  // chunk buffers, element (it - shift)
     const float* vals;
     float* yui;           // scratch [chunk nnz] (generic ialspp only)
-    double* loss;         // [0] numerator, [1] denominator (may be null)
+    double* loss;         // [0] numerator, [1] denominator (may be null).  Kernels instantiated with DET = true take it
+                          // as per-row terms instead: row r's pair is stored (not added) at loss[2 r], loss[2 r + 1]
     const int32_t* row_list;  // optional explicit row list (absolute row ids), else null
     int64_t shift;        // global offset of keys[0]
     int64_t row_begin, row_end;  // absolute rows [begin, end) (or range into row_list)
@@ -40,7 +41,7 @@ constexpr int GEN_WARPS = 8;
 // ---------------------------------------------------------------------------------------
 // manual_cg  (lib/algo.cc:58-82 on the system of als.cc:180-202)
 // ---------------------------------------------------------------------------------------
-template <int NC>
+template <int NC, bool DET = false>
 __global__ void __launch_bounds__(GEN_WARPS * 32) als_cg_warp_kernel(AlsArgs a) {
     __shared__ float ps_all[GEN_WARPS][NC * 32];
     const int lane = threadIdx.x & 31, wib = warp_id_uniform();
@@ -204,8 +205,15 @@ __global__ void __launch_bounds__(GEN_WARPS * 32) als_cg_warp_kernel(AlsArgs a) 
             }
         }
         __syncwarp();
+        if (DET) {   // every lane holds the row's terms, added in entry order
+            if (a.loss && a.compute_loss && lane == 0) {
+                a.loss[2 * row] = l_nume;
+                a.loss[2 * row + 1] = l_deno;
+            }
+            l_nume = l_deno = 0.0;
+        }
     }
-    if (a.loss && a.compute_loss && lane == 0) {
+    if (!DET && a.loss && a.compute_loss && lane == 0) {
         atomicAdd(a.loss, l_nume);
         atomicAdd(a.loss + 1, l_deno);
     }
@@ -214,7 +222,7 @@ __global__ void __launch_bounds__(GEN_WARPS * 32) als_cg_warp_kernel(AlsArgs a) 
 // ---------------------------------------------------------------------------------------
 // iALS++  (als.cc:211-358): block size <= 32*NC
 // ---------------------------------------------------------------------------------------
-template <int NC>
+template <int NC, bool DET = false>
 __global__ void __launch_bounds__(GEN_WARPS * 32) als_ialspp_warp_kernel(AlsArgs a) {
     __shared__ float xs_all[GEN_WARPS][NC * 32];
     __shared__ float ps_all[GEN_WARPS][NC * 32];
@@ -408,8 +416,15 @@ __global__ void __launch_bounds__(GEN_WARPS * 32) als_ialspp_warp_kernel(AlsArgs
                 for (int pr = 0; pr < a.n_peer; ++pr) a.peerX[pr][row * ld + c] = v;
             }
         }
+        if (DET) {   // every lane holds the row's terms, added in entry order
+            if (a.loss && a.compute_loss && lane == 0) {
+                a.loss[2 * row] = l_nume;
+                a.loss[2 * row + 1] = l_deno;
+            }
+            l_nume = l_deno = 0.0;
+        }
     }
-    if (a.loss && a.compute_loss && lane == 0) {
+    if (!DET && a.loss && a.compute_loss && lane == 0) {
         atomicAdd(a.loss, l_nume);
         atomicAdd(a.loss + 1, l_deno);
     }
@@ -425,6 +440,7 @@ __global__ void __launch_bounds__(GEN_WARPS * 32) als_ialspp_warp_kernel(AlsArgs
 constexpr int DIRECT_THREADS = 256;
 constexpr int DIRECT_NB = 8;
 
+template <bool DET = false>
 __global__ void __launch_bounds__(DIRECT_THREADS) als_direct_cta_kernel(AlsArgs a) {
     extern __shared__ float sm[];
     const int D = a.D, ld = a.ld, P1 = D + 1;
@@ -434,6 +450,7 @@ __global__ void __launch_bounds__(DIRECT_THREADS) als_direct_cta_kernel(AlsArgs 
     float* qb = wv + D;                  // [NB][D]
     __shared__ float s_v[DIRECT_NB];
     __shared__ double s_loss[2];
+    __shared__ double s_dn[DET ? DIRECT_NB : 1], s_dav[DET ? DIRECT_NB : 1];   // DET: the loss terms of a batch's entries
     const int tid = threadIdx.x, lane = tid & 31, wid = warp_id_uniform();
     if (tid < 2) s_loss[tid] = 0.0;
     for (int64_t ri = a.row_begin + blockIdx.x; ri < a.row_end; ri += gridDim.x) {
@@ -477,6 +494,13 @@ __global__ void __launch_bounds__(DIRECT_THREADS) als_direct_cta_kernel(AlsArgs 
         for (int64_t b0 = beg; b0 < end; b0 += DIRECT_NB) {
             const int nb = (int)((end - b0) < DIRECT_NB ? (end - b0) : DIRECT_NB);
             __syncthreads();
+            if (DET && a.compute_loss && a.axis == 1 && tid == 0 && b0 > beg) {
+                // the previous (full) batch's terms, in entry order; they are rewritten only after the next barrier
+                for (int b = 0; b < DIRECT_NB; ++b) {
+                    l_nume += s_dn[b];
+                    l_deno += s_dav[b];
+                }
+            }
             for (int e = tid; e < nb * D; e += DIRECT_THREADS) {
                 const int b = e / D, c = e - b * D;
                 const int key = a.keys[b0 + b - a.shift];
@@ -491,8 +515,13 @@ __global__ void __launch_bounds__(DIRECT_THREADS) als_direct_cta_kernel(AlsArgs 
                 if (lane == 0) {
                     const float av = a.alpha * s_v[wid];
                     double dn = -(double)(dot * dot) + (double)((dot - 1.f) * (dot - 1.f)) * (1.0 + (double)av);
-                    atomicAdd(&s_loss[0], dn);
-                    atomicAdd(&s_loss[1], (double)av);
+                    if (DET) {   // one term per entry; thread 0 adds them in entry order after the next barrier
+                        s_dn[wid] = dn;
+                        s_dav[wid] = (double)av;
+                    } else {
+                        atomicAdd(&s_loss[0], dn);
+                        atomicAdd(&s_loss[1], (double)av);
+                    }
                 }
             }
             for (int e = tid; e < D * D; e += DIRECT_THREADS) {
@@ -508,6 +537,12 @@ __global__ void __launch_bounds__(DIRECT_THREADS) als_direct_cta_kernel(AlsArgs 
             }
         }
         __syncthreads();
+        if (DET && a.compute_loss && a.axis == 1 && tid == 0) {   // the last batch's terms
+            for (int b = 0; b < (int)((n - 1) % DIRECT_NB) + 1; ++b) {
+                l_nume += s_dn[b];
+                l_deno += s_dav[b];
+            }
+        }
         // in-place Cholesky (lower), right-looking
         for (int j = 0; j < D; ++j) {
             if (tid == 0) M[j * P1 + j] = sqrtf(M[j * P1 + j]);
@@ -552,14 +587,19 @@ __global__ void __launch_bounds__(DIRECT_THREADS) als_direct_cta_kernel(AlsArgs 
                 xrow[i] = v;
                 for (int pr = 0; pr < a.n_peer; ++pr) a.peerX[pr][row * ld + i] = v;
             }
-            if (lane == 0 && a.compute_loss) {
+            if (DET) {
+                if (lane == 0 && a.loss && a.compute_loss) {
+                    a.loss[2 * row] = l_nume;
+                    a.loss[2 * row + 1] = l_deno;
+                }
+            } else if (lane == 0 && a.compute_loss) {
                 atomicAdd(&s_loss[0], l_nume);
                 atomicAdd(&s_loss[1], l_deno);
             }
         }
     }
     __syncthreads();
-    if (a.loss && a.compute_loss && tid < 2) atomicAdd(a.loss + tid, s_loss[tid]);
+    if (!DET && a.loss && a.compute_loss && tid < 2) atomicAdd(a.loss + tid, s_loss[tid]);
 }
 
 // ---------------------------------------------------------------------------------------

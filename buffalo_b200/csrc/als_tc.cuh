@@ -111,10 +111,28 @@ struct Smem {
     alignas(8) uint64_t plan_full[NPG], plan_empty[NPG], raw_full[NR], raw_empty[NR], op_full[NO], op_empty[NO];
     alignas(8) uint64_t acc_full, acc_empty, x_full[NXS], d_full[4];
 };
+// deterministic loss of the fused mode: the epilogue warps' terms of a row, handed to the last block's warp
+template <int D>
+struct SmemDet : Smem<D> {
+    double lossp[NXS][4][2];
+};
 
 // PARTIAL = false: rows of a.row_list[row_begin..row_end) are solved in place.
 // PARTIAL = true : the list holds chunk items of long rows (pairs: row, chunk index); the chunk's matrix and vectors are
 //                  added to scratch[slot] (slot = items[3*i+2]) and solved later by als_explicit_solve_kernel.
+// DET (deterministic mode, separate instantiations):
+//   PARTIAL: a scratch slot belongs to a CHUNK (slot = the item's index in this launch) and is written with plain stores;
+//            tc_chunk_reduce_kernel then adds the chunk slots of a row in ascending chunk order.  Every element of a chunk
+//            slot is stored exactly once, so the slots need no memset:
+//              matrix, d = 128 (r0 = c0 = 0): d0 holds rows 0..63, d1 rows 64..127, each over all 128 columns (N0 = 128); a
+//                thread's (n, h, i) enumerate distinct (r, c) and the four MMA warps own disjoint rows 16 wq + 0..15 (+ 64);
+//              matrix, d = 256: pass 0 stores rows / columns 0..127, pass 2 rows / columns 128..255, pass 1 rows 0..127 x
+//                columns 128..255 and (r0 != c0) the mirrored element (c, r) of each, i.e. rows 128..255 x columns 0..127:
+//                four disjoint quadrants, each element once;
+//              vectors (pass 0 only): b[0..D) and, with LOSS1, sum q[0..D) and the four floats (sum w, 0, 0, 0) by the
+//                epilogue thread j (and j + 128 at d = 256).  Without LOSS1 only matrix + b are written, and only those read.
+//   fused:   the loss terms of a row are reduced inside each epilogue warp, handed through shared memory along the
+//            delta hand-offs (d_full) to the warp of the last block, added there in warp order and stored at loss[2 row].
 struct TcArgs {
     AlsArgs a;
     const int32_t* items;   // PARTIAL: triples (row, chunk, scratch slot)
@@ -162,12 +180,13 @@ __global__ void tc_scale_kernel(const unsigned int* __restrict__ ymax, const uns
 
 // LOSS1: compute_loss on the item axis (the convert warps also hand sum q / sum w to the epilogue); a template parameter so
 // that the common case keeps a branch-free convert loop
-template <int D, bool PARTIAL, bool LOSS1>
+template <int D, bool PARTIAL, bool LOSS1, bool DET = false>
 __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
     static_assert(D == 128 || (D == 256 && PARTIAL), "fused row solve: d = 128; split-row mode: d = 128 or 256");
     constexpr int TILE = Cfg<D>::TILE, NF = Cfg<D>::NF, LBO = Cfg<D>::LBO;
     extern __shared__ __align__(1024) unsigned char smem_raw_[];
     Smem<D>& S = *reinterpret_cast<Smem<D>*>(smem_raw_);
+    [[maybe_unused]] SmemDet<D>& SD = *reinterpret_cast<SmemDet<D>*>(smem_raw_);   // DET instantiations only
     const AlsArgs& a = ta.a;
     const int tid = threadIdx.x, lane = tid & 31;
     const int warp = __shfl_sync(FULL, tid >> 5, 0);
@@ -211,7 +230,7 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
             const int64_t rn = a.indptr[row] - rb;
             beg = rb + (int64_t)p[1] * ta.split;
             n = min(ta.split, rn - (int64_t)p[1] * ta.split);
-            slot = p[2];
+            slot = DET ? (int)it : p[2];
         } else {
             row = a.row_list[a.row_begin + it];
             beg = row == 0 ? 0 : a.indptr[row - 1];
@@ -474,9 +493,10 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                     for (int i = 0; i < 64; ++i) { if (i < N0 / 2) acc_fence(d0[i]); acc_fence(d1[i]); }
                     mbar_wait_idle(&S.acc_empty, aph ^ 1u);   // the epilogue is done with the previous row
                     if constexpr (PARTIAL) {
-                        // the chunk of item my_first + seq * stride: float atomics (the chunks of one row are summed in
-                        // arrival order); pass 1 of d = 256 also adds the transposed block
-                        const int slot = ta.items[3 * (a.row_begin + my_first + seq * stride) + 2];
+                        // the chunk of item my_first + seq * stride; pass 1 of d = 256 also writes the transposed block.
+                        // Default: float atomics into the row's slot (the chunks of one row are summed in arrival order);
+                        // DET: plain stores into the chunk's own slot
+                        const int slot = DET ? (int)(my_first + seq * stride) : ta.items[3 * (a.row_begin + my_first + seq * stride) + 2];
                         float* sc = ta.scratch + (size_t)slot * scratch_floats<D>();
 #pragma unroll
                         for (int n = 0; n < 16; ++n)
@@ -486,11 +506,20 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                                 for (int i = 0; i < 2; ++i) {
                                     const int r = r0 + fr + 8 * h, c = c0 + 8 * n + fc + i;
                                     const float v0 = d0[4 * n + 2 * h + i] * inv2, v1 = d1[4 * n + 2 * h + i] * inv2;
-                                    atomicAdd(sc + (size_t)r * D + c, v0);
-                                    atomicAdd(sc + (size_t)(r + 64) * D + c, v1);
-                                    if (r0 != c0) {
-                                        atomicAdd(sc + (size_t)c * D + r, v0);
-                                        atomicAdd(sc + (size_t)c * D + r + 64, v1);
+                                    if constexpr (DET) {
+                                        sc[(size_t)r * D + c] = v0;
+                                        sc[(size_t)(r + 64) * D + c] = v1;
+                                        if (r0 != c0) {
+                                            sc[(size_t)c * D + r] = v0;
+                                            sc[(size_t)c * D + r + 64] = v1;
+                                        }
+                                    } else {
+                                        atomicAdd(sc + (size_t)r * D + c, v0);
+                                        atomicAdd(sc + (size_t)(r + 64) * D + c, v1);
+                                        if (r0 != c0) {
+                                            atomicAdd(sc + (size_t)c * D + r, v0);
+                                            atomicAdd(sc + (size_t)c * D + r + 64, v1);
+                                        }
                                     }
                                 }
                     } else {
@@ -806,7 +835,16 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                 const uint32_t bs = (uint32_t)(seq & (NBV - 1));
                 mbar_wait_idle(&S.acc_full, aph);
                 float* sc = ta.scratch + (size_t)slot * scratch_floats<D>();
-                if (ta.pass == 0) {
+                if constexpr (DET) {
+                    if (ta.pass == 0) {
+                        for (int jj = j; jj < D; jj += 128) {
+                            sc[(size_t)D * D + jj] = S.bvec[bs][0][jj] + (KH == 2 ? S.bvec[bs][KH - 1][jj] : 0.f);
+                            if (LOSS1) sc[(size_t)D * D + D + jj] = S.sumq[bs][0][jj] + (KH == 2 ? S.sumq[bs][KH - 1][jj] : 0.f);
+                        }
+                        if (LOSS1 && j < 4)
+                            sc[(size_t)D * D + 2 * D + j] = j == 0 ? S.wsum[bs][0] + (KH == 2 ? S.wsum[bs][KH - 1] : 0.f) : 0.f;
+                    }
+                } else if (ta.pass == 0) {
                     for (int jj = j; jj < D; jj += 128) {
                         atomicAdd(sc + (size_t)D * D + jj, S.bvec[bs][0][jj] + (KH == 2 ? S.bvec[bs][KH - 1][jj] : 0.f));
                         if (LOSS1) atomicAdd(sc + (size_t)D * D + D + jj, S.sumq[bs][0][jj] + (KH == 2 ? S.sumq[bs][KH - 1][jj] : 0.f));
@@ -863,6 +901,7 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                     continue;
                 }
                 const float bj = S.bvec[bs][0][j] + (KH == 2 ? S.bvec[bs][KH - 1][j] : 0.f);
+                double ln_row = 0.0, ld_row = 0.0;   // DET: this warp's loss terms of the row
                 // ---- h = M x - b; keep the diagonal block of M in registers ----
                 float hM = 0.f;
                 float md[32];
@@ -894,7 +933,18 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                             l_deno += (double)a.Y_rows + ws;
                         }
                     }
-                    l_nume += t;
+                    if constexpr (DET) {
+                        // the denominator only ever has thread 0's term (warp 0, lane 0): nothing to reduce
+                        ln_row = warp_sum_d(t);
+                        ld_row = l_deno;
+                        l_deno = 0.0;
+                        if (q < 3 && lane == 0) {   // published by this warp's d_full arrival below
+                            SD.lossp[xsl][q][0] = ln_row;
+                            SD.lossp[xsl][q][1] = ld_row;
+                        }
+                    } else {
+                        l_nume += t;
+                    }
                 }
                 float h = hM - bj;
                 // ---- fold in the deltas of the earlier blocks as they appear: h -= M[j, B] . delta_B ----
@@ -914,6 +964,19 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                         u1 = fmaf(mv[i + 3], d4.w, u1);
                     }
                     h -= u0 + u1;
+                }
+                if constexpr (DET) {
+                    // the waits on d_full[0 .. 2] above acquired the earlier warps' terms: add them in warp order
+                    if (q == 3 && lane == 0 && a.loss && a.compute_loss) {
+                        double sn = SD.lossp[xsl][0][0], sd = SD.lossp[xsl][0][1];
+#pragma unroll
+                        for (int w = 1; w < 3; ++w) {
+                            sn += SD.lossp[xsl][w][0];
+                            sd += SD.lossp[xsl][w][1];
+                        }
+                        a.loss[2 * (int64_t)row] = sn + ln_row;
+                        a.loss[2 * (int64_t)row + 1] = sd + ld_row;
+                    }
                 }
                 // this warp's reads of the matrix are done
                 __syncwarp();
@@ -977,7 +1040,7 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                 xj = x1; x1 = x2;
                 nlen = nlen1; nlen1 = nlen2;
             }
-            if (a.loss && a.compute_loss) {
+            if (!DET && a.loss && a.compute_loss) {
                 l_nume = warp_sum_d(l_nume);
                 l_deno = warp_sum_d(l_deno);
                 if (lane == 0 && (l_nume != 0.0 || l_deno != 0.0)) {
@@ -1038,10 +1101,56 @@ __global__ void tc_fill_items_kernel(const int64_t* __restrict__ indptr, const i
     }
 }
 
-// accumulates the chunk matrices of the split rows into scratch (zeroed here); a.row_begin/row_end index `items`
+// Deterministic mode: chunk counts of the long rows (scanned by the caller into END offsets) and items in list order, so
+// that the chunks of list row i are the items first[i] .. first[i] + nc_i (first = exclusive prefix) -- no atomic cursor.
+__global__ void tc_chunk_counts_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ list, int64_t nrows,
+                                       int64_t split, long long* __restrict__ counts) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nrows; i += (int64_t)gridDim.x * blockDim.x) {
+        const int row = list[i];
+        const int64_t n = indptr[row] - (row == 0 ? 0 : indptr[row - 1]);
+        counts[i] = (n + split - 1) / split;
+    }
+}
+__global__ void tc_fill_items_scanned_kernel(const int32_t* __restrict__ list, int64_t nrows,
+                                             const long long* __restrict__ chunk_end, int32_t* __restrict__ items) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nrows; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t pos = i == 0 ? 0 : chunk_end[i - 1], nc = chunk_end[i] - pos;
+        for (int64_t c = 0; c < nc; ++c) {
+            items[3 * (pos + c) + 0] = list[i];
+            items[3 * (pos + c) + 1] = (int32_t)c;
+            items[3 * (pos + c) + 2] = (int32_t)i;
+        }
+    }
+}
+
+// Deterministic mode: row slot i of `rows_out` = chunk slot first .. last of list row row0 + i, added in ascending chunk
+// order with rounded fp32 adds, starting from the first chunk.  chunk_end: END offsets of the whole list's chunks,
+// chunk0: the first chunk held by `chunks`.  blockIdx.y = row of the batch; threads run over the slot in 16-byte pieces
+// (nf4 of them: matrix + b, or the whole slot when the loss vectors were written), so every access is coalesced.
+__global__ void __launch_bounds__(256) tc_chunk_reduce_kernel(const float* __restrict__ chunks, const long long* __restrict__ chunk_end,
+                                                              int64_t row0, int64_t chunk0, size_t slot_floats, int nf4,
+                                                              float* __restrict__ rows_out) {
+    const int64_t i = row0 + blockIdx.y;
+    const int64_t c0 = (i == 0 ? 0 : chunk_end[i - 1]) - chunk0, c1 = chunk_end[i] - chunk0;
+    float4* out = reinterpret_cast<float4*>(rows_out + (size_t)blockIdx.y * slot_floats);
+    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < nf4; e += gridDim.x * blockDim.x) {
+        float4 acc = __ldg(reinterpret_cast<const float4*>(chunks + (size_t)c0 * slot_floats) + e);
+        for (int64_t c = c0 + 1; c < c1; ++c) {
+            const float4 v = __ldg(reinterpret_cast<const float4*>(chunks + (size_t)c * slot_floats) + e);
+            acc.x = __fadd_rn(acc.x, v.x);
+            acc.y = __fadd_rn(acc.y, v.y);
+            acc.z = __fadd_rn(acc.z, v.z);
+            acc.w = __fadd_rn(acc.w, v.w);
+        }
+        out[e] = acc;
+    }
+}
+
+// chunk matrices of the split rows; a.row_begin/row_end index `items`.  Default: added into one slot per row of
+// `scratch`, which is zeroed here.  det: stored into one slot per item, no memset (see the kernel's DET notes)
 template <int D>
 int tc_launch_partial(const AlsArgs& a, const int32_t* items, int64_t nitems, float* scratch, int64_t nslots,
-                      int64_t split, int num_sms, cudaStream_t st) {
+                      int64_t split, int num_sms, cudaStream_t st, bool det = false) {
     if (nitems <= 0) return BFL_OK;
     if (!a.tc_scales) BFL_FAIL(BFL_ERR_STATE, "tensor-core ALS kernel: operand scale not prepared");
     TcArgs ta;
@@ -1052,11 +1161,17 @@ int tc_launch_partial(const AlsArgs& a, const int32_t* items, int64_t nitems, fl
     ta.scratch = scratch;
     ta.split = split;
     ta.debug = 0;
-    BFL_CUDA(cudaMemsetAsync(scratch, 0, sizeof(float) * scratch_floats<D>() * (size_t)nslots, st));
+    if (!det) BFL_CUDA(cudaMemsetAsync(scratch, 0, sizeof(float) * scratch_floats<D>() * (size_t)nslots, st));
     const size_t smem = sizeof(Smem<D>);
     const int grid = (int)std::min<int64_t>(nitems, (int64_t)num_sms);
     for (ta.pass = 0; ta.pass < (D == 128 ? 1 : 3); ++ta.pass) {
-        if (a.compute_loss && a.axis == 1) {
+        if (det && a.compute_loss && a.axis == 1) {
+            BFL_CUDA(cudaFuncSetAttribute(als_tc_kernel<D, true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            als_tc_kernel<D, true, true, true><<<grid, THREADS, smem, st>>>(ta);
+        } else if (det) {
+            BFL_CUDA(cudaFuncSetAttribute(als_tc_kernel<D, true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            als_tc_kernel<D, true, false, true><<<grid, THREADS, smem, st>>>(ta);
+        } else if (a.compute_loss && a.axis == 1) {
             BFL_CUDA(cudaFuncSetAttribute(als_tc_kernel<D, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
             als_tc_kernel<D, true, true><<<grid, THREADS, smem, st>>>(ta);
         } else {
@@ -1068,8 +1183,9 @@ int tc_launch_partial(const AlsArgs& a, const int32_t* items, int64_t nitems, fl
     return BFL_OK;
 }
 
-// solves the rows a.row_list[a.row_begin .. a.row_end) (any length > 0) with the fused tensor-core kernel
-inline int tc_launch(const AlsArgs& a, int num_sms, cudaStream_t st) {
+// solves the rows a.row_list[a.row_begin .. a.row_end) (any length > 0) with the fused tensor-core kernel; det_loss:
+// a.loss takes per-row terms (the DET instantiations)
+inline int tc_launch(const AlsArgs& a, int num_sms, cudaStream_t st, bool det_loss = false) {
     const int64_t nrows = a.row_end - a.row_begin;
     if (nrows <= 0) return BFL_OK;
     if (!a.tc_scales) BFL_FAIL(BFL_ERR_STATE, "tensor-core ALS kernel: operand scale not prepared");
@@ -1082,7 +1198,16 @@ inline int tc_launch(const AlsArgs& a, int num_sms, cudaStream_t st) {
     ta.debug = getenv("BFL_TC_DEBUG") ? atoi(getenv("BFL_TC_DEBUG")) : 0;
     const size_t smem = sizeof(Smem<128>);
     const int grid = (int)std::min<int64_t>(nrows, (int64_t)num_sms);
-    if (a.compute_loss && a.axis == 1) {
+    if (det_loss) {
+        const size_t smem_det = sizeof(SmemDet<128>);
+        if (a.axis == 1) {
+            BFL_CUDA(cudaFuncSetAttribute(als_tc_kernel<128, false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_det));
+            als_tc_kernel<128, false, true, true><<<grid, THREADS, smem_det, st>>>(ta);
+        } else {
+            BFL_CUDA(cudaFuncSetAttribute(als_tc_kernel<128, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_det));
+            als_tc_kernel<128, false, false, true><<<grid, THREADS, smem_det, st>>>(ta);
+        }
+    } else if (a.compute_loss && a.axis == 1) {
         BFL_CUDA(cudaFuncSetAttribute(als_tc_kernel<128, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         als_tc_kernel<128, false, true><<<grid, THREADS, smem, st>>>(ta);
     } else {

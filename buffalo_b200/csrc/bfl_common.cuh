@@ -157,6 +157,56 @@ __device__ __forceinline__ int32_t draw_range(uint32_t seed, uint32_t epoch, uin
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return (uint32_t)__cvta_generic_to_shared(p);
 }
+
+// ---------------------------------------------------------------------------------------
+// Deterministic loss: per-row terms (NV doubles per row, interleaved) summed by a fixed two-stage tree whose shape
+// depends on the row count only.  Stage 1: fixed ranges of kLossRows rows, one CTA of 256 threads each.
+// ---------------------------------------------------------------------------------------
+constexpr int kLossRows = 4096;
+
+template <int NV>
+__global__ void __launch_bounds__(256) loss_tree_partial_kernel(const double* row_loss, int64_t n, double* part) {
+    __shared__ double s[NV][256];
+    const int64_t lo = (int64_t)blockIdx.x * kLossRows, hi = min(n, lo + kLossRows);
+    double t[NV];
+#pragma unroll
+    for (int v = 0; v < NV; ++v) t[v] = 0.0;
+    for (int64_t i = lo + threadIdx.x; i < hi; i += 256)
+#pragma unroll
+        for (int v = 0; v < NV; ++v) t[v] += row_loss[i * NV + v];
+#pragma unroll
+    for (int v = 0; v < NV; ++v) s[v][threadIdx.x] = t[v];
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+        if ((int)threadIdx.x < o)
+#pragma unroll
+            for (int v = 0; v < NV; ++v) s[v][threadIdx.x] += s[v][threadIdx.x + o];
+        __syncthreads();
+    }
+    if (threadIdx.x < NV) part[(int64_t)blockIdx.x * NV + threadIdx.x] = s[threadIdx.x][0];
+}
+
+// Stage 2 (one CTA of 256 threads): the partials by the same tree, added into loss[0 .. NV).
+template <int NV>
+__global__ void __launch_bounds__(256) loss_tree_final_kernel(const double* part, int64_t nblk, double* loss) {
+    __shared__ double s[NV][256];
+    double t[NV];
+#pragma unroll
+    for (int v = 0; v < NV; ++v) t[v] = 0.0;
+    for (int64_t i = threadIdx.x; i < nblk; i += 256)
+#pragma unroll
+        for (int v = 0; v < NV; ++v) t[v] += part[i * NV + v];
+#pragma unroll
+    for (int v = 0; v < NV; ++v) s[v][threadIdx.x] = t[v];
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+        if ((int)threadIdx.x < o)
+#pragma unroll
+            for (int v = 0; v < NV; ++v) s[v][threadIdx.x] += s[v][threadIdx.x + o];
+        __syncthreads();
+    }
+    if (threadIdx.x < NV) loss[threadIdx.x] += s[threadIdx.x][0];
+}
 #endif  // __CUDACC__
 
 // ---------------------------------------------------------------------------------------

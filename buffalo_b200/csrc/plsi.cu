@@ -32,7 +32,6 @@ constexpr int kColsumBlocks = 512;       // fixed partial count: the column sums
 // Entries per segment of a long item row in the deterministic item pass.  A compile-time constant, so the order of
 // every item sum depends on the data only, not on the grid, the SM count or the chunking.
 constexpr int64_t kItemSegment = 4096;
-constexpr int kLossRows = 4096;          // rows per fixed partial of the deterministic loss
 
 __device__ __forceinline__ void red4(float* p, float4 v) { atomicAdd(reinterpret_cast<float4*>(p), v); }
 
@@ -310,35 +309,6 @@ __global__ void __launch_bounds__(256) plsi_item_combine_kernel(const float* par
     }
 }
 
-// Deterministic loss, stage 1: the row losses of fixed ranges of kLossRows rows, each summed by a fixed tree.
-__global__ void __launch_bounds__(256) plsi_loss_partial_kernel(const double* row_loss, int64_t n, double* part) {
-    __shared__ double s[256];
-    const int64_t lo = (int64_t)blockIdx.x * kLossRows, hi = min(n, lo + kLossRows);
-    double t = 0.0;
-    for (int64_t i = lo + threadIdx.x; i < hi; i += 256) t += row_loss[i];
-    s[threadIdx.x] = t;
-    __syncthreads();
-    for (int o = 128; o > 0; o >>= 1) {
-        if ((int)threadIdx.x < o) s[threadIdx.x] += s[threadIdx.x + o];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) part[blockIdx.x] = s[0];
-}
-
-// Deterministic loss, stage 2 (one CTA of 256 threads): the partials by the same tree, added into *loss.
-__global__ void __launch_bounds__(256) plsi_loss_final_kernel(const double* part, int64_t nblk, double* loss) {
-    __shared__ double s[256];
-    double t = 0.0;
-    for (int64_t i = threadIdx.x; i < nblk; i += 256) t += part[i];
-    s[threadIdx.x] = t;
-    __syncthreads();
-    for (int o = 128; o > 0; o >>= 1) {
-        if ((int)threadIdx.x < o) s[threadIdx.x] += s[threadIdx.x + o];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) *loss += s[0];
-}
-
 // P rows: (row + alpha1) / sum(row + alpha1) over the d real columns (plsi.cc:115-119).  A row the last pass did not
 // write is the reference's zeroed accumulator row.  visited == null: every row is taken as it is.  G lanes per row.
 template <int G>
@@ -560,7 +530,7 @@ void launch_em_kernel(int nv4, int grid, const EmArgs& a, cudaStream_t st) {
 }
 
 // The row pass.  Deterministic mode: no item accumulation, and the loss (when a.loss is set) is the row losses of
-// the range summed by the fixed tree of plsi_loss_*_kernel, added into a.loss[0] by one thread.
+// the range summed by the fixed tree of loss_tree_*_kernel (bfl_common.cuh), added into a.loss[0] by one thread.
 int launch_em(bfl_plsi* h, EmArgs a, cudaStream_t st) {
     h->rows_done = true;
     if (a.n_rows <= 0) return BFL_OK;
@@ -577,9 +547,9 @@ int launch_em(bfl_plsi* h, EmArgs a, cudaStream_t st) {
     BFL_LAUNCHED();
     if (a.loss) {
         const int64_t nblk = (a.n_rows + kLossRows - 1) / kLossRows;
-        plsi_loss_partial_kernel<<<(unsigned)nblk, 256, 0, st>>>(h->row_loss.p, a.n_rows, h->loss_part.p);
+        loss_tree_partial_kernel<1><<<(unsigned)nblk, 256, 0, st>>>(h->row_loss.p, a.n_rows, h->loss_part.p);
         BFL_LAUNCHED();
-        plsi_loss_final_kernel<<<1, 256, 0, st>>>(h->loss_part.p, nblk, a.loss);
+        loss_tree_final_kernel<1><<<1, 256, 0, st>>>(h->loss_part.p, nblk, a.loss);
         BFL_LAUNCHED();
     }
     return BFL_OK;
