@@ -104,6 +104,16 @@ PROTOTYPES = {
     # evaluation top-k
     "bfl_topk_device": (C.c_int, [_vp, _i64, C.c_int, _vp, _i64, C.c_int, _vp, C.c_int, C.c_int, _vp, _vp, _vp]),
     "bfl_topk_host": (C.c_int, [_vp, _i64, C.c_int, _vp, _i64, C.c_int, _vp, C.c_int, C.c_int, _vp, _vp]),
+    # batch serving top-k
+    "bfl_serve_create": (_vp, []),
+    "bfl_serve_destroy": (None, [_vp]),
+    "bfl_serve_set_items": (C.c_int, [_vp, _vp, _i64, C.c_int, C.c_int, _vp]),
+    "bfl_serve_bind_items_device": (C.c_int, [_vp, _vp, _i64, C.c_int, C.c_int, _vp]),
+    "bfl_serve_set_queries": (C.c_int, [_vp, _vp, _i64, C.c_int]),
+    "bfl_serve_bind_queries_device": (C.c_int, [_vp, _vp, _i64, C.c_int]),
+    "bfl_serve_set_pool": (C.c_int, [_vp, _vp, _i64]),
+    "bfl_serve_topk": (C.c_int, [_vp, _vp, _i64, C.c_int, _vp, _vp]),
+    "bfl_serve_topk_device": (C.c_int, [_vp, _vp, _i64, C.c_int, _vp, _vp, _vp]),
     # validation metrics
     "bfl_eval_unsorted_rows_device": (C.c_int, [_vp, _vp, _i64, _vp, _vp]),
     "bfl_eval_topk_masked_device": (C.c_int, [_vp, _i64, C.c_int, _vp, _i64, C.c_int, _vp, C.c_int, C.c_int, _vp, _vp,

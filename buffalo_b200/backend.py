@@ -451,6 +451,126 @@ def topk_device(queries, items, item_bias, k, stream=None):
     return idx, val
 
 
+SERVE_KMAX = 4096
+
+
+class Serve(_Holder):
+    """Batch top-k handle (csrc/serve.cu, bfl_serve_*): the item and query factors stay on the device between calls.
+    Host arrays are uploaded once by set_items / set_queries; bind_items / bind_queries borrow torch CUDA tensors."""
+
+    def __init__(self):
+        super(Serve, self).__init__("serve")
+        self.num_items = self.num_queries = 0
+        self._d = None
+        self._bound = {}                            # device tensors the native side holds pointers to
+
+    def _destroy(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            self._fn("destroy")(h)
+        self._bound = {}
+
+    close = __del__ = _destroy
+
+    @staticmethod
+    def _matrix(a, name):
+        _host(a, np.float32, 2, name)
+        return a.ctypes.data, a.shape[0], a.shape[1]
+
+    def _items_changed(self, rows, d):
+        # the native side drops the pool and the queries with the old items
+        self.num_items, self._d, self.num_queries = rows, d, 0
+        self._bound = {}
+
+    def set_items(self, items, item_bias=None, d=None):
+        """items float32 [I, ld] host array (C-contiguous), the first d columns are used; item_bias float32 [I].
+        Clears the pool and the queries."""
+        ptr, rows, ld = self._matrix(items, "items")
+        d = ld if d is None else int(d)
+        if rows == 0 or not 0 < d <= ld:
+            raise ValueError("items must have rows and 0 < d <= its width")
+        b = None
+        if item_bias is not None:
+            b = np.ascontiguousarray(np.asarray(item_bias, dtype=np.float32).reshape(-1))
+            if b.shape[0] != rows:
+                raise ValueError("item_bias must have one value per item")
+        self._items_changed(0, None)
+        _cabi.check(self._fn("set_items")(self._h, ptr, rows, ld, d, None if b is None else b.ctypes.data), "set_items")
+        self._items_changed(rows, d)
+
+    def set_queries(self, queries):
+        """queries float32 [N, ld] host array; the array given to set_items shares its resident copy."""
+        ptr, rows, ld = self._matrix(queries, "queries")
+        if self._d is None:
+            raise ValueError("set the items before the queries")
+        if rows == 0 or ld < self._d:
+            raise ValueError("queries must have rows and at least d columns")
+        _cabi.check(self._fn("set_queries")(self._h, ptr, rows, ld), "set_queries")
+        self._bound.pop("queries", None)
+        self.num_queries = rows
+
+    def bind_items(self, items, item_bias=None, d=None):
+        """Borrows torch CUDA tensors (kept alive by this object).  Clears the pool and the queries."""
+        ptr = _dev(items, "float32", "items")
+        d = items.shape[1] if d is None else int(d)
+        b = None if item_bias is None else _dev(item_bias, "float32", "item_bias")
+        self._items_changed(0, None)
+        _cabi.check(self._fn("bind_items_device")(self._h, ptr, items.shape[0], items.stride(0), d, b), "bind_items")
+        self._items_changed(items.shape[0], d)
+        self._bound["items"] = (items, item_bias)
+
+    def bind_queries(self, queries):
+        _cabi.check(self._fn("bind_queries_device")(self._h, _dev(queries, "float32", "queries"), queries.shape[0],
+                                                    queries.stride(0)), "bind_queries")
+        self._bound["queries"] = queries
+        self.num_queries = queries.shape[0]
+
+    def set_pool(self, pool):
+        """pool: int32 indices into the items (None removes it).  An empty pool is an error."""
+        if pool is None:
+            _cabi.check(self._fn("set_pool")(self._h, None, 0), "set_pool")
+            return
+        p = np.ascontiguousarray(pool, dtype=np.int32).reshape(-1)
+        if p.size == 0:
+            raise ValueError("pool is empty")
+        if p.min() < 0 or p.max() >= self.num_items:
+            raise ValueError("pool index out of range")
+        _cabi.check(self._fn("set_pool")(self._h, p.ctypes.data, p.size), "set_pool")
+
+    @staticmethod
+    def _check_k(k):
+        k = int(k)
+        if not 1 <= k <= SERVE_KMAX:
+            raise ValueError("k must be in [1, %d]" % SERVE_KMAX)
+        return k
+
+    def topk(self, query_idx, k, want_scores=True):
+        """(int32 [n, k] item ids, float32 [n, k] scores or None) for the rows query_idx of the query matrix: best
+        first, ties to the smaller id, -1 / 0.0 where fewer than k candidates exist."""
+        k = self._check_k(k)
+        q = np.ascontiguousarray(query_idx, dtype=np.int32).reshape(-1)
+        if q.size and (q.min() < 0 or q.max() >= self.num_queries):
+            raise ValueError("query index out of range")
+        idx = np.empty((q.size, k), dtype=np.int32)
+        val = np.empty((q.size, k), dtype=np.float32) if want_scores else None
+        if q.size:
+            _cabi.check(self._fn("topk")(self._h, q.ctypes.data, q.size, k, idx.ctypes.data,
+                                         None if val is None else val.ctypes.data), "bfl_serve_topk")
+        return idx, val
+
+    def topk_device(self, query_idx, k, stream=None):
+        """torch CUDA int32 query_idx [n] -> (int32 [n, k], float32 [n, k]) CUDA tensors, stream-ordered."""
+        import torch
+        k = self._check_k(k)
+        n = query_idx.shape[0]
+        idx = torch.empty((n, k), dtype=torch.int32, device=query_idx.device)
+        val = torch.empty((n, k), dtype=torch.float32, device=query_idx.device)
+        if n:
+            _cabi.check(self._fn("topk_device")(self._h, _dev(query_idx, "int32", "query_idx"), n, k, idx.data_ptr(),
+                                                val.data_ptr(), _stream_ptr(stream)), "bfl_serve_topk_device")
+        return idx, val
+
+
 def csr_from_triples_device(major, minor, vals, num_major, num_minor, sort_minor=True, stream=None):
     """(indptr_end int64, key int32, val float32) torch CUDA tensors of one orientation from int32 major / minor and
     float32 vals CUDA tensors, through the device radix sort (bfl_csr_from_triples_device)."""

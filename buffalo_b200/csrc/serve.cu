@@ -1,0 +1,620 @@
+// Batch serving top-k on the device (DESIGN.md 4.9): the device path of buffalo.parallel's ParALS / ParBPRMF
+// (dot_topn, buffalo/parallel/_core.hpp:88-142).  A bfl_serve_t keeps the item and query factors resident and answers
+// "k best items for these n query rows" for any n, cut into batches.  Scores are bitwise those of topk_score_slice
+// (topk_common.cuh), so Algo, validation and Par* share one ranking.
+//   serve_slice_kernel : a CTA scores 32 gathered query rows against a slice of 1024 candidates.  Candidate rows (pool
+//                        indirection resolved here) are staged in shared memory in tiles through cp.async.bulk on two
+//                        mbarriers; a thread holds a 4 query x IR item register tile; each warp then radix-selects the
+//                        slice's k best for its own 4 queries without block barriers.
+//   topk_merge         : the merge of topk.cu, unchanged.
+//   serve_finish_kernel: candidate positions -> item ids through the pool, 0.0f scores on the -1 padding.
+#include <climits>
+#include <new>
+
+#include "sm90_ptx.cuh"
+#include "topk_common.cuh"
+
+using namespace bfl;
+
+namespace {
+
+constexpr int SV_THREADS = 256;
+constexpr int SV_QR = 4;                            // queries per warp (register tile rows)
+constexpr int SV_QT = SV_QR * (SV_THREADS / 32);    // queries per CTA
+constexpr int SV_SLICE = 1024;                      // candidates per CTA
+constexpr int SV_DMAX = 256;                        // widest d of the batch kernel (shared memory)
+constexpr int SV_BATCH_MAX = 16384;                 // queries per internal batch
+constexpr size_t SV_CAND_BYTES = (size_t)1 << 30;   // candidate scratch aimed at per batch
+
+// row pitch of a staged tile in floats: pitch / 4 is odd, so the float4 reads of 8 consecutive lanes (one row each) fall
+// into 8 different bank groups
+__host__ __device__ inline int tile_pitch(int dpad) { return ((dpad >> 2) & 1) ? dpad : dpad + 4; }
+
+struct ScoreCtx {
+    const float* q;      // the warp's SV_QR query rows in shared memory, pitch dpad
+    const float* t;      // the lane's first tile row; its b-th row is t + b * 32 * pitch
+    int dpad, pitch, d;
+    bool vec;
+};
+
+// Lane l's partial sum of topk_score_slice for every (query, item) of the register tile: the same columns in the same
+// order with the same fmaf nesting.
+template <int IR>
+__device__ __forceinline__ void leaf(const ScoreCtx& s, int l, float (&p)[SV_QR][IR]) {
+#pragma unroll
+    for (int a = 0; a < SV_QR; ++a)
+#pragma unroll
+        for (int b = 0; b < IR; ++b) p[a][b] = 0.f;
+    if (s.vec) {
+        for (int c = l * 4; c < s.d; c += 128) {
+            float4 x[SV_QR], v[IR];
+#pragma unroll
+            for (int a = 0; a < SV_QR; ++a) x[a] = *reinterpret_cast<const float4*>(s.q + a * s.dpad + c);
+#pragma unroll
+            for (int b = 0; b < IR; ++b) v[b] = *reinterpret_cast<const float4*>(s.t + b * 32 * s.pitch + c);
+#pragma unroll
+            for (int a = 0; a < SV_QR; ++a)
+#pragma unroll
+                for (int b = 0; b < IR; ++b)
+                    p[a][b] = fmaf(v[b].x, x[a].x, fmaf(v[b].y, x[a].y, fmaf(v[b].z, x[a].z, fmaf(v[b].w, x[a].w, p[a][b]))));
+        }
+    } else {
+        for (int c = l; c < s.d; c += 32) {
+            float x[SV_QR], v[IR];
+#pragma unroll
+            for (int a = 0; a < SV_QR; ++a) x[a] = s.q[a * s.dpad + c];
+#pragma unroll
+            for (int b = 0; b < IR; ++b) v[b] = s.t[b * 32 * s.pitch + c];
+#pragma unroll
+            for (int a = 0; a < SV_QR; ++a)
+#pragma unroll
+                for (int b = 0; b < IR; ++b) p[a][b] = fmaf(v[b], x[a], p[a][b]);
+        }
+    }
+}
+
+// warp_sum's butterfly (offsets 16, 8, 4, 2, 1) as an expression tree over the 32 lane partials: the sum over the lanes
+// whose low NB bits are X is the sum of the two halves that differ in bit NB.  tree<0, 0> is lane 0's warp_sum.
+template <int NB, int X, int IR>
+__device__ __forceinline__ void tree(const ScoreCtx& s, float (&out)[SV_QR][IR]) {
+    if constexpr (NB == 5) {
+        leaf<IR>(s, X, out);
+    } else {
+        float hi[SV_QR][IR];
+        tree<NB + 1, X, IR>(s, out);
+        tree<NB + 1, X | (1 << NB), IR>(s, hi);
+#pragma unroll
+        for (int a = 0; a < SV_QR; ++a)
+#pragma unroll
+            for (int b = 0; b < IR; ++b) out[a][b] = out[a][b] + hi[a][b];
+    }
+}
+
+// One warp: the k largest of vals[0..n) -> (out_v, out_i)[0..k) unordered, index = idx0 + position, ties at the k-th
+// value to the smaller position.  The selection of block_select (topk.cu) at warp scope, so that the 8 warps of a CTA
+// select for 8 queries at once with no block barrier.  hist: 256 counters of the warp.
+__device__ void warp_select(const float* vals, int idx0, int n, int k, float* out_v, int32_t* out_i, unsigned* hist) {
+    const int lane = threadIdx.x & 31;
+    if (n <= k) {
+        for (int i = lane; i < k; i += 32) {
+            out_v[i] = i < n ? vals[i] : -INFINITY;
+            out_i[i] = i < n ? idx0 + i : -1;
+        }
+        return;
+    }
+    uint32_t prefix = 0, mask = 0;
+    unsigned kk = (unsigned)k;
+    for (int shift = 24; shift >= 0; shift -= 8) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) hist[lane + 32 * j] = 0;
+        __syncwarp();
+        for (int i = lane; i < n; i += 32) {
+            const uint32_t u = ord_of(vals[i]);
+            if ((u & mask) == prefix) atomicAdd(&hist[(u >> shift) & 255u], 1u);
+        }
+        __syncwarp();
+        // lane owns bins 8 lane .. 8 lane + 7; suf = matches in its bins and all higher ones
+        unsigned loc[8], own = 0;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            loc[j] = hist[8 * lane + j];
+            own += loc[j];
+        }
+        unsigned suf = own;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned t = __shfl_down_sync(FULL, suf, o);
+            if (lane + o < 32) suf += t;
+        }
+        // the k-th largest is in the one lane with (suf - own) < kk <= suf
+        const bool mine = suf - own < kk && kk <= suf;
+        unsigned bin = 0, left = 0;
+        if (mine) {
+            unsigned cum = suf - own;
+            int b = 7;
+            for (; b > 0; --b) {
+                if (cum + loc[b] >= kk) break;
+                cum += loc[b];
+            }
+            bin = 8u * lane + b;
+            left = kk - cum;                        // still needed inside the bin
+        }
+        const int src = __ffs(__ballot_sync(FULL, mine)) - 1;
+        bin = __shfl_sync(FULL, bin, src);
+        kk = __shfl_sync(FULL, left, src);
+        prefix |= bin << shift;
+        mask |= 255u << shift;
+        __syncwarp();
+    }
+    const uint32_t T = prefix;                      // kk ties to take; k - kk elements are strictly larger
+    unsigned n_gt = 0, n_tie = 0;
+    const unsigned below = (1u << lane) - 1u;
+    for (int i0 = 0; i0 < n; i0 += 32) {
+        const int i = i0 + lane;
+        const float v = i < n ? vals[i] : 0.f;
+        const uint32_t u = ord_of(v);
+        const bool gt = i < n && u > T, tie = i < n && u == T;
+        const unsigned bg = __ballot_sync(FULL, gt), bt = __ballot_sync(FULL, tie);
+        if (gt) {
+            const unsigned pos = n_gt + __popc(bg & below);
+            out_v[pos] = v;
+            out_i[pos] = idx0 + i;
+        }
+        const unsigned r = n_tie + __popc(bt & below);
+        if (tie && r < kk) {
+            out_v[(k - kk) + r] = v;
+            out_i[(k - kk) + r] = idx0 + i;
+        }
+        n_gt += __popc(bg);
+        n_tie += __popc(bt);
+    }
+}
+
+// Qm rows are gathered through qidx (an index outside [0, n_qrows) reads as a zero row); candidate c of the slice is
+// item row pool[c] (or c).  cand_i holds candidate POSITIONS (so ties resolve as on a gathered item matrix).
+template <int IR>
+__global__ void __launch_bounds__(SV_THREADS)
+    serve_slice_kernel(const float* __restrict__ Qm, int64_t n_qrows, int ldq, const int32_t* __restrict__ qidx, int nq,
+                       const float* __restrict__ It, int ldi, int64_t n_cand, const int32_t* __restrict__ pool,
+                       const float* __restrict__ bias, int d, int k, int nslices, int bulk, int tile_floats,
+                       float* __restrict__ cand_v, int32_t* __restrict__ cand_i) {
+    constexpr int IT = 32 * IR;
+    extern __shared__ __align__(128) float sv_smem[];
+    __shared__ __align__(8) uint64_t bar[2];
+    const int dpad = (d + 3) & ~3, pitch = tile_pitch(dpad);
+    float* scores = sv_smem;                        // [SV_QT][SV_SLICE]
+    float* qs = scores + SV_QT * SV_SLICE;          // [SV_QT][dpad]
+    float* tiles = qs + SV_QT * dpad;               // [2][tile_floats]; the select histograms afterwards
+    const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+    const int slice = blockIdx.x;
+    const int q0 = blockIdx.y * SV_QT;
+    const int64_t i0 = (int64_t)slice * SV_SLICE;
+    const int ni = (int)min((long long)SV_SLICE, (long long)(n_cand - i0));
+    const int ntiles = (ni + IT - 1) / IT;
+
+    if (tid == 0) {
+        sm90::mbar_init(&bar[0], 1);
+        sm90::mbar_init(&bar[1], 1);
+        sm90::mbar_init_fence();
+    }
+    for (int e = tid; e < SV_QT * dpad; e += SV_THREADS) {
+        const int qi = e / dpad, c = e - qi * dpad;
+        float v = 0.f;
+        if (q0 + qi < nq && c < d) {
+            const int64_t r = qidx[q0 + qi];
+            if (r >= 0 && r < n_qrows) v = Qm[r * ldq + c];
+        }
+        qs[e] = v;
+    }
+    __syncthreads();
+
+    // warp 0 stages tile t with one bulk copy per row, all completing on bar[t & 1]
+    auto stage_bulk = [&](int t) {
+        const int nt = min(IT, ni - t * IT);
+        float* dst = tiles + (t & 1) * tile_floats;
+        if (lane == 0) sm90::mbar_arrive_expect_tx(&bar[t & 1], (uint32_t)nt * d * 4u);
+        __syncwarp();
+        for (int j = lane; j < nt; j += 32) {
+            const int64_t c = i0 + t * IT + j;
+            const int64_t row = pool ? pool[c] : c;
+            sm90::cp_async_bulk_g2s(dst + j * pitch, It + row * ldi, (uint32_t)d * 4u, &bar[t & 1]);
+        }
+    };
+    if (bulk && w == 0) stage_bulk(0);
+
+    ScoreCtx s;
+    s.q = qs + w * SV_QR * dpad;
+    s.dpad = dpad;
+    s.pitch = pitch;
+    s.d = d;
+    s.vec = (ldi & 3) == 0 && (d & 3) == 0;
+    for (int t = 0; t < ntiles; ++t) {
+        float* tile = tiles + (t & 1) * tile_floats;
+        if (bulk) {
+            if (w == 0 && t + 1 < ntiles) stage_bulk(t + 1);   // its buffer was released by the barrier ending tile t - 1
+            sm90::mbar_wait(&bar[t & 1], (t >> 1) & 1);
+        } else {
+            const int nt = min(IT, ni - t * IT);
+            for (int e = tid; e < nt * d; e += SV_THREADS) {
+                const int j = e / d, c = e - j * d;
+                const int64_t cp = i0 + t * IT + j;
+                const int64_t row = pool ? pool[cp] : cp;
+                tile[j * pitch + c] = It[row * ldi + c];
+            }
+            __syncthreads();
+        }
+        s.t = tile + lane * pitch;
+        float acc[SV_QR][IR];
+        tree<0, 0, IR>(s, acc);
+#pragma unroll
+        for (int b = 0; b < IR; ++b) {
+            const int it = t * IT + b * 32 + lane;
+            if (it < ni) {
+                float bv = 0.f;
+                if (bias) bv = bias[pool ? (int64_t)pool[i0 + it] : i0 + it];
+#pragma unroll
+                for (int a = 0; a < SV_QR; ++a) scores[(w * SV_QR + a) * SV_SLICE + it] = acc[a][b] + bv;
+            }
+        }
+        __syncthreads();
+    }
+    unsigned* hist = reinterpret_cast<unsigned*>(tiles) + w * 256;
+    for (int a = 0; a < SV_QR; ++a) {
+        const int q = q0 + w * SV_QR + a;
+        if (q >= nq) break;
+        const size_t o = ((size_t)q * nslices + slice) * k;
+        warp_select(scores + (w * SV_QR + a) * SV_SLICE, (int)i0, ni, k, cand_v + o, cand_i + o, hist);
+        __syncwarp();
+    }
+}
+
+__global__ void serve_finish_kernel(int32_t* __restrict__ idx, float* __restrict__ val, size_t n,
+                                    const int32_t* __restrict__ pool) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int32_t c = idx[i];
+    if (c < 0) {
+        val[i] = 0.f;
+    } else if (pool) {
+        idx[i] = pool[c];
+    }
+}
+
+// dst[r] = src[idx[r]] for rows of d floats (pitch ld on both sides, padding columns zero)
+__global__ void serve_gather_rows_kernel(const float* __restrict__ src, int64_t n_src, int ld, const int32_t* __restrict__ idx,
+                                         int64_t n, int d, float* __restrict__ dst) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n * ld) return;
+    const int64_t r = e / ld;
+    const int c = (int)(e - r * ld);
+    const int64_t s = idx[r];
+    dst[e] = (c < d && s >= 0 && s < n_src) ? src[s * ld + c] : 0.f;
+}
+
+size_t slice_smem_bytes(int d, int IR, int* tile_floats) {
+    const int dpad = (d + 3) & ~3;
+    int tf = 32 * IR * tile_pitch(dpad);
+    if (2 * tf < (SV_THREADS / 32) * 256) tf = (SV_THREADS / 32) * 128;   // room for the select histograms
+    *tile_floats = tf;
+    return sizeof(float) * ((size_t)SV_QT * SV_SLICE + (size_t)SV_QT * dpad + 2 * (size_t)tf);
+}
+
+}  // namespace
+
+struct bfl_serve {
+    // items / queries: owned uploads of host arrays, or borrowed device memory
+    DevBuf<float> own_items, own_bias, own_queries;
+    const float *items = nullptr, *bias = nullptr, *queries = nullptr;
+    const float* host_items = nullptr;              // the host array own_items mirrors (alias check of set_queries)
+    int64_t n_items = 0, n_q = 0;
+    int ldi = 0, ldq = 0, d = 0;
+    DevBuf<int32_t> pool;
+    int64_t n_pool = -1;                            // -1: no pool
+
+    int num_sms = 0;
+    cudaStream_t compute = nullptr, copy = nullptr;
+    cudaEvent_t scored[2] = {nullptr, nullptr}, copied[2] = {nullptr, nullptr};
+    DevBuf<float> cand_v;
+    DevBuf<int32_t> cand_i;
+    DevBuf<int32_t> qidx;
+    DevBuf<int32_t> out_i[2];
+    DevBuf<float> out_v[2];
+    DevBuf<float> gq, gi, gb;                       // gathered rows for the widths the batch kernel does not take
+    int32_t* pin_i[2] = {nullptr, nullptr};
+    float* pin_v[2] = {nullptr, nullptr};
+    size_t pin_cap = 0;
+
+    int attach() {
+        if (compute) return BFL_OK;
+        if (BFL_OK != require_device()) return BFL_ERR_CUDA;
+        int dev = 0;
+        BFL_CUDA(cudaGetDevice(&dev));
+        BFL_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
+        BFL_CUDA(cudaStreamCreateWithFlags(&compute, cudaStreamNonBlocking));
+        BFL_CUDA(cudaStreamCreateWithFlags(&copy, cudaStreamNonBlocking));
+        for (int s = 0; s < 2; ++s) {
+            BFL_CUDA(cudaEventCreateWithFlags(&scored[s], cudaEventDisableTiming));
+            BFL_CUDA(cudaEventCreateWithFlags(&copied[s], cudaEventDisableTiming));
+        }
+        return BFL_OK;
+    }
+    int reserve_pinned(size_t n) {
+        if (n <= pin_cap) return BFL_OK;
+        release_pinned();
+        for (int s = 0; s < 2; ++s) {
+            BFL_CUDA(cudaMallocHost(&pin_i[s], n * sizeof(int32_t)));
+            BFL_CUDA(cudaMallocHost(&pin_v[s], n * sizeof(float)));
+        }
+        pin_cap = n;
+        return BFL_OK;
+    }
+    void release_pinned() {
+        for (int s = 0; s < 2; ++s) {
+            if (pin_i[s]) cudaFreeHost(pin_i[s]);
+            if (pin_v[s]) cudaFreeHost(pin_v[s]);
+            pin_i[s] = nullptr;
+            pin_v[s] = nullptr;
+        }
+        pin_cap = 0;
+    }
+    ~bfl_serve() {
+        if (compute) cudaStreamSynchronize(compute);
+        if (copy) cudaStreamSynchronize(copy);
+        release_pinned();
+        for (int s = 0; s < 2; ++s) {
+            if (scored[s]) cudaEventDestroy(scored[s]);
+            if (copied[s]) cudaEventDestroy(copied[s]);
+        }
+        if (compute) cudaStreamDestroy(compute);
+        if (copy) cudaStreamDestroy(copy);
+    }
+
+    // new items invalidate what was set relative to the old ones: the pool and the queries (which may alias the old
+    // item buffer or be narrower than the new d)
+    void items_changed() {
+        n_pool = -1;
+        own_queries.release();
+        queries = nullptr;
+        n_q = 0;
+        ldq = 0;
+    }
+    int64_t n_cand() const { return n_pool >= 0 ? n_pool : n_items; }
+    // The one place that picks the kernels for a batch of nb queries.  The batch kernel takes every width its
+    // shared-memory tiles hold, except a call of fewer queries than one CTA's tile over more slices than the card has
+    // SMs: such a call runs whole waves of mostly empty 32-query CTAs, and the 4-query kernels of topk.cu on gathered
+    // rows answer it sooner (benchmarks/serve_bench.py --small, DESIGN.md 4.9).  Wider rows always go there.
+    bool batch_kernel(int64_t nb) const {
+        return d <= SV_DMAX && (nb >= SV_QT || (n_cand() + SV_SLICE - 1) / SV_SLICE <= num_sms);
+    }
+    int slice_len() const { return d <= SV_DMAX ? SV_SLICE : TK_SLICE; }
+    // queries per internal batch for this k: the candidate scratch stays near SV_CAND_BYTES
+    int64_t batch_rows(int k) const {
+        const int64_t nsl = (n_cand() + slice_len() - 1) / slice_len();
+        int64_t b = (int64_t)(SV_CAND_BYTES / ((size_t)nsl * k * 8));
+        b = b / SV_QT * SV_QT;
+        return b < SV_QT ? SV_QT : (b > SV_BATCH_MAX ? SV_BATCH_MAX : b);
+    }
+    int check_ready(int64_t n, int k, const void* a, const void* b) {
+        if (!items || !queries) BFL_FAIL(BFL_ERR_STATE, "serve: set the items and the queries before topk");
+        if (!a || !b || n <= 0) BFL_FAIL(BFL_ERR_ARG, "bad serve top-k arguments");
+        if (k <= 0 || k > TK_KMAX) BFL_FAIL(BFL_ERR_ARG, "top-k: k must be in [1, 4096]");
+        const int64_t nsl = (n_cand() + slice_len() - 1) / slice_len();
+        if (nsl * k > INT_MAX) BFL_FAIL(BFL_ERR_ARG, "serve: too many candidates for this k");
+        return BFL_OK;
+    }
+    // one batch, stream-ordered: d_qidx[0..nb) -> d_out_i / d_out_v [nb x k]
+    int run_batch(const int32_t* d_qidx, int64_t nb, int k, int32_t* d_out_i, float* d_out_v, cudaStream_t st);
+};
+
+int bfl_serve::run_batch(const int32_t* d_qidx, int64_t nb, int k, int32_t* d_out_i, float* d_out_v, cudaStream_t st) {
+    const int64_t nc = n_cand();
+    const int32_t* dpool = n_pool >= 0 ? pool.p : nullptr;
+    if (!batch_kernel(nb)) {
+        const int ew = 256;
+        if (BFL_OK != gq.reserve((size_t)nb * ldq)) return BFL_ERR_CUDA;
+        serve_gather_rows_kernel<<<(unsigned)((nb * ldq + ew - 1) / ew), ew, 0, st>>>(queries, n_q, ldq, d_qidx, nb, d, gq.p);
+        BFL_LAUNCHED();
+        const float *it = items, *bs = bias;
+        if (dpool) {
+            if (BFL_OK != gi.reserve((size_t)nc * ldi)) return BFL_ERR_CUDA;
+            serve_gather_rows_kernel<<<(unsigned)((nc * ldi + ew - 1) / ew), ew, 0, st>>>(items, n_items, ldi, dpool, nc, d, gi.p);
+            BFL_LAUNCHED();
+            it = gi.p;
+            if (bias) {
+                if (BFL_OK != gb.reserve((size_t)nc)) return BFL_ERR_CUDA;
+                serve_gather_rows_kernel<<<(unsigned)((nc + ew - 1) / ew), ew, 0, st>>>(bias, n_items, 1, dpool, nc, 1, gb.p);
+                BFL_LAUNCHED();
+                bs = gb.p;
+            }
+        }
+        const int rc = bfl_topk_device(gq.p, nb, ldq, it, nc, ldi, bs, d, k, d_out_i, d_out_v, st);
+        if (rc != BFL_OK) return rc;
+    } else {
+        const int nslices = (int)((nc + SV_SLICE - 1) / SV_SLICE);
+        const int ncand = nslices * k;
+        if (BFL_OK != cand_v.reserve((size_t)nb * ncand) || BFL_OK != cand_i.reserve((size_t)nb * ncand))
+            return BFL_ERR_CUDA;
+        const int IR = d <= 128 ? 2 : 1;
+        int tile_floats = 0;
+        const size_t smem = slice_smem_bytes(d, IR, &tile_floats);
+        // bulk copies need 16-byte aligned rows of a multiple of 16 bytes (bind_items_device checks the base address);
+        // other row shapes are staged with plain loads
+        const int bulk = (ldi & 3) == 0 && (d & 3) == 0;
+        auto kern = IR == 2 ? serve_slice_kernel<2> : serve_slice_kernel<1>;
+        BFL_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        dim3 grid(nslices, (unsigned)((nb + SV_QT - 1) / SV_QT));
+        kern<<<grid, SV_THREADS, smem, st>>>(queries, n_q, ldq, d_qidx, (int)nb, items, ldi, nc, dpool, bias, d, k, nslices,
+                                             bulk, tile_floats, cand_v.p, cand_i.p);
+        BFL_LAUNCHED();
+        const int rc = topk_merge(cand_v.p, cand_i.p, nb, ncand, k, d_out_i, d_out_v, st);
+        if (rc != BFL_OK) return rc;
+    }
+    const size_t n = (size_t)nb * k;
+    serve_finish_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_out_i, d_out_v, n, dpool);
+    BFL_LAUNCHED();
+    return BFL_OK;
+}
+
+extern "C" {
+
+bfl_serve_t* bfl_serve_create(void) { return new (std::nothrow) bfl_serve(); }
+
+void bfl_serve_destroy(bfl_serve_t* h) { delete h; }
+
+static int check_matrix(const void* p, int64_t rows, int ld, int d) {
+    if (!p || rows <= 0 || d <= 0 || ld < d) BFL_FAIL(BFL_ERR_ARG, "serve: bad matrix arguments");
+    if (rows > INT_MAX) BFL_FAIL(BFL_ERR_ARG, "serve: the row count must be below 2^31");
+    return BFL_OK;
+}
+
+int bfl_serve_bind_items_device(bfl_serve_t* h, const float* d_items, int64_t n_items, int ld, int d,
+                                const float* d_item_bias) {
+    if (!h) BFL_FAIL(BFL_ERR_ARG, "serve: null handle");
+    if (BFL_OK != check_matrix(d_items, n_items, ld, d)) return BFL_ERR_ARG;
+    // aligned-shaped rows are read 16 bytes at a time (float4 loads, bulk copies), as topk_score_slice reads them
+    if ((ld & 3) == 0 && (d & 3) == 0 && ((uintptr_t)d_items & 15) != 0)
+        BFL_FAIL(BFL_ERR_ARG, "serve: device item rows of a multiple of 4 floats must be 16-byte aligned");
+    if (BFL_OK != h->attach()) return BFL_ERR_CUDA;
+    h->items_changed();
+    h->items = nullptr;
+    h->own_items.release();
+    h->own_bias.release();
+    h->host_items = nullptr;
+    h->items = d_items;
+    h->bias = d_item_bias;
+    h->n_items = n_items;
+    h->ldi = ld;
+    h->d = d;
+    return BFL_OK;
+}
+
+int bfl_serve_set_items(bfl_serve_t* h, const float* items, int64_t n_items, int ld, int d, const float* item_bias) {
+    if (!h) BFL_FAIL(BFL_ERR_ARG, "serve: null handle");
+    if (BFL_OK != check_matrix(items, n_items, ld, d)) return BFL_ERR_ARG;
+    if (BFL_OK != h->attach()) return BFL_ERR_CUDA;
+    h->items_changed();
+    h->items = nullptr;                             // stays unset if the upload below fails
+    if (BFL_OK != h->own_items.reserve((size_t)n_items * ld)) return BFL_ERR_CUDA;
+    BFL_CUDA(cudaMemcpy(h->own_items.p, items, sizeof(float) * (size_t)n_items * ld, cudaMemcpyHostToDevice));
+    if (item_bias) {
+        if (BFL_OK != h->own_bias.reserve((size_t)n_items)) return BFL_ERR_CUDA;
+        BFL_CUDA(cudaMemcpy(h->own_bias.p, item_bias, sizeof(float) * (size_t)n_items, cudaMemcpyHostToDevice));
+    }
+    h->host_items = items;
+    h->items = h->own_items.p;
+    h->bias = item_bias ? h->own_bias.p : nullptr;
+    h->n_items = n_items;
+    h->ldi = ld;
+    h->d = d;
+    return BFL_OK;
+}
+
+int bfl_serve_bind_queries_device(bfl_serve_t* h, const float* d_queries, int64_t n_q, int ld) {
+    if (!h) BFL_FAIL(BFL_ERR_ARG, "serve: null handle");
+    if (!h->items) BFL_FAIL(BFL_ERR_STATE, "serve: set the items before the queries");
+    if (BFL_OK != check_matrix(d_queries, n_q, ld, h->d)) return BFL_ERR_ARG;
+    h->own_queries.release();
+    h->queries = d_queries;
+    h->n_q = n_q;
+    h->ldq = ld;
+    return BFL_OK;
+}
+
+int bfl_serve_set_queries(bfl_serve_t* h, const float* queries, int64_t n_q, int ld) {
+    if (!h) BFL_FAIL(BFL_ERR_ARG, "serve: null handle");
+    if (!h->items) BFL_FAIL(BFL_ERR_STATE, "serve: set the items before the queries");
+    if (BFL_OK != check_matrix(queries, n_q, ld, h->d)) return BFL_ERR_ARG;
+    if (queries == h->host_items && n_q == h->n_items && ld == h->ldi) {   // most_similar: one resident copy
+        h->own_queries.release();
+        h->queries = h->items;
+    } else {
+        if (BFL_OK != h->own_queries.reserve((size_t)n_q * ld)) return BFL_ERR_CUDA;
+        BFL_CUDA(cudaMemcpy(h->own_queries.p, queries, sizeof(float) * (size_t)n_q * ld, cudaMemcpyHostToDevice));
+        h->queries = h->own_queries.p;
+    }
+    h->n_q = n_q;
+    h->ldq = ld;
+    return BFL_OK;
+}
+
+int bfl_serve_set_pool(bfl_serve_t* h, const int32_t* pool_idx, int64_t n_pool) {
+    if (!h) BFL_FAIL(BFL_ERR_ARG, "serve: null handle");
+    if (!h->items) BFL_FAIL(BFL_ERR_STATE, "serve: set the items before the pool");
+    if (!pool_idx) {
+        h->n_pool = -1;
+        return BFL_OK;
+    }
+    if (n_pool <= 0) BFL_FAIL(BFL_ERR_ARG, "serve: pool is empty");
+    if (n_pool > INT_MAX) BFL_FAIL(BFL_ERR_ARG, "serve: the pool must hold fewer than 2^31 indices");
+    for (int64_t i = 0; i < n_pool; ++i)
+        if (pool_idx[i] < 0 || pool_idx[i] >= h->n_items) BFL_FAIL(BFL_ERR_ARG, "serve: pool index out of range");
+    if (BFL_OK != h->pool.reserve((size_t)n_pool)) return BFL_ERR_CUDA;
+    BFL_CUDA(cudaMemcpy(h->pool.p, pool_idx, sizeof(int32_t) * (size_t)n_pool, cudaMemcpyHostToDevice));
+    h->n_pool = n_pool;
+    return BFL_OK;
+}
+
+int bfl_serve_topk_device(bfl_serve_t* h, const int32_t* d_query_idx, int64_t n, int k, int32_t* d_out_idx,
+                          float* d_out_val, void* stream) {
+    if (!h) BFL_FAIL(BFL_ERR_ARG, "serve: null handle");
+    int rc = h->check_ready(n, k, d_query_idx, d_out_idx);
+    if (rc != BFL_OK) return rc;
+    if (!d_out_val) BFL_FAIL(BFL_ERR_ARG, "serve: the device variant needs d_out_val");
+    const int64_t B = h->batch_rows(k);
+    for (int64_t b0 = 0; b0 < n; b0 += B) {
+        const int64_t nb = n - b0 < B ? n - b0 : B;
+        rc = h->run_batch(d_query_idx + b0, nb, k, d_out_idx + b0 * k, d_out_val + b0 * k, (cudaStream_t)stream);
+        if (rc != BFL_OK) return rc;
+    }
+    return BFL_OK;
+}
+
+int bfl_serve_topk(bfl_serve_t* h, const int32_t* query_idx, int64_t n, int k, int32_t* out_idx, float* out_val) {
+    if (!h) BFL_FAIL(BFL_ERR_ARG, "serve: null handle");
+    int rc = h->check_ready(n, k, query_idx, out_idx);
+    if (rc != BFL_OK) return rc;
+    for (int64_t i = 0; i < n; ++i)
+        if (query_idx[i] < 0 || query_idx[i] >= h->n_q) BFL_FAIL(BFL_ERR_ARG, "serve: query index out of range");
+    const int64_t B = h->batch_rows(k) < n ? h->batch_rows(k) : n;
+    const size_t per = (size_t)B * k;
+    if (BFL_OK != h->qidx.reserve((size_t)n) || BFL_OK != h->reserve_pinned(per)) return BFL_ERR_CUDA;
+    for (int s = 0; s < 2; ++s)
+        if (BFL_OK != h->out_i[s].reserve(per) || BFL_OK != h->out_v[s].reserve(per)) return BFL_ERR_CUDA;
+    BFL_CUDA(cudaMemcpyAsync(h->qidx.p, query_idx, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, h->compute));
+    // batch b is scored on `compute` into slot b & 1 and copied to that slot's pinned buffers on `copy`; the host
+    // drains batch b - 1 into the caller's arrays while batch b runs
+    auto drain = [&](int64_t b) -> int {
+        const int s = (int)(b & 1);
+        const int64_t b0 = b * B, nb = n - b0 < B ? n - b0 : B;
+        BFL_CUDA(cudaEventSynchronize(h->copied[s]));
+        memcpy(out_idx + b0 * k, h->pin_i[s], sizeof(int32_t) * (size_t)nb * k);
+        if (out_val) memcpy(out_val + b0 * k, h->pin_v[s], sizeof(float) * (size_t)nb * k);
+        return BFL_OK;
+    };
+    const int64_t nbatch = (n + B - 1) / B;
+    for (int64_t b = 0; b < nbatch; ++b) {
+        const int s = (int)(b & 1);
+        const int64_t b0 = b * B, nb = n - b0 < B ? n - b0 : B;
+        rc = h->run_batch(h->qidx.p + b0, nb, k, h->out_i[s].p, h->out_v[s].p, h->compute);
+        if (rc == BFL_OK) {
+            BFL_CUDA(cudaEventRecord(h->scored[s], h->compute));
+            BFL_CUDA(cudaStreamWaitEvent(h->copy, h->scored[s], 0));
+            BFL_CUDA(cudaMemcpyAsync(h->pin_i[s], h->out_i[s].p, sizeof(int32_t) * (size_t)nb * k, cudaMemcpyDeviceToHost,
+                                     h->copy));
+            BFL_CUDA(cudaMemcpyAsync(h->pin_v[s], h->out_v[s].p, sizeof(float) * (size_t)nb * k, cudaMemcpyDeviceToHost,
+                                     h->copy));
+            BFL_CUDA(cudaEventRecord(h->copied[s], h->copy));
+            if (b > 0) rc = drain(b - 1);
+        }
+        if (rc != BFL_OK) {   // leave nothing in flight behind a failed call
+            cudaStreamSynchronize(h->compute);
+            cudaStreamSynchronize(h->copy);
+            return rc;
+        }
+    }
+    rc = drain(nbatch - 1);
+    BFL_CUDA(cudaStreamSynchronize(h->compute));
+    return rc;
+}
+
+}  // extern "C"

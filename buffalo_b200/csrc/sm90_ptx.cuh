@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for the sm_90a features the tensor-core ALS kernel uses: mbarrier, cp.async (SASS LDGSTS)
-// and warpgroup MMA (wgmma.mma_async, SASS HGMMA) with shared-memory matrix descriptors.  No CUTLASS: every string
+// Thin inline-PTX wrappers for the sm_90a features the tensor-core ALS kernel and the batch top-k kernel use: mbarrier,
+// cp.async (SASS LDGSTS), cp.async.bulk and warpgroup MMA (wgmma.mma_async, SASS HGMMA) with shared-memory matrix descriptors.  No CUTLASS: every string
 // below is plain PTX ISA 8.x.
 #pragma once
 #include <cuda_runtime.h>
@@ -37,6 +37,19 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 // issue slots from the working warps of its scheduler
 __device__ __forceinline__ void mbar_wait_idle(uint64_t* bar, uint32_t parity) {
     while (!mbar_try_wait(bar, parity)) __nanosleep(128);
+}
+
+// transaction-count completion: one arrival that also announces `bytes` of bulk-copy traffic for the current phase
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(s32(bar)), "r"(bytes) : "memory");
+}
+// bulk asynchronous copy global -> shared (SASS UBLKCP): 16-byte aligned addresses, size a multiple of 16; its bytes
+// complete on `bar`
+__device__ __forceinline__ void cp_async_bulk_g2s(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
+                     s32(smem_dst)),
+                 "l"(gsrc), "r"(bytes), "r"(s32(bar))
+                 : "memory");
 }
 
 // generic-proxy writes to shared memory -> visible to the async proxy (tensor-core operand reads)

@@ -165,6 +165,23 @@ __global__ void __launch_bounds__(TK_THREADS) topk_merge_kernel(const float* __r
 
 }  // namespace
 
+int bfl::topk_merge(const float* cand_v, const int32_t* cand_i, int64_t nq, int ncand, int k, int32_t* out_idx,
+                    float* out_val, cudaStream_t st) {
+    float* sel_v = nullptr;
+    int32_t* sel_i = nullptr;
+    const size_t ns = (size_t)nq * k;
+    BFL_CUDA(cudaMallocAsync(&sel_v, ns * sizeof(float), st));
+    BFL_CUDA(cudaMallocAsync(&sel_i, ns * sizeof(int32_t), st));
+    int kpad = 2;
+    while (kpad < k) kpad <<= 1;
+    topk_merge_kernel<<<(unsigned)nq, TK_THREADS, kpad * sizeof(unsigned long long), st>>>(cand_v, cand_i, ncand, k, kpad,
+                                                                                          sel_v, sel_i, out_idx, out_val);
+    BFL_LAUNCHED();
+    BFL_CUDA(cudaFreeAsync(sel_v, st));
+    BFL_CUDA(cudaFreeAsync(sel_i, st));
+    return BFL_OK;
+}
+
 extern "C" {
 
 // all pointers are device pointers; out_idx [nq x k] (best first, -1 = fewer than k items), out_val [nq x k]
@@ -179,13 +196,9 @@ int bfl_topk_device(const float* queries, int64_t nq, int ldq, const float* item
     const int ncand = nslices * k;
     float* cand_v = nullptr;
     int32_t* cand_i = nullptr;
-    float* sel_v = nullptr;
-    int32_t* sel_i = nullptr;
-    const size_t nc = (size_t)nq * ncand, ns = (size_t)nq * k;
+    const size_t nc = (size_t)nq * ncand;
     BFL_CUDA(cudaMallocAsync(&cand_v, nc * sizeof(float), st));
     BFL_CUDA(cudaMallocAsync(&cand_i, nc * sizeof(int32_t), st));
-    BFL_CUDA(cudaMallocAsync(&sel_v, ns * sizeof(float), st));
-    BFL_CUDA(cudaMallocAsync(&sel_i, ns * sizeof(int32_t), st));
     const int dpad = (d + 3) & ~3;
     const size_t smem1 = sizeof(float) * ((size_t)TK_QB * TK_SLICE + (size_t)TK_QB * dpad);
     BFL_CUDA(cudaFuncSetAttribute(topk_slice_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
@@ -193,16 +206,10 @@ int bfl_topk_device(const float* queries, int64_t nq, int ldq, const float* item
     topk_slice_kernel<<<grid, TK_THREADS, smem1, st>>>(queries, nq, ldq, items, n_items, ldi, item_bias, d, k, nslices,
                                                        cand_v, cand_i);
     BFL_LAUNCHED();
-    int kpad = 2;
-    while (kpad < k) kpad <<= 1;
-    topk_merge_kernel<<<(unsigned)nq, TK_THREADS, kpad * sizeof(unsigned long long), st>>>(cand_v, cand_i, ncand, k, kpad,
-                                                                                          sel_v, sel_i, out_idx, out_val);
-    BFL_LAUNCHED();
+    const int rc = topk_merge(cand_v, cand_i, nq, ncand, k, out_idx, out_val, st);
     BFL_CUDA(cudaFreeAsync(cand_v, st));
     BFL_CUDA(cudaFreeAsync(cand_i, st));
-    BFL_CUDA(cudaFreeAsync(sel_v, st));
-    BFL_CUDA(cudaFreeAsync(sel_i, st));
-    return BFL_OK;
+    return rc;
 }
 
 // host pointers: copies queries / items / bias to the device, runs bfl_topk_device, copies the result back

@@ -63,4 +63,9 @@ __device__ __forceinline__ void topk_score_slice(const float* __restrict__ Qr, i
     __syncthreads();
 }
 
+// topk.cu: per query, the k best of its ncand candidates (score, index; index -1 = empty) ordered best first, ties to
+// the smaller index, into out_idx / out_val [nq x k] (-1 / -inf where fewer than k candidates exist).  Stream-ordered.
+int topk_merge(const float* cand_v, const int32_t* cand_i, int64_t nq, int ncand, int k, int32_t* out_idx, float* out_val,
+               cudaStream_t st);
+
 }  // namespace bfl

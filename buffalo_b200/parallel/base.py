@@ -1,7 +1,10 @@
-"""Batch query helpers (buffalo/parallel/base.py): ParALS / ParBPRMF.  Serving-side brute-force MIPS is outside
-the training hot path (SURVEY.md 2.1 #10); this is a NumPy implementation of the same interface
-(dot_topn semantics of buffalo/parallel/_core.hpp:88-142: best-first indexes, -1 padded)."""
+"""Batch query helpers (buffalo/parallel/base.py): ParALS / ParBPRMF, the dot_topn semantics of
+buffalo/parallel/_core.hpp:88-142 (best-first indexes, -1 padded).  With a GPU the queries run on a backend.Serve
+handle that keeps the item factors resident (DESIGN.md 4.9); without one, or above its limits, the NumPy
+implementation below runs."""
 import numpy as np
+
+from buffalo_b200 import backend
 
 
 def quickselect(scores, result, sorted=True, num_threads=4):
@@ -34,7 +37,48 @@ class Parallel(object):
         self.algo = algo
         self.num_workers = int(kwargs.get("num_workers", algo.opt.num_workers))
 
+    @staticmethod
+    def _fingerprint(*arrays):
+        """Checksum of the arrays' bits, one pass over the data: the xor of all 32-bit words and the sum of the row
+        sums weighted by odd row numbers (so a changed value, and rows that changed places, both show)."""
+        out = []
+        for x in arrays:
+            if x is None:
+                out.append(None)
+                continue
+            w = x.view(np.uint32).reshape(x.shape[0], -1)
+            rows = w.sum(axis=1, dtype=np.uint64)
+            out.append((x.shape, int(np.bitwise_xor.reduce(w, axis=None)),
+                        int((rows * (np.arange(len(rows), dtype=np.uint64) * np.uint64(2) + np.uint64(1))).sum(dtype=np.uint64))))
+        return tuple(out)
+
+    def _serve_handle(self, B, Bb):
+        """The handle holding items B (and bias Bb) on the device.  The factor arrays are the model's live arrays and
+        training, normalize() or the user may rewrite them, in place or not, between two calls; so every call
+        checksums them and uploads again when they differ from what is resident."""
+        key = self._fingerprint(B, Bb)
+        if getattr(self, "_serve_key", None) != key:
+            if getattr(self, "_serve", None) is None:
+                self._serve = backend.Serve()
+            self._serve_key = None
+            self._serve.set_items(B, Bb)
+            self._serve_key = key
+        return self._serve
+
     def _run(self, indexes, A, B, Bb, topk, pool):
+        if Bb is not None and not Bb.size:
+            Bb = None
+        # On the device when one is present and the call is within the kernels' limits.  The items must fit in device
+        # memory next to the gathered query rows: an allocation failure is an error, not a silent switch to NumPy.
+        on_device = (backend.device_available() and len(indexes) and 0 < topk <= backend.SERVE_KMAX
+                     and B.shape[0] < 2 ** 31
+                     and all(x.dtype == np.float32 and x.flags["C_CONTIGUOUS"] for x in (A, B)))
+        if on_device:
+            h = self._serve_handle(B, None if Bb is None else np.ascontiguousarray(Bb, dtype=np.float32))
+            # only the rows asked for go to the device, read from the live array at every call
+            h.set_queries(np.ascontiguousarray(A[indexes]))
+            h.set_pool(None if pool is None or len(pool) == 0 else pool)
+            return h.topk(np.arange(len(indexes), dtype=np.int32), topk)
         keys = np.zeros((len(indexes), topk), dtype=np.int32)
         scores = np.zeros((len(indexes), topk), dtype=np.float32)
         dot_topn(indexes, A, B, Bb, keys, scores, pool, topk, self.num_workers)

@@ -309,6 +309,43 @@ int bfl_topk_host(const float* queries, int64_t nq, int ldq, const float* items,
                   const float* item_bias /* nullable */, int d, int k, int32_t* out_idx, float* out_val);
 
 /* =====================================================================================
+ * Batch serving top-k (DESIGN.md 4.9); the device path of buffalo.parallel's ParALS / ParBPRMF
+ * (dot_topn, buffalo/parallel/_core.hpp:88-142).  A handle keeps the item factors (and bias) and the query factors
+ * resident on the device and answers "the k best items for these n query rows" for any n:
+ *  - score = query . item (+ item_bias), best first, ties to the smaller item id, -1 / 0.0f where fewer than k
+ *    candidates exist; k <= 4096, row counts < 2^31.  Keys and scores are bitwise those of bfl_topk_device on the same
+ *    rows (same row pitches).
+ *  - set_items / set_queries upload HOST arrays once; bind_*_device borrow caller-owned DEVICE memory that must stay
+ *    valid while the handle uses it.  Items first: setting or binding the items clears the pool AND the queries (topk
+ *    is BFL_ERR_STATE until the queries are set again); the queries must have at least the items' width.  Device item
+ *    rows of a multiple of 4 floats (ld and d) must be 16-byte aligned.  set_queries with the very array given to
+ *    set_items (same rows, same ld) shares the resident copy (most_similar).
+ *  - set_pool restricts the candidates to HOST indices into the item matrix (any order, duplicates allowed: candidates
+ *    rank as the rows of items[pool] would, ties to the smaller pool position); results carry item ids.  NULL removes
+ *    the pool; an empty pool or an index outside the items is BFL_ERR_ARG.
+ *  - topk: HOST query_idx[n] (rows of the query matrix), HOST out_idx [n x k] and out_val [n x k] (nullable).  The call
+ *    is cut into batches; a batch's result is copied out through two pinned buffers while the next batch runs.
+ *  - topk_device: DEVICE arrays, stream-ordered on `stream`; indices outside the query matrix read as zero rows.
+ *  A handle serves one call at a time: topk and topk_device use scratch buffers the handle owns and grows on demand, so
+ *  calls on one handle must not overlap, on any stream or thread (use one handle per concurrent caller).
+ *  The handle owns two streams and its pinned buffers and starts no thread; destroy releases all of it.
+ * ===================================================================================== */
+typedef struct bfl_serve bfl_serve_t;
+bfl_serve_t* bfl_serve_create(void);
+void bfl_serve_destroy(bfl_serve_t* h);
+int bfl_serve_set_items(bfl_serve_t* h, const float* items, int64_t n_items, int ld, int d,
+                        const float* item_bias /* nullable */);
+int bfl_serve_bind_items_device(bfl_serve_t* h, const float* d_items, int64_t n_items, int ld, int d,
+                                const float* d_item_bias /* nullable */);
+int bfl_serve_set_queries(bfl_serve_t* h, const float* queries, int64_t n_q, int ld);
+int bfl_serve_bind_queries_device(bfl_serve_t* h, const float* d_queries, int64_t n_q, int ld);
+int bfl_serve_set_pool(bfl_serve_t* h, const int32_t* pool_idx /* nullable */, int64_t n_pool);
+int bfl_serve_topk(bfl_serve_t* h, const int32_t* query_idx, int64_t n, int k, int32_t* out_idx,
+                   float* out_val /* nullable */);
+int bfl_serve_topk_device(bfl_serve_t* h, const int32_t* d_query_idx, int64_t n, int k, int32_t* d_out_idx,
+                          float* d_out_val, void* stream);
+
+/* =====================================================================================
  * Validation metrics on the device (DESIGN.md 4.8): the device path of Evaluable.get_validation_results
  * (buffalo/evaluate/base.py:44-148).  Device pointers, stream-ordered.  A "seen" CSR (END offsets, int32 keys, every
  * row non-decreasing) holds training rows; seen_row[q] names the row of query q.  The held-out CSR is indexed by user.
