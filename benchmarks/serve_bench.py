@@ -14,6 +14,7 @@ limit are read in the same process.
 
     python benchmarks/serve_bench.py --queries 1000000
     python benchmarks/serve_bench.py --small 1,4,16,32,64      # calls of a handful of queries, both kernels
+    python benchmarks/serve_bench.py --exclude-seen             # the same calls with each user's seen items left out
 """
 import argparse
 import json
@@ -93,6 +94,87 @@ def small_calls(a, name, limit):
             h.close()
 
 
+def seen_histories(U, I, seed):
+    """Sorted, duplicate-free rows of U users: Pareto (Zipf-like) lengths, alpha 1.5 and scale 17 (mean about 51),
+    capped at 5000; items uniform over [0, I).  Returns (END offsets int64, keys int32)."""
+    rng = np.random.default_rng(seed)
+    lens = np.minimum((rng.pareto(1.5, U) + 1) * 17, 5000).astype(np.int64)
+    rows = np.repeat(np.arange(U, dtype=np.int64), lens)
+    keys = rng.integers(0, I, size=len(rows)).astype(np.int64)
+    order = np.lexsort((keys, rows))
+    rows, keys = rows[order], keys[order]
+    keep = np.ones(len(keys), bool)
+    keep[1:] = (rows[1:] != rows[:-1]) | (keys[1:] != keys[:-1])
+    rows, keys = rows[keep], keys[keep]
+    ptr = np.cumsum(np.bincount(rows, minlength=U)).astype(np.int64)
+    return ptr, keys.astype(np.int32)
+
+
+def exclude_seen_calls(a, name, limit):
+    """The filtered call (Serve.topk_seen / topk_seen_device) alternated with the unfiltered one on the same handle,
+    `--queries` users x {100k, 1M} items, d = 128, k = 10, every user with a history from seen_histories."""
+    import torch
+    from buffalo_b200 import _cabi, backend
+    d, k = 128, 10
+    for I in (100_000, 1_000_000):
+        U = a.queries
+        g = torch.Generator(device="cuda").manual_seed(a.seed)
+        P = torch.randn((U, d), generator=g, device="cuda") * 0.1
+        Q = torch.randn((I, d), generator=g, device="cuda") * 0.1
+        ptr, keys = seen_histories(U, I, a.seed)
+        qidx = np.arange(U, dtype=np.int32)
+        qdev, dptr, dkeys = (torch.from_numpy(x).cuda() for x in (qidx, ptr, keys))
+        h = backend.Serve()
+        h.bind_items(Q)
+        h.bind_queries(P)
+        plain_dev = lambda: h.topk_device(qdev, k)
+        # the C entry point itself: Serve.topk_seen_device adds argument checks and a sortedness check that synchronise
+        rows = torch.arange(U, dtype=torch.int32, device="cuda")
+        s_idx = torch.empty((U, k), dtype=torch.int32, device="cuda")
+        s_val = torch.empty((U, k), dtype=torch.float32, device="cuda")
+        seen_dev = lambda: (_cabi.check(_cabi.lib().bfl_seen_topk_device(
+            h._h, qdev.data_ptr(), U, k, dptr.data_ptr(), dkeys.data_ptr(), rows.data_ptr(), s_idx.data_ptr(),
+            s_val.data_ptr(), backend._stream_ptr(None)), "bfl_seen_topk_device"), (s_idx, s_val))[1]
+        for fn in (plain_dev, seen_dev):     # warm-up
+            fn()
+        h.topk(qidx, k)
+        h.topk_seen(qidx, k, ptr, keys)
+        torch.cuda.synchronize()
+        dev = {"plain": [], "seen": []}
+        e2e = {"plain": [], "seen": []}
+        for _ in range(a.repeats):
+            for arm, fn in (("plain", plain_dev), ("seen", seen_dev)):
+                out, t = events(fn, 1)
+                dev[arm] += t
+            for arm in ("plain", "seen"):
+                t0 = time.perf_counter()
+                res = h.topk(qidx, k) if arm == "plain" else h.topk_seen(qidx, k, ptr, keys)
+                e2e[arm].append(time.perf_counter() - t0)
+                if arm == "seen":
+                    sk = res[0]
+        # no seen item comes back: (user, item) pairs as user * I + item, the seen ones sorted already
+        lens = np.diff(ptr, prepend=0)
+        seen_pairs = np.repeat(np.arange(U, dtype=np.int64), lens) * I + keys
+        got = (np.arange(U, dtype=np.int64)[:, None] * I + sk)[sk >= 0]
+        at = np.minimum(np.searchsorted(seen_pairs, got), len(seen_pairs) - 1)
+        seen_returned = bool((seen_pairs[at] == got).any())
+        di, _ = h.topk_seen_device(qdev, k, dptr, dkeys)
+        print(json.dumps(dict(
+            gpu=name, power_limit=limit, exclude_seen=True, users=U, items=I, d=d, k=k, seen_keys=int(len(keys)),
+            mean_history=round(float(lens.mean()), 1), max_history=int(lens.max()),
+            device_plain_s=round(min(dev["plain"]), 4), device_seen_s=round(min(dev["seen"]), 4),
+            device_ratio=round(min(dev["seen"]) / min(dev["plain"]), 3),
+            e2e_plain_s=round(min(e2e["plain"]), 4), e2e_seen_s=round(min(e2e["seen"]), 4),
+            e2e_ratio=round(min(e2e["seen"]) / min(e2e["plain"]), 3),
+            device_s_all={x: [round(v, 4) for v in dev[x]] for x in dev},
+            e2e_s_all={x: [round(v, 4) for v in e2e[x]] for x in e2e},
+            seen_item_returned=seen_returned,
+            host_and_device_paths_equal=bool(np.array_equal(sk, di.cpu().numpy())))), flush=True)
+        h.close()
+        del P, Q, qdev, dptr, dkeys, rows, s_idx, s_val
+        torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--shapes", default="1000000x100000,10000000x1000000", help="users x items, comma separated")
@@ -103,6 +185,8 @@ def main():
     ap.add_argument("--numpy-sample", type=int, default=64)
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--small", default="", help="e.g. 1,4,16,32,64: time calls of that many queries instead (see small_calls)")
+    ap.add_argument("--exclude-seen", action="store_true",
+                    help="time the calls that leave each user's seen items out instead (see exclude_seen_calls)")
     ap.add_argument("--seed", type=int, default=0)
     a = ap.parse_args()
     import torch
@@ -113,6 +197,9 @@ def main():
     name = name or torch.cuda.get_device_properties(0).name
     if a.small:
         small_calls(a, name, limit)
+        return
+    if a.exclude_seen:
+        exclude_seen_calls(a, name, limit)
         return
     for shape in a.shapes.split(","):
         U, I = [int(x) for x in shape.split("x")]

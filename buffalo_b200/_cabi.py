@@ -114,6 +114,8 @@ PROTOTYPES = {
     "bfl_serve_set_pool": (C.c_int, [_vp, _vp, _i64]),
     "bfl_serve_topk": (C.c_int, [_vp, _vp, _i64, C.c_int, _vp, _vp]),
     "bfl_serve_topk_device": (C.c_int, [_vp, _vp, _i64, C.c_int, _vp, _vp, _vp]),
+    "bfl_seen_topk": (C.c_int, [_vp, _vp, _i64, C.c_int, _vp, _vp, _vp, _vp]),
+    "bfl_seen_topk_device": (C.c_int, [_vp, _vp, _i64, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp]),
     # validation metrics
     "bfl_eval_unsorted_rows_device": (C.c_int, [_vp, _vp, _i64, _vp, _vp]),
     "bfl_eval_topk_masked_device": (C.c_int, [_vp, _i64, C.c_int, _vp, _i64, C.c_int, _vp, C.c_int, C.c_int, _vp, _vp,

@@ -570,6 +570,76 @@ class Serve(_Holder):
                                                 val.data_ptr(), _stream_ptr(stream)), "bfl_serve_topk_device")
         return idx, val
 
+    def _check_seen(self, n, seen_indptr, seen_keys, host):
+        """Argument checks of the seen rows: END offsets int64 [n], non-decreasing from 0, keys int32 in the items."""
+        check = _host if host else (lambda a, dt, nd, name: _dev(a, np.dtype(dt).name, name))
+        check(seen_indptr, np.int64, 1, "seen_indptr")
+        check(seen_keys, np.int32, 1, "seen_keys")
+        if seen_indptr.shape[0] != n:
+            raise ValueError("seen_indptr must hold one END offset per query (%d), got %d" % (n, seen_indptr.shape[0]))
+        ptr = seen_indptr if host else seen_indptr.cpu().numpy()
+        nnz = int(ptr[-1]) if n else 0
+        if n and (ptr[0] < 0 or (np.diff(ptr) < 0).any()):
+            raise ValueError("seen_indptr must be non-decreasing END offsets from 0")
+        if nnz > seen_keys.shape[0]:
+            raise ValueError("seen_indptr ends past the %d seen keys" % seen_keys.shape[0])
+        if nnz:
+            keys = seen_keys[:nnz]
+            lo, hi = (int(keys.min()), int(keys.max())) if host else (int(keys.min().item()), int(keys.max().item()))
+            if lo < 0 or hi >= self.num_items:
+                raise ValueError("seen key out of range [0, %d)" % self.num_items)
+        return nnz
+
+    def topk_seen(self, query_idx, k, seen_indptr, seen_keys, want_scores=True):
+        """topk with query i's seen items left out: row i of the host CSR (seen_indptr int64 END offsets [n], seen_keys
+        int32 item ids in any order, duplicates allowed).  The survivors keep their order and score bits; -1 / 0.0 pad
+        when fewer than k candidates remain."""
+        k = self._check_k(k)
+        q = np.ascontiguousarray(query_idx, dtype=np.int32).reshape(-1)
+        if q.size and (q.min() < 0 or q.max() >= self.num_queries):
+            raise ValueError("query index out of range")
+        nnz = self._check_seen(q.size, seen_indptr, seen_keys, host=True)
+        keys = seen_keys if nnz else np.zeros(1, np.int32)
+        idx = np.empty((q.size, k), dtype=np.int32)
+        val = np.empty((q.size, k), dtype=np.float32) if want_scores else None
+        if q.size:
+            _cabi.check(self._lib.bfl_seen_topk(self._h, q.ctypes.data, q.size, k, seen_indptr.ctypes.data,
+                                                keys.ctypes.data, idx.ctypes.data,
+                                                None if val is None else val.ctypes.data), "bfl_seen_topk")
+        return idx, val
+
+    def topk_seen_device(self, query_idx, k, seen_indptr, seen_keys, seen_row=None, stream=None):
+        """topk_device with query q's seen items left out: row seen_row[q] (default q) of a CSR of torch CUDA tensors
+        (int64 END offsets, int32 keys).  Rows not in ascending order are sorted first with the device radix sort
+        (eval_unsorted_rows, csr_from_triples_device); that check synchronises."""
+        import torch
+        k = self._check_k(k)
+        n = query_idx.shape[0]
+        dev = query_idx.device
+        nnz = self._check_seen(seen_indptr.shape[0], seen_indptr, seen_keys, host=False)
+        keys = seen_keys[:nnz] if nnz else torch.zeros(1, dtype=torch.int32, device=dev)
+        if nnz and eval_unsorted_rows(seen_indptr, keys, stream):
+            lens = torch.diff(seen_indptr, prepend=seen_indptr.new_zeros(1))
+            major = torch.repeat_interleave(torch.arange(seen_indptr.shape[0], dtype=torch.int32, device=dev), lens)
+            seen_indptr, keys, _ = csr_from_triples_device(major, keys, torch.ones(nnz, dtype=torch.float32, device=dev),
+                                                           seen_indptr.shape[0], self.num_items, stream=stream)
+        if seen_row is None:
+            if seen_indptr.shape[0] != n:
+                raise ValueError("without seen_row the CSR needs one row per query")
+            seen_row = torch.arange(n, dtype=torch.int32, device=dev)
+        elif seen_row.shape[0] != n:
+            raise ValueError("seen_row must name one row per query")
+        elif n and (int(seen_row.min().item()) < 0 or int(seen_row.max().item()) >= seen_indptr.shape[0]):
+            raise ValueError("seen_row names a row outside the seen CSR")
+        idx = torch.empty((n, k), dtype=torch.int32, device=dev)
+        val = torch.empty((n, k), dtype=torch.float32, device=dev)
+        if n:
+            _cabi.check(self._lib.bfl_seen_topk_device(
+                self._h, _dev(query_idx, "int32", "query_idx"), n, k, seen_indptr.data_ptr(), keys.data_ptr(),
+                _dev(seen_row, "int32", "seen_row"), idx.data_ptr(), val.data_ptr(), _stream_ptr(stream)),
+                "bfl_seen_topk_device")
+        return idx, val
+
 
 def csr_from_triples_device(major, minor, vals, num_major, num_minor, sort_minor=True, stream=None):
     """(indptr_end int64, key int32, val float32) torch CUDA tensors of one orientation from int32 major / minor and

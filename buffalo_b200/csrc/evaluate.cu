@@ -7,17 +7,16 @@
 //   eval_rank_terms_kernel : per user, hits against the held-out row, DCG, AP, accuracy and AUC in fp64;
 //   eval_score_terms_kernel: per held-out triple, the model's score with NumPy's float32 arithmetic and its error;
 //   eval_sum_*_kernel      : column sums of per-row terms in a fixed order (bitwise repeatable).
-// Ranking is on one 64-bit key per item: (~ord(score)) << 32 | item.  Smaller key = better item, so the order is score
-// descending, then item ascending, and the keys of distinct items are distinct: selection needs no tie rule and no
-// score is ever used as a marker.
-#include "topk_common.cuh"
+// Ranking is on the 64-bit rank keys of seen_common.cuh, so selection needs no tie rule and no score is ever used as a
+// marker.  masked_topk (a pool, scores out) and seen_merge also serve the seen-aware calls of serve.cu.
+#include "seen_common.cuh"
 
 using namespace bfl;
 
 namespace {
 
 constexpr int EV_QB = 4;
-constexpr unsigned long long EV_EMPTY = ~0ull;   // never a rank key: the item half of a key is below 2^31
+constexpr unsigned long long EV_EMPTY = SEEN_EMPTY;
 constexpr int EV_SUM_BLOCKS = 128;
 constexpr int EV_SUM_WIDTH = 8;
 
@@ -27,23 +26,6 @@ struct KeySel {
     unsigned int kk, cnt;
     int stop;
 };
-
-__device__ __forceinline__ unsigned long long rank_key(float s, int64_t item) {
-    return ((unsigned long long)(~ord_of(s)) << 32) | (unsigned long long)(uint32_t)item;
-}
-
-// First position in [lo, hi) of the non-decreasing a[] holding a value >= x.  All 32 lanes of a warp call it.
-__device__ int64_t warp_lower_bound(const int32_t* __restrict__ a, int64_t lo, int64_t hi, int32_t x, int lane) {
-    while (hi - lo > 32) {
-        const int64_t step = (hi - lo + 31) / 32;
-        const int64_t p = lo + lane * step;
-        const int c = __popc(__ballot_sync(FULL, p < hi && a[p] < x));   // probes 0..c-1 are below x
-        const int64_t nlo = c == 0 ? lo : lo + (int64_t)(c - 1) * step + 1;
-        hi = min(hi, lo + (int64_t)c * step);
-        lo = nlo;
-    }
-    return lo + __popc(__ballot_sync(FULL, lo + lane < hi && a[lo + lane] < x));
-}
 
 // The k smallest of the keys get(0..n) that are not EV_EMPTY (n_valid of them, all distinct) -> out[0..min(k, n_valid))
 // in no particular order; returns that count.  MSB-first radix select over 8-bit digits, stopping as soon as the
@@ -100,8 +82,8 @@ __device__ int select_smallest(Get get, int64_t n, int64_t n_valid, int k, unsig
 __global__ void __launch_bounds__(TK_THREADS) eval_slice_kernel(
     const float* __restrict__ Qr, int64_t nq, int ldq, const float* __restrict__ It, int64_t n_items, int ldi,
     const float* __restrict__ bias, int d, int k, int nslices, const int64_t* __restrict__ seen_indptr,
-    const int32_t* __restrict__ seen_keys, const int32_t* __restrict__ seen_row, unsigned long long* __restrict__ cand,
-    int32_t* __restrict__ cand_cnt) {
+    const int32_t* __restrict__ seen_keys, const int32_t* __restrict__ seen_row, const int32_t* __restrict__ pool,
+    unsigned long long* __restrict__ cand, int32_t* __restrict__ cand_cnt) {
     extern __shared__ __align__(16) unsigned char ev_smem[];
     unsigned long long* keys = reinterpret_cast<unsigned long long*>(ev_smem);   // [TK_SLICE]
     float* scores = reinterpret_cast<float*>(keys + TK_SLICE);                    // [EV_QB][TK_SLICE]
@@ -115,11 +97,11 @@ __global__ void __launch_bounds__(TK_THREADS) eval_slice_kernel(
     const int slice = blockIdx.y;
     const int64_t i0 = (int64_t)slice * TK_SLICE;
     const int ni = (int)min((long long)TK_SLICE, (long long)(n_items - i0));
-    if (w < nqb) {   // the user's training items inside [i0, i0 + ni)
-        const int64_t r = seen_row[q0 + w];
-        const int64_t b = r > 0 ? seen_indptr[r - 1] : 0, e = seen_indptr[r];
-        const int64_t lo = warp_lower_bound(seen_keys, b, e, (int32_t)i0, lane);
-        const int64_t hi = warp_lower_bound(seen_keys, lo, e, (int32_t)(i0 + ni), lane);
+    if (w < nqb) {   // the user's seen items inside [i0, i0 + ni); with a pool, the whole row
+        const int64_t r = seen_row ? seen_row[q0 + w] : q0 + w;
+        const int64_t b = seen_row_begin(seen_indptr, r), e = seen_indptr[r];
+        const int64_t lo = pool ? b : warp_lower_bound(seen_keys, b, e, (int32_t)i0, lane);
+        const int64_t hi = pool ? e : warp_lower_bound(seen_keys, lo, e, (int32_t)(i0 + ni), lane);
         if (lane == 0) {
             seen_lo[w] = lo;
             seen_hi[w] = hi;
@@ -130,9 +112,12 @@ __global__ void __launch_bounds__(TK_THREADS) eval_slice_kernel(
         for (int j = tid; j < TK_SLICE / 32; j += TK_THREADS) seen_bits[j] = 0;
         if (tid == 0) sc.cnt = 0;
         __syncthreads();
-        for (int64_t e = seen_lo[qi] + tid; e < seen_hi[qi]; e += TK_THREADS) {
-            const int p = seen_keys[e] - (int)i0;
-            atomicOr(&seen_bits[p >> 5], 1u << (p & 31));
+        if (!pool) {
+            mark_seen_range(seen_keys, seen_lo[qi], seen_hi[qi], i0, seen_bits, tid, TK_THREADS);
+        } else if (seen_hi[qi] > seen_lo[qi]) {   // candidate it is item pool[i0 + it], pool order is arbitrary
+            for (int it = tid; it < ni; it += TK_THREADS)
+                if (row_contains(seen_keys, seen_lo[qi], seen_hi[qi], pool[i0 + it]))
+                    atomicOr(&seen_bits[it >> 5], 1u << (it & 31));
         }
         __syncthreads();
         for (int it0 = 0; it0 < ni; it0 += TK_THREADS) {
@@ -155,7 +140,8 @@ __global__ void __launch_bounds__(TK_THREADS) eval_slice_kernel(
 
 __global__ void __launch_bounds__(TK_THREADS) eval_merge_kernel(const unsigned long long* __restrict__ cand,
                                                                 const int32_t* __restrict__ cand_cnt, int nslices,
-                                                                int k, int kpad, int32_t* __restrict__ out_idx) {
+                                                                int k, int kpad, int32_t* __restrict__ out_idx,
+                                                                float* __restrict__ out_val) {
     extern __shared__ __align__(16) unsigned long long ev_sorted[];   // [kpad]
     __shared__ KeySel sc;
     __shared__ long long part[TK_THREADS / 32];
@@ -194,8 +180,10 @@ __global__ void __launch_bounds__(TK_THREADS) eval_merge_kernel(const unsigned l
             __syncthreads();
         }
     }
-    for (int i = tid; i < k; i += TK_THREADS)
+    for (int i = tid; i < k; i += TK_THREADS) {
         out_idx[q * k + i] = i < got ? (int32_t)(uint32_t)(ev_sorted[i] & 0xffffffffull) : -1;
+        if (out_val) out_val[q * k + i] = i < got ? rank_key_score(ev_sorted[i]) : 0.f;
+    }
 }
 
 __global__ void eval_unsorted_rows_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ keys,
@@ -362,6 +350,39 @@ __global__ void __launch_bounds__(EV_SUM_BLOCKS) eval_sum_final_kernel(const dou
 
 }  // namespace
 
+int bfl::masked_topk(const float* queries, int64_t nq, int ldq, const float* items, int64_t n_items, int ldi,
+                     const float* item_bias, int d, int k, const int64_t* seen_indptr, const int32_t* seen_keys,
+                     const int32_t* seen_row, const int32_t* pool, int32_t* out_idx, float* out_val, cudaStream_t st) {
+    const int64_t nslices = (n_items + TK_SLICE - 1) / TK_SLICE;
+    if (n_items > INT32_MAX || nslices > 65535) BFL_FAIL(BFL_ERR_ARG, "masked top-k: too many items");
+    unsigned long long* cand = nullptr;
+    int32_t* cand_cnt = nullptr;
+    BFL_CUDA(cudaMallocAsync(&cand, sizeof(unsigned long long) * (size_t)nq * nslices * k, st));
+    BFL_CUDA(cudaMallocAsync(&cand_cnt, sizeof(int32_t) * (size_t)nq * nslices, st));
+    const int dpad = (d + 3) & ~3;
+    const size_t smem1 = sizeof(unsigned long long) * TK_SLICE + sizeof(float) * ((size_t)EV_QB * TK_SLICE + (size_t)EV_QB * dpad);
+    BFL_CUDA(cudaFuncSetAttribute(eval_slice_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
+    dim3 grid((unsigned)((nq + EV_QB - 1) / EV_QB), (unsigned)nslices);
+    eval_slice_kernel<<<grid, TK_THREADS, smem1, st>>>(queries, nq, ldq, items, n_items, ldi, item_bias, d, k,
+                                                       (int)nslices, seen_indptr, seen_keys, seen_row, pool, cand,
+                                                       cand_cnt);
+    BFL_LAUNCHED();
+    const int rc = seen_merge(cand, cand_cnt, nq, (int)nslices, k, out_idx, out_val, st);
+    BFL_CUDA(cudaFreeAsync(cand, st));
+    BFL_CUDA(cudaFreeAsync(cand_cnt, st));
+    return rc;
+}
+
+int bfl::seen_merge(const unsigned long long* cand, const int32_t* cand_cnt, int64_t nq, int nslices, int k,
+                    int32_t* out_idx, float* out_val, cudaStream_t st) {
+    int kpad = 2;
+    while (kpad < k) kpad <<= 1;
+    eval_merge_kernel<<<(unsigned)nq, TK_THREADS, kpad * sizeof(unsigned long long), st>>>(cand, cand_cnt, nslices, k,
+                                                                                          kpad, out_idx, out_val);
+    BFL_LAUNCHED();
+    return BFL_OK;
+}
+
 extern "C" {
 
 int bfl_eval_unsorted_rows_device(const int64_t* d_indptr, const int32_t* d_keys, int64_t rows,
@@ -386,29 +407,8 @@ int bfl_eval_topk_masked_device(const float* d_queries, int64_t nq, int ldq, con
         n_items <= 0 || d <= 0 || ldq < d || ldi < d)
         BFL_FAIL(BFL_ERR_ARG, "bad masked top-k arguments");
     if (k <= 0 || k > TK_KMAX) BFL_FAIL(BFL_ERR_ARG, "masked top-k: k must be in [1, 4096]");
-    const int64_t nslices = (n_items + TK_SLICE - 1) / TK_SLICE;
-    if (n_items > INT32_MAX || nslices > 65535) BFL_FAIL(BFL_ERR_ARG, "masked top-k: too many items");
-    cudaStream_t st = (cudaStream_t)stream;
-    unsigned long long* cand = nullptr;
-    int32_t* cand_cnt = nullptr;
-    BFL_CUDA(cudaMallocAsync(&cand, sizeof(unsigned long long) * (size_t)nq * nslices * k, st));
-    BFL_CUDA(cudaMallocAsync(&cand_cnt, sizeof(int32_t) * (size_t)nq * nslices, st));
-    const int dpad = (d + 3) & ~3;
-    const size_t smem1 = sizeof(unsigned long long) * TK_SLICE + sizeof(float) * ((size_t)EV_QB * TK_SLICE + (size_t)EV_QB * dpad);
-    BFL_CUDA(cudaFuncSetAttribute(eval_slice_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
-    dim3 grid((unsigned)((nq + EV_QB - 1) / EV_QB), (unsigned)nslices);
-    eval_slice_kernel<<<grid, TK_THREADS, smem1, st>>>(d_queries, nq, ldq, d_items, n_items, ldi, d_item_bias, d, k,
-                                                       (int)nslices, d_seen_indptr, d_seen_keys, d_seen_row, cand,
-                                                       cand_cnt);
-    BFL_LAUNCHED();
-    int kpad = 2;
-    while (kpad < k) kpad <<= 1;
-    eval_merge_kernel<<<(unsigned)nq, TK_THREADS, kpad * sizeof(unsigned long long), st>>>(cand, cand_cnt, (int)nslices,
-                                                                                          k, kpad, d_out_idx);
-    BFL_LAUNCHED();
-    BFL_CUDA(cudaFreeAsync(cand, st));
-    BFL_CUDA(cudaFreeAsync(cand_cnt, st));
-    return BFL_OK;
+    return masked_topk(d_queries, nq, ldq, d_items, n_items, ldi, d_item_bias, d, k, d_seen_indptr, d_seen_keys,
+                       d_seen_row, nullptr, d_out_idx, nullptr, (cudaStream_t)stream);
 }
 
 int bfl_eval_ranking_terms_device(const int32_t* d_ranked, int64_t nq, int k, const int32_t* d_users,

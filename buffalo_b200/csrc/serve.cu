@@ -8,11 +8,16 @@
 //                        slice's k best for its own 4 queries without block barriers.
 //   topk_merge         : the merge of topk.cu, unchanged.
 //   serve_finish_kernel: candidate positions -> item ids through the pool, 0.0f scores on the -1 padding.
+// The seen-aware calls (bfl_seen_topk*) leave each query's seen items out: serve_slice_seen_kernel marks them in a
+// per-warp bitmask before its warp_select, which then never counts them and hands the merge rank keys and a count per
+// slice (seen_merge); calls that go to the 4-query kernels run masked_topk on the gathered rows.  Both in
+// seen_common.cuh / evaluate.cu.
+#include <algorithm>
 #include <climits>
 #include <new>
 
 #include "sm90_ptx.cuh"
-#include "topk_common.cuh"
+#include "seen_common.cuh"
 
 using namespace bfl;
 
@@ -25,10 +30,22 @@ constexpr int SV_SLICE = 1024;                      // candidates per CTA
 constexpr int SV_DMAX = 256;                        // widest d of the batch kernel (shared memory)
 constexpr int SV_BATCH_MAX = 16384;                 // queries per internal batch
 constexpr size_t SV_CAND_BYTES = (size_t)1 << 30;   // candidate scratch aimed at per batch
+constexpr int64_t SV_SEEN_KEYS = (int64_t)1 << 24;  // seen keys per internal batch aimed at (a longer row is a batch)
 
 // row pitch of a staged tile in floats: pitch / 4 is odd, so the float4 reads of 8 consecutive lanes (one row each) fall
 // into 8 different bank groups
 __host__ __device__ inline int tile_pitch(int dpad) { return ((dpad >> 2) & 1) ? dpad : dpad + 4; }
+
+// words of a warp's selection scratch in the tile buffers once scoring is done: 256 histogram counters, then with
+// seen items 32 words of seen bitmask (one bit per candidate of the slice)
+__host__ __device__ constexpr int sel_words(bool seen) { return seen ? 256 + SV_SLICE / 32 : 256; }
+
+// A seen CSR on the device (END offsets, every row non-decreasing); query q of a batch reads row row[q], or row q.
+struct SeenRows {
+    const int64_t* indptr;
+    const int32_t* keys;
+    const int32_t* row;
+};
 
 struct ScoreCtx {
     const float* q;      // the warp's SV_QR query rows in shared memory, pitch dpad
@@ -93,9 +110,29 @@ __device__ __forceinline__ void tree(const ScoreCtx& s, float (&out)[SV_QR][IR])
 // One warp: the k largest of vals[0..n) -> (out_v, out_i)[0..k) unordered, index = idx0 + position, ties at the k-th
 // value to the smaller position.  The selection of block_select (topk.cu) at warp scope, so that the 8 warps of a CTA
 // select for 8 queries at once with no block barrier.  hist: 256 counters of the warp.
-__device__ void warp_select(const float* vals, int idx0, int n, int k, float* out_v, int32_t* out_i, unsigned* hist) {
+// SEEN: position i does not exist for the selection when bit i of seen[0..32) is set (n <= 1024, no bit at or past n);
+// the min(k, unseen) selected go to out_key as rank keys, unordered, and their number to *out_cnt.
+template <bool SEEN>
+__device__ void warp_select(const float* vals, int idx0, int n, int k, float* out_v, int32_t* out_i, unsigned* hist,
+                            const uint32_t* seen = nullptr, unsigned long long* out_key = nullptr,
+                            int32_t* out_cnt = nullptr) {
     const int lane = threadIdx.x & 31;
-    if (n <= k) {
+    auto live = [&](int i) { return !SEEN || !((seen[i >> 5] >> (i & 31)) & 1u); };
+    if constexpr (SEEN) {
+        const int nv = n - (int)__reduce_add_sync(FULL, (unsigned)__popc(seen[lane]));
+        if (lane == 0) *out_cnt = nv < k ? nv : k;
+        if (nv <= k) {
+            unsigned base = 0;
+            for (int i0 = 0; i0 < n; i0 += 32) {
+                const int i = i0 + lane;
+                const bool keep = i < n && live(i);
+                const unsigned bal = __ballot_sync(FULL, keep);
+                if (keep) out_key[base + __popc(bal & ((1u << lane) - 1u))] = rank_key(vals[i], idx0 + i);
+                base += __popc(bal);
+            }
+            return;
+        }
+    } else if (n <= k) {
         for (int i = lane; i < k; i += 32) {
             out_v[i] = i < n ? vals[i] : -INFINITY;
             out_i[i] = i < n ? idx0 + i : -1;
@@ -110,7 +147,7 @@ __device__ void warp_select(const float* vals, int idx0, int n, int k, float* ou
         __syncwarp();
         for (int i = lane; i < n; i += 32) {
             const uint32_t u = ord_of(vals[i]);
-            if ((u & mask) == prefix) atomicAdd(&hist[(u >> shift) & 255u], 1u);
+            if ((u & mask) == prefix && live(i)) atomicAdd(&hist[(u >> shift) & 255u], 1u);
         }
         __syncwarp();
         // lane owns bins 8 lane .. 8 lane + 7; suf = matches in its bins and all higher ones
@@ -153,17 +190,26 @@ __device__ void warp_select(const float* vals, int idx0, int n, int k, float* ou
         const int i = i0 + lane;
         const float v = i < n ? vals[i] : 0.f;
         const uint32_t u = ord_of(v);
-        const bool gt = i < n && u > T, tie = i < n && u == T;
+        const bool ok = i < n && live(i);
+        const bool gt = ok && u > T, tie = ok && u == T;
         const unsigned bg = __ballot_sync(FULL, gt), bt = __ballot_sync(FULL, tie);
         if (gt) {
             const unsigned pos = n_gt + __popc(bg & below);
-            out_v[pos] = v;
-            out_i[pos] = idx0 + i;
+            if constexpr (SEEN) {
+                out_key[pos] = rank_key(v, idx0 + i);
+            } else {
+                out_v[pos] = v;
+                out_i[pos] = idx0 + i;
+            }
         }
         const unsigned r = n_tie + __popc(bt & below);
         if (tie && r < kk) {
-            out_v[(k - kk) + r] = v;
-            out_i[(k - kk) + r] = idx0 + i;
+            if constexpr (SEEN) {
+                out_key[(k - kk) + r] = rank_key(v, idx0 + i);
+            } else {
+                out_v[(k - kk) + r] = v;
+                out_i[(k - kk) + r] = idx0 + i;
+            }
         }
         n_gt += __popc(bg);
         n_tie += __popc(bt);
@@ -172,12 +218,17 @@ __device__ void warp_select(const float* vals, int idx0, int n, int k, float* ou
 
 // Qm rows are gathered through qidx (an index outside [0, n_qrows) reads as a zero row); candidate c of the slice is
 // item row pool[c] (or c).  cand_i holds candidate POSITIONS (so ties resolve as on a gathered item matrix).
-template <int IR>
-__global__ void __launch_bounds__(SV_THREADS)
-    serve_slice_kernel(const float* __restrict__ Qm, int64_t n_qrows, int ldq, const int32_t* __restrict__ qidx, int nq,
-                       const float* __restrict__ It, int ldi, int64_t n_cand, const int32_t* __restrict__ pool,
-                       const float* __restrict__ bias, int d, int k, int nslices, int bulk, int tile_floats,
-                       float* __restrict__ cand_v, int32_t* __restrict__ cand_i) {
+// SEEN: query q leaves out the items of row seen.row[q] (or q) of the sorted seen CSR; the slice's candidates go to
+// cand_key / cand_cnt (rank keys and their number) instead of cand_v / cand_i.  The body of serve_slice_kernel and
+// serve_slice_seen_kernel.
+template <int IR, bool SEEN>
+__device__ __forceinline__ void serve_slice(const float* __restrict__ Qm, int64_t n_qrows, int ldq,
+                                            const int32_t* __restrict__ qidx, int nq, const float* __restrict__ It,
+                                            int ldi, int64_t n_cand, const int32_t* __restrict__ pool,
+                                            const float* __restrict__ bias, int d, int k, int nslices, int bulk,
+                                            int tile_floats, float* __restrict__ cand_v, int32_t* __restrict__ cand_i,
+                                            SeenRows seen, unsigned long long* __restrict__ cand_key,
+                                            int32_t* __restrict__ cand_cnt) {
     constexpr int IT = 32 * IR;
     extern __shared__ __align__(128) float sv_smem[];
     __shared__ __align__(8) uint64_t bar[2];
@@ -258,14 +309,58 @@ __global__ void __launch_bounds__(SV_THREADS)
         }
         __syncthreads();
     }
-    unsigned* hist = reinterpret_cast<unsigned*>(tiles) + w * 256;
+    unsigned* hist = reinterpret_cast<unsigned*>(tiles) + w * sel_words(SEEN);
     for (int a = 0; a < SV_QR; ++a) {
         const int q = q0 + w * SV_QR + a;
         if (q >= nq) break;
         const size_t o = ((size_t)q * nslices + slice) * k;
-        warp_select(scores + (w * SV_QR + a) * SV_SLICE, (int)i0, ni, k, cand_v + o, cand_i + o, hist);
+        if constexpr (SEEN) {
+            // bit c of `bits`: candidate i0 + c is one of the query's seen items
+            uint32_t* bits = hist + 256;
+            const int64_t r = seen.row ? seen.row[q] : q;
+            const int64_t b = seen_row_begin(seen.indptr, r), e = seen.indptr[r];
+            bits[lane] = 0;
+            __syncwarp();
+            if (e > b && pool) {   // pool order is arbitrary: each candidate is looked up in the row
+                for (int c0 = 0; c0 < ni; c0 += 32) {
+                    const int c = c0 + lane;
+                    const unsigned m = __ballot_sync(FULL, c < ni && row_contains(seen.keys, b, e, pool[i0 + c]));
+                    if (lane == 0) bits[c0 >> 5] = m;
+                }
+            } else if (e > b) {    // the slice's seen items are one run of the sorted row
+                const int64_t lo = warp_lower_bound(seen.keys, b, e, (int32_t)i0, lane);
+                const int64_t hi = warp_lower_bound(seen.keys, lo, e, (int32_t)(i0 + ni), lane);
+                mark_seen_range(seen.keys, lo, hi, i0, bits, lane, 32);
+            }
+            __syncwarp();
+            warp_select<true>(scores + (w * SV_QR + a) * SV_SLICE, (int)i0, ni, k, nullptr, nullptr, hist, bits,
+                              cand_key + o, cand_cnt + (size_t)q * nslices + slice);
+        } else {
+            warp_select<false>(scores + (w * SV_QR + a) * SV_SLICE, (int)i0, ni, k, cand_v + o, cand_i + o, hist);
+        }
         __syncwarp();
     }
+}
+
+template <int IR>
+__global__ void __launch_bounds__(SV_THREADS)
+    serve_slice_kernel(const float* __restrict__ Qm, int64_t n_qrows, int ldq, const int32_t* __restrict__ qidx, int nq,
+                       const float* __restrict__ It, int ldi, int64_t n_cand, const int32_t* __restrict__ pool,
+                       const float* __restrict__ bias, int d, int k, int nslices, int bulk, int tile_floats,
+                       float* __restrict__ cand_v, int32_t* __restrict__ cand_i) {
+    serve_slice<IR, false>(Qm, n_qrows, ldq, qidx, nq, It, ldi, n_cand, pool, bias, d, k, nslices, bulk, tile_floats,
+                           cand_v, cand_i, SeenRows{nullptr, nullptr, nullptr}, nullptr, nullptr);
+}
+
+template <int IR>
+__global__ void __launch_bounds__(SV_THREADS)
+    serve_slice_seen_kernel(const float* __restrict__ Qm, int64_t n_qrows, int ldq, const int32_t* __restrict__ qidx,
+                            int nq, const float* __restrict__ It, int ldi, int64_t n_cand,
+                            const int32_t* __restrict__ pool, const float* __restrict__ bias, int d, int k, int nslices,
+                            int bulk, int tile_floats, SeenRows seen, unsigned long long* __restrict__ cand_key,
+                            int32_t* __restrict__ cand_cnt) {
+    serve_slice<IR, true>(Qm, n_qrows, ldq, qidx, nq, It, ldi, n_cand, pool, bias, d, k, nslices, bulk, tile_floats,
+                          nullptr, nullptr, seen, cand_key, cand_cnt);
 }
 
 __global__ void serve_finish_kernel(int32_t* __restrict__ idx, float* __restrict__ val, size_t n,
@@ -291,10 +386,19 @@ __global__ void serve_gather_rows_kernel(const float* __restrict__ src, int64_t 
     dst[e] = (c < d && s >= 0 && s < n_src) ? src[s * ld + c] : 0.f;
 }
 
-size_t slice_smem_bytes(int d, int IR, int* tile_floats) {
+// writes r to major[indptr[r - 1] .. indptr[r]) for every row r: the row ids the device radix sort orders by
+__global__ void seen_row_ids_kernel(const int64_t* __restrict__ indptr, int64_t rows, int32_t* __restrict__ major) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+    for (int64_t r = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < rows; r += warps)
+        for (int64_t e = seen_row_begin(indptr, r) + lane; e < indptr[r]; e += 32) major[e] = (int32_t)r;
+}
+
+size_t slice_smem_bytes(int d, int IR, bool seen, int* tile_floats) {
     const int dpad = (d + 3) & ~3;
     int tf = 32 * IR * tile_pitch(dpad);
-    if (2 * tf < (SV_THREADS / 32) * 256) tf = (SV_THREADS / 32) * 128;   // room for the select histograms
+    const int sel = (SV_THREADS / 32) * sel_words(seen);
+    if (2 * tf < sel) tf = sel / 2;                 // room for the select histograms (and seen bitmasks)
     *tile_floats = tf;
     return sizeof(float) * ((size_t)SV_QT * SV_SLICE + (size_t)SV_QT * dpad + 2 * (size_t)tf);
 }
@@ -323,6 +427,17 @@ struct bfl_serve {
     int32_t* pin_i[2] = {nullptr, nullptr};
     float* pin_v[2] = {nullptr, nullptr};
     size_t pin_cap = 0;
+    // seen-aware calls: candidate rank keys and counts of the batch kernel; the batch's seen rows as uploaded (sp / sk,
+    // staged through two pinned slots) and, for rows given unsorted, the device radix sort's scratch and output
+    DevBuf<unsigned long long> cand_k;
+    DevBuf<int32_t> cand_cnt;
+    DevBuf<int64_t> sp, sorted_sp;
+    DevBuf<int32_t> sk, sorted_sk, sort_major;
+    DevBuf<float> sort_vals;
+    cudaEvent_t staged[2] = {nullptr, nullptr};
+    int64_t* pin_sp[2] = {nullptr, nullptr};
+    int32_t* pin_sk[2] = {nullptr, nullptr};
+    size_t pin_sp_cap = 0, pin_sk_cap = 0;
 
     int attach() {
         if (compute) return BFL_OK;
@@ -335,6 +450,7 @@ struct bfl_serve {
         for (int s = 0; s < 2; ++s) {
             BFL_CUDA(cudaEventCreateWithFlags(&scored[s], cudaEventDisableTiming));
             BFL_CUDA(cudaEventCreateWithFlags(&copied[s], cudaEventDisableTiming));
+            BFL_CUDA(cudaEventCreateWithFlags(&staged[s], cudaEventDisableTiming));
         }
         return BFL_OK;
     }
@@ -357,13 +473,36 @@ struct bfl_serve {
         }
         pin_cap = 0;
     }
+    // the two pinned slots the seen rows of a batch are staged in: rows END offsets and n_keys keys each
+    int reserve_seen_pinned(size_t rows, size_t n_keys) {
+        if (rows <= pin_sp_cap && n_keys <= pin_sk_cap) return BFL_OK;
+        release_seen_pinned();
+        for (int s = 0; s < 2; ++s) {
+            BFL_CUDA(cudaMallocHost(&pin_sp[s], rows * sizeof(int64_t)));
+            BFL_CUDA(cudaMallocHost(&pin_sk[s], n_keys * sizeof(int32_t)));
+        }
+        pin_sp_cap = rows;
+        pin_sk_cap = n_keys;
+        return BFL_OK;
+    }
+    void release_seen_pinned() {
+        for (int s = 0; s < 2; ++s) {
+            if (pin_sp[s]) cudaFreeHost(pin_sp[s]);
+            if (pin_sk[s]) cudaFreeHost(pin_sk[s]);
+            pin_sp[s] = nullptr;
+            pin_sk[s] = nullptr;
+        }
+        pin_sp_cap = pin_sk_cap = 0;
+    }
     ~bfl_serve() {
         if (compute) cudaStreamSynchronize(compute);
         if (copy) cudaStreamSynchronize(copy);
         release_pinned();
+        release_seen_pinned();
         for (int s = 0; s < 2; ++s) {
             if (scored[s]) cudaEventDestroy(scored[s]);
             if (copied[s]) cudaEventDestroy(copied[s]);
+            if (staged[s]) cudaEventDestroy(staged[s]);
         }
         if (compute) cudaStreamDestroy(compute);
         if (copy) cudaStreamDestroy(copy);
@@ -402,11 +541,20 @@ struct bfl_serve {
         if (nsl * k > INT_MAX) BFL_FAIL(BFL_ERR_ARG, "serve: too many candidates for this k");
         return BFL_OK;
     }
-    // one batch, stream-ordered: d_qidx[0..nb) -> d_out_i / d_out_v [nb x k]
-    int run_batch(const int32_t* d_qidx, int64_t nb, int k, int32_t* d_out_i, float* d_out_v, cudaStream_t st);
+    // one batch, stream-ordered: d_qidx[0..nb) -> d_out_i / d_out_v [nb x k]; with seen rows, query q of the batch
+    // leaves out the items of its row
+    int run_batch(const int32_t* d_qidx, int64_t nb, int k, int32_t* d_out_i, float* d_out_v, cudaStream_t st,
+                  const SeenRows* seen = nullptr);
+    // the host-array call of bfl_serve_topk and bfl_seen_topk (seen_indptr == nullptr: no seen rows)
+    int topk_host(const int32_t* query_idx, int64_t n, int k, int32_t* out_idx, float* out_val,
+                  const int64_t* seen_indptr, const int32_t* seen_keys);
+    // uploads the seen rows [r0, r0 + nb) of a host CSR through pinned slot s; sorts them on the device when unsorted
+    int stage_seen(const int64_t* indptr, const int32_t* keys, int64_t r0, int64_t nb, bool unsorted, int s,
+                   SeenRows* out);
 };
 
-int bfl_serve::run_batch(const int32_t* d_qidx, int64_t nb, int k, int32_t* d_out_i, float* d_out_v, cudaStream_t st) {
+int bfl_serve::run_batch(const int32_t* d_qidx, int64_t nb, int k, int32_t* d_out_i, float* d_out_v, cudaStream_t st,
+                         const SeenRows* seen) {
     const int64_t nc = n_cand();
     const int32_t* dpool = n_pool >= 0 ? pool.p : nullptr;
     if (!batch_kernel(nb)) {
@@ -427,32 +575,151 @@ int bfl_serve::run_batch(const int32_t* d_qidx, int64_t nb, int k, int32_t* d_ou
                 bs = gb.p;
             }
         }
-        const int rc = bfl_topk_device(gq.p, nb, ldq, it, nc, ldi, bs, d, k, d_out_i, d_out_v, st);
+        const int rc = seen ? masked_topk(gq.p, nb, ldq, it, nc, ldi, bs, d, k, seen->indptr, seen->keys, seen->row,
+                                          dpool, d_out_i, d_out_v, st)
+                            : bfl_topk_device(gq.p, nb, ldq, it, nc, ldi, bs, d, k, d_out_i, d_out_v, st);
         if (rc != BFL_OK) return rc;
     } else {
         const int nslices = (int)((nc + SV_SLICE - 1) / SV_SLICE);
         const int ncand = nslices * k;
-        if (BFL_OK != cand_v.reserve((size_t)nb * ncand) || BFL_OK != cand_i.reserve((size_t)nb * ncand))
+        if (seen ? (BFL_OK != cand_k.reserve((size_t)nb * ncand) || BFL_OK != cand_cnt.reserve((size_t)nb * nslices))
+                 : (BFL_OK != cand_v.reserve((size_t)nb * ncand) || BFL_OK != cand_i.reserve((size_t)nb * ncand)))
             return BFL_ERR_CUDA;
         const int IR = d <= 128 ? 2 : 1;
         int tile_floats = 0;
-        const size_t smem = slice_smem_bytes(d, IR, &tile_floats);
+        const size_t smem = slice_smem_bytes(d, IR, seen != nullptr, &tile_floats);
         // bulk copies need 16-byte aligned rows of a multiple of 16 bytes (bind_items_device checks the base address);
         // other row shapes are staged with plain loads
         const int bulk = (ldi & 3) == 0 && (d & 3) == 0;
-        auto kern = IR == 2 ? serve_slice_kernel<2> : serve_slice_kernel<1>;
-        BFL_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         dim3 grid(nslices, (unsigned)((nb + SV_QT - 1) / SV_QT));
-        kern<<<grid, SV_THREADS, smem, st>>>(queries, n_q, ldq, d_qidx, (int)nb, items, ldi, nc, dpool, bias, d, k, nslices,
-                                             bulk, tile_floats, cand_v.p, cand_i.p);
+        if (seen) {
+            auto kern = IR == 2 ? serve_slice_seen_kernel<2> : serve_slice_seen_kernel<1>;
+            BFL_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            kern<<<grid, SV_THREADS, smem, st>>>(queries, n_q, ldq, d_qidx, (int)nb, items, ldi, nc, dpool, bias, d, k,
+                                                 nslices, bulk, tile_floats, *seen, cand_k.p, cand_cnt.p);
+        } else {
+            auto kern = IR == 2 ? serve_slice_kernel<2> : serve_slice_kernel<1>;
+            BFL_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            kern<<<grid, SV_THREADS, smem, st>>>(queries, n_q, ldq, d_qidx, (int)nb, items, ldi, nc, dpool, bias, d, k,
+                                                 nslices, bulk, tile_floats, cand_v.p, cand_i.p);
+        }
         BFL_LAUNCHED();
-        const int rc = topk_merge(cand_v.p, cand_i.p, nb, ncand, k, d_out_i, d_out_v, st);
+        const int rc = seen ? seen_merge(cand_k.p, cand_cnt.p, nb, nslices, k, d_out_i, d_out_v, st)
+                            : topk_merge(cand_v.p, cand_i.p, nb, ncand, k, d_out_i, d_out_v, st);
         if (rc != BFL_OK) return rc;
     }
     const size_t n = (size_t)nb * k;
     serve_finish_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_out_i, d_out_v, n, dpool);
     BFL_LAUNCHED();
     return BFL_OK;
+}
+
+int bfl_serve::stage_seen(const int64_t* indptr, const int32_t* keys, int64_t r0, int64_t nb, bool unsorted, int s,
+                          SeenRows* out) {
+    const int64_t kb = r0 > 0 ? indptr[r0 - 1] : 0, nk = indptr[r0 + nb - 1] - kb;
+    // slot s was last read by the upload of the batch before the previous one
+    BFL_CUDA(cudaEventSynchronize(staged[s]));
+    memcpy(pin_sk[s], keys + kb, sizeof(int32_t) * (size_t)nk);
+    for (int64_t i = 0; i < nb; ++i) pin_sp[s][i] = indptr[r0 + i] - kb;
+    if (BFL_OK != sp.reserve((size_t)nb) || BFL_OK != sk.reserve((size_t)(nk > 0 ? nk : 1))) return BFL_ERR_CUDA;
+    BFL_CUDA(cudaMemcpyAsync(sp.p, pin_sp[s], sizeof(int64_t) * (size_t)nb, cudaMemcpyHostToDevice, compute));
+    BFL_CUDA(cudaMemcpyAsync(sk.p, pin_sk[s], sizeof(int32_t) * (size_t)nk, cudaMemcpyHostToDevice, compute));
+    BFL_CUDA(cudaEventRecord(staged[s], compute));
+    *out = SeenRows{sp.p, sk.p, nullptr};
+    if (!unsorted) return BFL_OK;
+    // rows in session order (or with duplicates out of place): the device radix sort of the ingest path, by (row, key)
+    if (BFL_OK != sorted_sp.reserve((size_t)nb) || BFL_OK != sorted_sk.reserve((size_t)nk) ||
+        BFL_OK != sort_major.reserve((size_t)nk) || BFL_OK != sort_vals.reserve((size_t)nk))
+        return BFL_ERR_CUDA;
+    const unsigned g = (unsigned)std::min<int64_t>((nb + 7) / 8, 4096);
+    seen_row_ids_kernel<<<g, 256, 0, compute>>>(sp.p, nb, sort_major.p);
+    BFL_LAUNCHED();
+    // the values ride along and are dropped: only the order of the keys is wanted
+    const int rc = bfl_csr_from_triples_device(sort_major.p, sk.p, sort_vals.p, nk, (int32_t)nb, (int32_t)n_items, 1,
+                                               sorted_sp.p, sorted_sk.p, sort_vals.p, compute);
+    if (rc != BFL_OK) return rc;
+    *out = SeenRows{sorted_sp.p, sorted_sk.p, nullptr};
+    return BFL_OK;
+}
+
+int bfl_serve::topk_host(const int32_t* query_idx, int64_t n, int k, int32_t* out_idx, float* out_val,
+                         const int64_t* seen_indptr, const int32_t* seen_keys) {
+    int rc = BFL_OK;
+    // batches of at most batch_rows(k) queries; with seen rows also of at most SV_SEEN_KEYS seen keys, unless a single
+    // row holds more (it is then a batch of its own)
+    const int64_t B = batch_rows(k) < n ? batch_rows(k) : n;
+    std::vector<int64_t> start{0};
+    int64_t max_keys = 1;
+    while (start.back() < n) {
+        const int64_t b0 = start.back();
+        int64_t e = n - b0 < B ? n : b0 + B;
+        if (seen_indptr) {
+            const int64_t kb = b0 > 0 ? seen_indptr[b0 - 1] : 0;
+            e = std::max<int64_t>(b0 + 1, std::upper_bound(seen_indptr + b0, seen_indptr + e, kb + SV_SEEN_KEYS) - seen_indptr);
+            max_keys = std::max<int64_t>(max_keys, seen_indptr[e - 1] - kb);
+        }
+        start.push_back(e);
+    }
+    const int64_t nbatch = (int64_t)start.size() - 1;
+    // batches holding a row that is not non-decreasing are sorted on the device
+    std::vector<char> unsorted(seen_indptr ? nbatch : 0, 0);
+    bool any_unsorted = false;
+    for (int64_t b = 0; b < (int64_t)unsorted.size(); ++b) {
+        for (int64_t r = start[b]; r < start[b + 1] && !unsorted[b]; ++r)
+            for (int64_t e = (r > 0 ? seen_indptr[r - 1] : 0) + 1; e < seen_indptr[r]; ++e)
+                if (seen_keys[e] < seen_keys[e - 1]) {
+                    unsorted[b] = 1;
+                    break;
+                }
+        any_unsorted |= unsorted[b] != 0;
+    }
+    const size_t per = (size_t)B * k;
+    if (BFL_OK != qidx.reserve((size_t)n) || BFL_OK != reserve_pinned(per)) return BFL_ERR_CUDA;
+    for (int s = 0; s < 2; ++s)
+        if (BFL_OK != out_i[s].reserve(per) || BFL_OK != out_v[s].reserve(per)) return BFL_ERR_CUDA;
+    // the seen buffers at their largest before the first batch: a reserve that grows frees a buffer kernels may read
+    if (seen_indptr && (BFL_OK != reserve_seen_pinned((size_t)B, (size_t)max_keys) || BFL_OK != sp.reserve((size_t)B) ||
+                        BFL_OK != sk.reserve((size_t)max_keys)))
+        return BFL_ERR_CUDA;
+    if (any_unsorted && (BFL_OK != sorted_sp.reserve((size_t)B) || BFL_OK != sorted_sk.reserve((size_t)max_keys) ||
+                         BFL_OK != sort_major.reserve((size_t)max_keys) || BFL_OK != sort_vals.reserve((size_t)max_keys)))
+        return BFL_ERR_CUDA;
+    BFL_CUDA(cudaMemcpyAsync(qidx.p, query_idx, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, compute));
+    // batch b is scored on `compute` into slot b & 1 and copied to that slot's pinned buffers on `copy`; the host
+    // drains batch b - 1 into the caller's arrays (and stages the seen rows of batch b + 1) while batch b runs
+    auto drain = [&](int64_t b) -> int {
+        const int s = (int)(b & 1);
+        const int64_t b0 = start[b], nb = start[b + 1] - b0;
+        BFL_CUDA(cudaEventSynchronize(copied[s]));
+        memcpy(out_idx + b0 * k, pin_i[s], sizeof(int32_t) * (size_t)nb * k);
+        if (out_val) memcpy(out_val + b0 * k, pin_v[s], sizeof(float) * (size_t)nb * k);
+        return BFL_OK;
+    };
+    for (int64_t b = 0; b < nbatch; ++b) {
+        const int s = (int)(b & 1);
+        const int64_t b0 = start[b], nb = start[b + 1] - b0;
+        SeenRows seen{};
+        if (seen_indptr) rc = stage_seen(seen_indptr, seen_keys, b0, nb, unsorted[b] != 0, s, &seen);
+        if (rc == BFL_OK) rc = run_batch(qidx.p + b0, nb, k, out_i[s].p, out_v[s].p, compute, seen_indptr ? &seen : nullptr);
+        if (rc == BFL_OK) {
+            BFL_CUDA(cudaEventRecord(scored[s], compute));
+            BFL_CUDA(cudaStreamWaitEvent(copy, scored[s], 0));
+            BFL_CUDA(cudaMemcpyAsync(pin_i[s], out_i[s].p, sizeof(int32_t) * (size_t)nb * k, cudaMemcpyDeviceToHost,
+                                     copy));
+            BFL_CUDA(cudaMemcpyAsync(pin_v[s], out_v[s].p, sizeof(float) * (size_t)nb * k, cudaMemcpyDeviceToHost,
+                                     copy));
+            BFL_CUDA(cudaEventRecord(copied[s], copy));
+            if (b > 0) rc = drain(b - 1);
+        }
+        if (rc != BFL_OK) {   // leave nothing in flight behind a failed call
+            cudaStreamSynchronize(compute);
+            cudaStreamSynchronize(copy);
+            return rc;
+        }
+    }
+    rc = drain(nbatch - 1);
+    BFL_CUDA(cudaStreamSynchronize(compute));
+    return rc;
 }
 
 extern "C" {
@@ -575,46 +842,44 @@ int bfl_serve_topk(bfl_serve_t* h, const int32_t* query_idx, int64_t n, int k, i
     if (rc != BFL_OK) return rc;
     for (int64_t i = 0; i < n; ++i)
         if (query_idx[i] < 0 || query_idx[i] >= h->n_q) BFL_FAIL(BFL_ERR_ARG, "serve: query index out of range");
-    const int64_t B = h->batch_rows(k) < n ? h->batch_rows(k) : n;
-    const size_t per = (size_t)B * k;
-    if (BFL_OK != h->qidx.reserve((size_t)n) || BFL_OK != h->reserve_pinned(per)) return BFL_ERR_CUDA;
-    for (int s = 0; s < 2; ++s)
-        if (BFL_OK != h->out_i[s].reserve(per) || BFL_OK != h->out_v[s].reserve(per)) return BFL_ERR_CUDA;
-    BFL_CUDA(cudaMemcpyAsync(h->qidx.p, query_idx, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, h->compute));
-    // batch b is scored on `compute` into slot b & 1 and copied to that slot's pinned buffers on `copy`; the host
-    // drains batch b - 1 into the caller's arrays while batch b runs
-    auto drain = [&](int64_t b) -> int {
-        const int s = (int)(b & 1);
-        const int64_t b0 = b * B, nb = n - b0 < B ? n - b0 : B;
-        BFL_CUDA(cudaEventSynchronize(h->copied[s]));
-        memcpy(out_idx + b0 * k, h->pin_i[s], sizeof(int32_t) * (size_t)nb * k);
-        if (out_val) memcpy(out_val + b0 * k, h->pin_v[s], sizeof(float) * (size_t)nb * k);
-        return BFL_OK;
-    };
-    const int64_t nbatch = (n + B - 1) / B;
-    for (int64_t b = 0; b < nbatch; ++b) {
-        const int s = (int)(b & 1);
-        const int64_t b0 = b * B, nb = n - b0 < B ? n - b0 : B;
-        rc = h->run_batch(h->qidx.p + b0, nb, k, h->out_i[s].p, h->out_v[s].p, h->compute);
-        if (rc == BFL_OK) {
-            BFL_CUDA(cudaEventRecord(h->scored[s], h->compute));
-            BFL_CUDA(cudaStreamWaitEvent(h->copy, h->scored[s], 0));
-            BFL_CUDA(cudaMemcpyAsync(h->pin_i[s], h->out_i[s].p, sizeof(int32_t) * (size_t)nb * k, cudaMemcpyDeviceToHost,
-                                     h->copy));
-            BFL_CUDA(cudaMemcpyAsync(h->pin_v[s], h->out_v[s].p, sizeof(float) * (size_t)nb * k, cudaMemcpyDeviceToHost,
-                                     h->copy));
-            BFL_CUDA(cudaEventRecord(h->copied[s], h->copy));
-            if (b > 0) rc = drain(b - 1);
-        }
-        if (rc != BFL_OK) {   // leave nothing in flight behind a failed call
-            cudaStreamSynchronize(h->compute);
-            cudaStreamSynchronize(h->copy);
-            return rc;
-        }
+    return h->topk_host(query_idx, n, k, out_idx, out_val, nullptr, nullptr);
+}
+
+int bfl_seen_topk(bfl_serve_t* h, const int32_t* query_idx, int64_t n, int k, const int64_t* seen_indptr,
+                  const int32_t* seen_keys, int32_t* out_idx, float* out_val) {
+    if (!h) BFL_FAIL(BFL_ERR_ARG, "serve: null handle");
+    int rc = h->check_ready(n, k, query_idx, out_idx);
+    if (rc != BFL_OK) return rc;
+    if (!seen_indptr) BFL_FAIL(BFL_ERR_ARG, "serve: the seen rows need their END offsets");
+    for (int64_t i = 0; i < n; ++i)
+        if (query_idx[i] < 0 || query_idx[i] >= h->n_q) BFL_FAIL(BFL_ERR_ARG, "serve: query index out of range");
+    int64_t prev = 0;
+    for (int64_t i = 0; i < n; ++i) {
+        if (seen_indptr[i] < prev) BFL_FAIL(BFL_ERR_ARG, "serve: seen END offsets must be non-decreasing from 0");
+        prev = seen_indptr[i];
     }
-    rc = drain(nbatch - 1);
-    BFL_CUDA(cudaStreamSynchronize(h->compute));
-    return rc;
+    if (prev > 0 && !seen_keys) BFL_FAIL(BFL_ERR_ARG, "serve: seen keys missing");
+    for (int64_t e = 0; e < prev; ++e)
+        if (seen_keys[e] < 0 || seen_keys[e] >= h->n_items) BFL_FAIL(BFL_ERR_ARG, "serve: seen key out of range");
+    return h->topk_host(query_idx, n, k, out_idx, out_val, seen_indptr, seen_keys);
+}
+
+int bfl_seen_topk_device(bfl_serve_t* h, const int32_t* d_query_idx, int64_t n, int k, const int64_t* d_seen_indptr,
+                         const int32_t* d_seen_keys, const int32_t* d_seen_row, int32_t* d_out_idx, float* d_out_val,
+                         void* stream) {
+    if (!h) BFL_FAIL(BFL_ERR_ARG, "serve: null handle");
+    int rc = h->check_ready(n, k, d_query_idx, d_out_idx);
+    if (rc != BFL_OK) return rc;
+    if (!d_out_val) BFL_FAIL(BFL_ERR_ARG, "serve: the device variant needs d_out_val");
+    if (!d_seen_indptr || !d_seen_keys || !d_seen_row) BFL_FAIL(BFL_ERR_ARG, "serve: bad seen rows");
+    const int64_t B = h->batch_rows(k);
+    for (int64_t b0 = 0; b0 < n; b0 += B) {
+        const int64_t nb = n - b0 < B ? n - b0 : B;
+        const SeenRows seen{d_seen_indptr, d_seen_keys, d_seen_row + b0};
+        rc = h->run_batch(d_query_idx + b0, nb, k, d_out_idx + b0 * k, d_out_val + b0 * k, (cudaStream_t)stream, &seen);
+        if (rc != BFL_OK) return rc;
+    }
+    return BFL_OK;
 }
 
 }  // extern "C"

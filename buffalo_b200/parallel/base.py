@@ -3,6 +3,7 @@ buffalo/parallel/_core.hpp:88-142 (best-first indexes, -1 padded).  With a GPU t
 handle that keeps the item factors resident (DESIGN.md 4.9); without one, or above its limits, the NumPy
 implementation below runs."""
 import numpy as np
+import scipy.sparse
 
 from buffalo_b200 import backend
 
@@ -16,11 +17,15 @@ def quickselect(scores, result, sorted=True, num_threads=4):
     result[:, :part.shape[1]] = part
 
 
-def dot_topn(indexes, P, Q, Qb, out_keys, out_scores, pool, topk, num_workers=4):
+def dot_topn(indexes, P, Q, Qb, out_keys, out_scores, pool, topk, num_workers=4, seen_indptr=None, seen_keys=None):
+    """seen_indptr / seen_keys (optional): a CSR of END offsets whose row i holds item ids query i does not get back."""
     cand = Q if pool is None or len(pool) == 0 else Q[pool]
     scores = P[indexes].dot(cand.T)
     if Qb is not None and Qb.size:
         scores = scores + (Qb if pool is None or len(pool) == 0 else Qb[pool]).reshape(1, -1)
+    if seen_indptr is not None:
+        _topn_unseen(scores, Q.shape[0], pool, topk, seen_indptr, seen_keys, out_keys, out_scores)
+        return
     k = min(topk, scores.shape[1])
     part = np.argpartition(-scores, k - 1, axis=1)[:, :k]
     vals = np.take_along_axis(scores, part, axis=1)
@@ -30,6 +35,24 @@ def dot_topn(indexes, P, Q, Qb, out_keys, out_scores, pool, topk, num_workers=4)
     out_scores[:] = 0
     out_keys[:, :k] = part if pool is None or len(pool) == 0 else np.asarray(pool)[part]
     out_scores[:, :k] = vals
+
+
+def _topn_unseen(scores, num_items, pool, topk, seen_indptr, seen_keys, out_keys, out_scores):
+    """dot_topn's result with the seen candidates of each row left out: one stable sort on (seen, -score), so ties go
+    to the smaller position and no score value marks a seen candidate; -1 / 0 pad rows left with fewer than topk."""
+    n, C = scores.shape
+    lens = np.diff(np.asarray(seen_indptr, dtype=np.int64), prepend=0)
+    seen = np.zeros((n, num_items), dtype=bool)
+    seen[np.repeat(np.arange(n), lens), np.asarray(seen_keys)[:int(lens.sum())]] = True
+    if pool is not None and len(pool):
+        seen = seen[:, np.asarray(pool)]
+    k = min(topk, C)
+    order = np.lexsort((-scores, seen), axis=-1)[:, :k]
+    valid = np.arange(k)[None, :] < (C - seen.sum(axis=1))[:, None]
+    out_keys[:] = -1
+    out_scores[:] = 0
+    out_keys[:, :k] = np.where(valid, order if pool is None or len(pool) == 0 else np.asarray(pool)[order], -1)
+    out_scores[:, :k] = np.where(valid, np.take_along_axis(scores, order, axis=1), 0)
 
 
 class Parallel(object):
@@ -65,7 +88,8 @@ class Parallel(object):
             self._serve_key = key
         return self._serve
 
-    def _run(self, indexes, A, B, Bb, topk, pool):
+    def _run(self, indexes, A, B, Bb, topk, pool, seen=None):
+        """seen: None, or (END offsets int64, keys int32) whose row i holds the items query indexes[i] must not get."""
         if Bb is not None and not Bb.size:
             Bb = None
         # On the device when one is present and the call is within the kernels' limits.  The items must fit in device
@@ -78,10 +102,15 @@ class Parallel(object):
             # only the rows asked for go to the device, read from the live array at every call
             h.set_queries(np.ascontiguousarray(A[indexes]))
             h.set_pool(None if pool is None or len(pool) == 0 else pool)
+            if seen is not None:
+                return h.topk_seen(np.arange(len(indexes), dtype=np.int32), topk, *seen)
             return h.topk(np.arange(len(indexes), dtype=np.int32), topk)
         keys = np.zeros((len(indexes), topk), dtype=np.int32)
         scores = np.zeros((len(indexes), topk), dtype=np.float32)
-        dot_topn(indexes, A, B, Bb, keys, scores, pool, topk, self.num_workers)
+        if seen is not None:
+            dot_topn(indexes, A, B, Bb, keys, scores, pool, topk, self.num_workers, *seen)
+        else:
+            dot_topn(indexes, A, B, Bb, keys, scores, pool, topk, self.num_workers)
         return keys, scores
 
 
@@ -110,12 +139,42 @@ class ParALS(Parallel):
             topks = [[names[t] for t in tt if t != -1] for tt in topks]
         return topks, scores
 
-    def topk_recommendation(self, keys, topk=10, pool=None, repr=False):
+    def _seen_rows(self, idx, exclude_seen):
+        """(END offsets int64, keys int32) of the seen rows of users idx: rows of the algo's training data ("rowwise"
+        group) for exclude_seen=True, of a scipy sparse (num_users, num_items) matrix otherwise."""
+        num_users, num_items = self.algo.P.shape[0], self.algo.Q.shape[0]
+        if scipy.sparse.issparse(exclude_seen):
+            m = exclude_seen.tocsr()
+            if m.shape != (num_users, num_items):
+                raise ValueError("exclude_seen must be a (%d, %d) matrix, got %s" % (num_users, num_items, m.shape))
+            ends = np.asarray(m.indptr[1:], dtype=np.int64)
+            keys = np.asarray(m.indices[:int(m.indptr[-1])])
+            if keys.size and (keys.min() < 0 or keys.max() >= num_items):
+                raise ValueError("exclude_seen holds a column outside [0, %d)" % num_items)
+        else:
+            data = getattr(self.algo, "data", None)
+            if data is None:
+                raise ValueError("exclude_seen=True needs the training data attached to the model; pass a scipy "
+                                 "sparse (num_users, num_items) matrix of the seen items instead")
+            grp = data.get_group("rowwise")
+            ends = np.asarray(grp["indptr"][:], dtype=np.int64)
+            keys = np.asarray(grp["key"][:int(ends[-1]) if len(ends) else 0])
+        from buffalo_b200.evaluate.device import _gather_rows
+        return _gather_rows(ends, keys, idx)
+
+    def topk_recommendation(self, keys, topk=10, pool=None, repr=False, exclude_seen=False):
+        """exclude_seen: False; True to leave out each user's training items (the "rowwise" rows of the algo's data);
+        or a scipy sparse (num_users, num_items) matrix whose row u lists the items user u does not get back.  Rows
+        left with fewer than topk candidates are padded with -1 / 0.0."""
         if self.algo.opt._nrz_P or self.algo.opt._nrz_Q:
             raise RuntimeError("Cannot make topk recommendation with normalized factors")
         kept, idx, pool = self._resolve(keys, pool, "user")
         Qb = self.algo.Qb if self._bias and self.algo.opt.get("use_bias") else None
-        topks, scores = self._run(idx, self.algo.P, self.algo.Q, Qb, topk, pool)
+        if scipy.sparse.issparse(exclude_seen) or exclude_seen:
+            seen = self._seen_rows(idx, exclude_seen)
+            topks, scores = self._run(idx, self.algo.P, self.algo.Q, Qb, topk, pool, seen)
+        else:
+            topks, scores = self._run(idx, self.algo.P, self.algo.Q, Qb, topk, pool)
         if repr:
             topks = [[self.algo._idmanager.itemids[t] for t in tt if t != -1] for tt in topks]
         return kept, topks, scores

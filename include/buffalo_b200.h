@@ -346,6 +346,25 @@ int bfl_serve_topk_device(bfl_serve_t* h, const int32_t* d_query_idx, int64_t n,
                           float* d_out_val, void* stream);
 
 /* =====================================================================================
+ * Batch serving top-k without each query's seen items (DESIGN.md 4.9), on a serve handle: what bfl_serve_topk /
+ * bfl_serve_topk_device return with the query's seen items left out of its candidates (with a pool: the pool's
+ * candidates whose item is seen).  The survivors keep their order, keys and score bits; -1 / 0.0f pad when fewer
+ * than k candidates remain.  The seen rows are arguments of the call, so nothing of them stays on the handle.
+ *  - seen_topk: HOST arrays.  seen_indptr[n] END offsets (row i holds the items of query i: seen_keys[seen_indptr[i - 1]
+ *    .. seen_indptr[i]), from 0), keys in [0, n_items), any order, duplicates allowed.  Each batch's rows are staged
+ *    through two pinned buffers and uploaded next to it; rows not in ascending order are sorted on the device.  A
+ *    batch also holds at most 2^24 seen keys (a longer row is a batch of its own).  Non-monotone offsets or a key out
+ *    of range is BFL_ERR_ARG before any device work.
+ *  - seen_topk_device: DEVICE arrays, stream-ordered; query q reads row d_seen_row[q] of the CSR (END offsets, rows
+ *    non-decreasing: the caller sorts them, e.g. with bfl_csr_from_triples_device).
+ * ===================================================================================== */
+int bfl_seen_topk(bfl_serve_t* h, const int32_t* query_idx, int64_t n, int k, const int64_t* seen_indptr,
+                  const int32_t* seen_keys, int32_t* out_idx, float* out_val /* nullable */);
+int bfl_seen_topk_device(bfl_serve_t* h, const int32_t* d_query_idx, int64_t n, int k, const int64_t* d_seen_indptr,
+                         const int32_t* d_seen_keys, const int32_t* d_seen_row, int32_t* d_out_idx, float* d_out_val,
+                         void* stream);
+
+/* =====================================================================================
  * Validation metrics on the device (DESIGN.md 4.8): the device path of Evaluable.get_validation_results
  * (buffalo/evaluate/base.py:44-148).  Device pointers, stream-ordered.  A "seen" CSR (END offsets, int32 keys, every
  * row non-decreasing) holds training rows; seen_row[q] names the row of query q.  The held-out CSR is indexed by user.
