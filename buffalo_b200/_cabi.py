@@ -101,6 +101,7 @@ PROTOTYPES = {
     "bfl_plsi_item_segment_len": (C.c_int, []),
     "bfl_plsi_bind_colwise_csr_device": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64]),
     "bfl_plsi_update_items_device": (C.c_int, [_vp, _i64, _i64, _vp]),
+    "bfl_plsi_fold_in_device": (C.c_int, [_vp, _vp, _i64, _vp, _vp, _vp, _i64, _i64, _vp, C.c_int, _f, _vp]),
     # evaluation top-k
     "bfl_topk_device": (C.c_int, [_vp, _i64, C.c_int, _vp, _i64, C.c_int, _vp, C.c_int, C.c_int, _vp, _vp, _vp]),
     "bfl_topk_host": (C.c_int, [_vp, _i64, C.c_int, _vp, _i64, C.c_int, _vp, C.c_int, C.c_int, _vp, _vp]),

@@ -11,6 +11,7 @@ import time
 
 import numpy as np
 
+from buffalo_b200.algo import fold_in
 from buffalo_b200.algo.base import Algo, Serializable
 from buffalo_b200.algo.options import ALSOption
 from buffalo_b200.backend import CuALS
@@ -85,6 +86,44 @@ class ALS(Algo, ALSOption, Evaluable, Serializable):
 
     def _device_eval_model(self):
         return EvalModel(self.P, self.Q, None, None, False)
+
+    # ---- fold-in (DESIGN.md 4.10) -------------------------------------------------------------
+    def fold_in(self, histories, init=None, sweeps=1):
+        """float32 [n, d] user rows for n histories, with the item factors fixed: `sweeps` applications of the row
+        solve that train()'s user half-epoch applies (the model's optimizer and options, against the Gram of the current
+        Q).  histories: a scipy sparse (n, num_items) matrix in the units of the training data, or a list of n lists of
+        item ids (unknown ids dropped, value 1.0).  init: None (zero rows) or an (n, d) array of start rows, e.g.
+        self.P[rows] for returning users.  Rows without history keep their start row.  P, Q and the training holder
+        are not touched.  On the GPU only: without one the backend's "no CPU fallback" error is raised."""
+        tX, _ = self._fold_in_device(histories, init, sweeps)
+        return tX[:, :self.opt.d].cpu().numpy()
+
+    def _fold_in_device(self, histories, init=None, sweeps=1):
+        """fold_in's rows as a torch CUDA tensor [n, vdim] (padding zero), and the histories' device CSR
+        (END offsets int64, keys int32, vals float32; keys / vals hold at least one element)."""
+        if self.opt._nrz_Q:
+            raise RuntimeError("Cannot fold in users with normalized item factors")
+        sweeps = fold_in.positive_int(sweeps, "sweeps")
+        st, h, (ind_t, keys_t, vals_t, tX) = fold_in.begin(self, CuALS, histories, init, 0.0)
+        n = tX.shape[0]
+        if n:
+            import torch
+            try:
+                h.bind_factors(tX, st.Q)
+                if st.derived_key != st.key:            # the Gram of this Q, computed once
+                    st.derived_key = None
+                    h.precompute_device(0)
+                    st.derived_key = st.key
+                h.bind_csr(0, ind_t, keys_t, vals_t)
+                # the loss pair train() passes as well, so the solve is the very instantiation of the user half-epoch
+                loss = torch.zeros(2, dtype=torch.float64, device=tX.device)
+                for _ in range(sweeps):
+                    h.update_device(0, 0, n, loss)
+            finally:
+                # the rows and the CSR belong to this call and are freed with its results (every call binds its own
+                # before it solves); the holder keeps only its scratch, the resident Q is st.Q
+                h._keep = []
+        return tX, (ind_t, keys_t, vals_t)
 
     # ---- training -----------------------------------------------------------------------------
     def _get_buffer(self):

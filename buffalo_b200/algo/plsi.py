@@ -15,6 +15,7 @@ import time
 
 import numpy as np
 
+from buffalo_b200.algo import fold_in
 from buffalo_b200.algo.base import Algo, Serializable
 from buffalo_b200.algo.options import PLSIOption
 from buffalo_b200.backend import CuPLSI
@@ -121,6 +122,24 @@ class PLSI(Algo, PLSIOption, Evaluable, Serializable):
 
     def _device_eval_model(self):
         return EvalModel(self.P, self.Q, None, None, False)
+
+    # ---- fold-in (DESIGN.md 4.10) -------------------------------------------------------------
+    def fold_in(self, histories, init=None, iters=None):
+        """float32 [n, d] rows p(z|u) for n histories by Hofmann's folding-in: `iters` EM iterations on each row with
+        the item factors Q fixed.  An iteration is the row pass of training (acc = sum v * l / sum(l),
+        l = max(p * q, 1e-10)) followed by its row normalisation ((acc + alpha1 / d) / sum).  histories: a scipy sparse
+        (n, num_items) matrix or a list of n lists of item ids (unknown ids dropped, value 1.0).  init: None (the
+        uniform row 1/d) or an (n, d) array; iters: None means opt.num_iters.  Rows without history keep their start
+        row.  P, Q and the training holder are not touched.  On the GPU only (kernel plsi_fold_in_kernel)."""
+        tX, _ = self._fold_in_device(histories, init, iters)
+        return tX[:, :self.opt.d].cpu().numpy()
+
+    def _fold_in_device(self, histories, init=None, iters=None):
+        """fold_in's rows as a torch CUDA tensor [n, vdim] (padding zero), and the histories' device CSR."""
+        iters = fold_in.positive_int(self.opt.num_iters if iters is None else iters, "iters")
+        st, h, (ind_t, keys_t, vals_t, tX) = fold_in.begin(self, CuPLSI, histories, init, 1.0 / self.opt.d)
+        h.fold_in_device(st.Q, ind_t, keys_t, vals_t, tX, iters, self.opt.alpha1)
+        return tX, (ind_t, keys_t, vals_t)
 
     # ---- training -----------------------------------------------------------------------------
     def _deterministic(self):

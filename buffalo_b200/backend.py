@@ -408,6 +408,21 @@ class CuPLSI(_Holder):
     def swap_device(self, stream=None):
         _cabi.check(self._lib.bfl_plsi_swap_device(self._h, _stream_ptr(stream)), "swap_device")
 
+    def fold_in_device(self, Q, indptr, keys, vals, X, iters, alpha1, stream=None):
+        """Folding-in (bfl_plsi_fold_in_device): `iters` EM iterations on the rows of X [rows, vdim] (start rows in,
+        results out) against the fixed item factors Q [Q_rows, vdim], for the history CSR indptr int64[rows] END
+        offsets, keys int32, vals float32.  All torch CUDA tensors; keys must lie in [0, Q_rows) (not checked here)."""
+        vdim = self.get_vdim()
+        if Q.ndim != 2 or X.ndim != 2 or Q.shape[1] != vdim or X.shape[1] != vdim:
+            raise ValueError("Q and X must be [rows, vdim=%d] (got %s, %s)" % (vdim, tuple(Q.shape), tuple(X.shape)))
+        if indptr.shape[0] != X.shape[0]:
+            raise ValueError("indptr must hold one END offset per row of X")
+        nnz = keys.shape[0]
+        _cabi.check(self._lib.bfl_plsi_fold_in_device(
+            self._h, _dev(Q, "float32", "Q"), Q.shape[0], _dev(indptr, "int64", "indptr"), _dev(keys, "int32", "keys"),
+            _dev(vals, "float32", "vals"), X.shape[0], nnz, _dev(X, "float32", "X"), int(iters), float(alpha1),
+            _stream_ptr(stream)), "bfl_plsi_fold_in_device")
+
 
 def device_available():
     """True when the CUDA library is loadable and a GPU is visible (used by host-side helpers that have a device

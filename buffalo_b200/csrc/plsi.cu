@@ -182,6 +182,122 @@ __global__ void __launch_bounds__(256) plsi_em_kernel(const EmArgs a) {
     }
 }
 
+struct FoldArgs {
+    const float* Q;          // [Q_rows x vdim] item factors, fixed
+    const int64_t* ends;     // END offsets of the history rows (row 0 starts at entry 0)
+    const int32_t* keys;     // item of each entry
+    const float* vals;
+    float* X;                // [n_rows x vdim]: start rows in, folded rows out
+    int64_t n_rows;
+    int iters, d, vdim;
+    float a1;                // alpha1 / d, as normalize_all passes it to the row normalisation
+};
+
+// Folding-in (Hofmann): EM on one user row with the item factors fixed.  One warp per history row, the lane layout of
+// plsi_em_kernel (G lanes per entry, NV float4 slices per lane, U item rows in flight per group).  The row stays in
+// registers for all `iters` iterations; each iteration streams the row's keys, values and item rows, accumulates as
+// the deterministic row pass does (a product, then a sum, in entry order per group; groups folded by a butterfly, so
+// every group holds the same bits), and divides (acc + a1) by its sum over the d real columns with the rounding of
+// plsi_normalize_rows_kernel.  No atomics and no shared state: the result depends on the row's own data only.  Rows
+// without entries keep their start row.  Only the final row is stored.
+template <int G, int NV, int U>
+__global__ void __launch_bounds__(256) plsi_fold_in_kernel(const FoldArgs a) {
+    constexpr int NG = 32 / G;
+    const int lane = threadIdx.x & 31, g = lane / G, gl = lane % G;
+    const int nv4 = a.vdim >> 2;
+    const int64_t warp0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t x = warp0; x < a.n_rows; x += nwarps) {
+        const int64_t beg = (x == 0) ? 0 : a.ends[x - 1];
+        const int64_t end = a.ends[x];
+        if (end <= beg) continue;
+        float* xrow = a.X + x * a.vdim;
+        float4 p[NV], acc[NV];
+#pragma unroll
+        for (int k = 0; k < NV; ++k) {
+            const int s = gl + G * k;
+            p[k] = s < nv4 ? *reinterpret_cast<const float4*>(xrow + 4 * s) : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+        for (int it = 0; it < a.iters; ++it) {
+#pragma unroll
+            for (int k = 0; k < NV; ++k) acc[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+            for (int64_t base = beg; base < end; base += 32) {
+                const int cnt = (int)min((int64_t)32, end - base);
+                const int my_key = lane < cnt ? __ldg(a.keys + base + lane) : 0;
+                const float my_val = lane < cnt ? __ldg(a.vals + base + lane) : 0.f;
+                for (int t = 0; t < cnt; t += NG * U) {
+                    bool ok[U];
+                    float v[U];
+                    float4 q[U][NV];
+#pragma unroll
+                    for (int u = 0; u < U; ++u) {
+                        const int e = t + u * NG + g;
+                        ok[u] = e < cnt;
+                        const int c = __shfl_sync(FULL, my_key, e & 31);
+                        v[u] = __shfl_sync(FULL, my_val, e & 31);
+#pragma unroll
+                        for (int k = 0; k < NV; ++k) {
+                            const int s = gl + G * k;
+                            q[u][k] = (ok[u] && s < nv4) ? ld4(a.Q + (int64_t)c * a.vdim + 4 * s)
+                                                         : make_float4(0.f, 0.f, 0.f, 0.f);
+                        }
+                    }
+#pragma unroll
+                    for (int u = 0; u < U; ++u) {
+                        float4 l[NV];
+                        float ps = 0.f;
+#pragma unroll
+                        for (int k = 0; k < NV; ++k) {
+                            l[k] = latent4(p[k], q[u][k], 4 * (gl + G * k), a.d);
+                            ps += (l[k].x + l[k].y) + (l[k].z + l[k].w);
+                        }
+#pragma unroll
+                        for (int o = G / 2; o > 0; o >>= 1) ps += __shfl_xor_sync(FULL, ps, o);
+                        const float w = ok[u] ? v[u] / ps : 0.f;
+#pragma unroll
+                        for (int k = 0; k < NV; ++k) {
+                            acc[k].x = __fadd_rn(acc[k].x, __fmul_rn(l[k].x, w));
+                            acc[k].y = __fadd_rn(acc[k].y, __fmul_rn(l[k].y, w));
+                            acc[k].z = __fadd_rn(acc[k].z, __fmul_rn(l[k].z, w));
+                            acc[k].w = __fadd_rn(acc[k].w, __fmul_rn(l[k].w, w));
+                        }
+                    }
+                }
+            }
+            float ps = 0.f;
+#pragma unroll
+            for (int k = 0; k < NV; ++k) {
+#pragma unroll
+                for (int o = G; o < 32; o <<= 1) {
+                    acc[k].x += __shfl_xor_sync(FULL, acc[k].x, o);
+                    acc[k].y += __shfl_xor_sync(FULL, acc[k].y, o);
+                    acc[k].z += __shfl_xor_sync(FULL, acc[k].z, o);
+                    acc[k].w += __shfl_xor_sync(FULL, acc[k].w, o);
+                }
+                const int col = 4 * (gl + G * k);
+                if (gl + G * k < nv4)
+                    ps += (col + 0 < a.d ? acc[k].x + a.a1 : 0.f) + (col + 1 < a.d ? acc[k].y + a.a1 : 0.f) +
+                          (col + 2 < a.d ? acc[k].z + a.a1 : 0.f) + (col + 3 < a.d ? acc[k].w + a.a1 : 0.f);
+            }
+#pragma unroll
+            for (int o = G / 2; o > 0; o >>= 1) ps += __shfl_xor_sync(FULL, ps, o);
+#pragma unroll
+            for (int k = 0; k < NV; ++k) {
+                const int col = 4 * (gl + G * k);
+                p[k].x = col + 0 < a.d ? (acc[k].x + a.a1) / ps : 0.f;
+                p[k].y = col + 1 < a.d ? (acc[k].y + a.a1) / ps : 0.f;
+                p[k].z = col + 2 < a.d ? (acc[k].z + a.a1) / ps : 0.f;
+                p[k].w = col + 3 < a.d ? (acc[k].w + a.a1) / ps : 0.f;
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < NV; ++k) {
+            const int s = gl + G * k;
+            if (g == 0 && s < nv4) *reinterpret_cast<float4*>(xrow + 4 * s) = p[k];
+        }
+    }
+}
+
 struct ItemArgs {
     const float* P;          // [P_rows x vdim] current user rows (read only during the pass)
     const float* Q;          // [Q_rows x vdim] current item rows (read only)
@@ -908,6 +1024,34 @@ int bfl_plsi_update_items_device(bfl_plsi_t* h, int64_t item_begin, int64_t item
     a.ends = h->ccsr.indptr + item_begin; a.keys = h->ccsr.keys; a.vals = h->ccsr.vals; a.shift = 0;
     a.item_begin = item_begin; a.n_items = item_end - item_begin;
     return launch_items(h, a, h->bound_long, la, lb, st);
+}
+
+int bfl_plsi_fold_in_device(bfl_plsi_t* h, const float* d_Q, int64_t Q_rows, const int64_t* d_indptr,
+                            const int32_t* d_keys, const float* d_vals, int64_t rows, int64_t nnz, float* d_X, int iters,
+                            float alpha1, void* stream) {
+    if (!h || !h->opt_set) BFL_FAIL(BFL_ERR_STATE, "init() must succeed before fold_in");
+    if (rows < 0 || nnz < 0 || Q_rows <= 0 || iters < 1) BFL_FAIL(BFL_ERR_ARG, "bad fold_in sizes (rows, nnz, Q_rows, iters)");
+    if (rows == 0) return BFL_OK;
+    if (!d_Q || !d_indptr || !d_X || (nnz > 0 && (!d_keys || !d_vals))) BFL_FAIL(BFL_ERR_ARG, "null fold_in argument");
+    if (((uintptr_t)d_Q | (uintptr_t)d_X) & 15) BFL_FAIL(BFL_ERR_ARG, "d_Q and d_X must be 16-byte aligned");
+    FoldArgs a;
+    a.Q = d_Q; a.ends = d_indptr; a.keys = d_keys; a.vals = d_vals; a.X = d_X; a.n_rows = rows;
+    a.iters = iters; a.d = h->d; a.vdim = h->vdim;
+    a.a1 = alpha1 / (float)h->d;                                   // normalize_all's alpha1 /= d
+    const int grid = grid_for(h, rows, 8, 16);
+    const int nv4 = h->vdim / 4;
+    cudaStream_t st = (cudaStream_t)stream;
+    // (G, NV, U) of plsi_em_kernel's default instantiations; U, the item rows in flight per group, changes no sum
+    if (nv4 <= 1) plsi_fold_in_kernel<1, 1, 2><<<grid, 256, 0, st>>>(a);
+    else if (nv4 <= 2) plsi_fold_in_kernel<2, 1, 2><<<grid, 256, 0, st>>>(a);
+    else if (nv4 <= 4) plsi_fold_in_kernel<4, 1, 2><<<grid, 256, 0, st>>>(a);
+    else if (nv4 <= 8) plsi_fold_in_kernel<8, 1, 2><<<grid, 256, 0, st>>>(a);
+    else if (nv4 <= 16) plsi_fold_in_kernel<16, 1, 3><<<grid, 256, 0, st>>>(a);   // U = 4 spills 4 bytes here
+    else if (nv4 <= 32) plsi_fold_in_kernel<32, 1, 4><<<grid, 256, 0, st>>>(a);
+    else if (nv4 <= 64) plsi_fold_in_kernel<32, 2, 4><<<grid, 256, 0, st>>>(a);
+    else plsi_fold_in_kernel<32, 4, 2><<<grid, 256, 0, st>>>(a);
+    BFL_LAUNCHED();
+    return BFL_OK;
 }
 
 }  // extern "C"

@@ -179,6 +179,42 @@ class ParALS(Parallel):
             topks = [[self.algo._idmanager.itemids[t] for t in tt if t != -1] for tt in topks]
         return kept, topks, scores
 
+    def fold_in_recommendation(self, histories, topk=10, pool=None, exclude_seen=True, repr=False):
+        """(topks, scores), one row per history row, for users folded into the model (DESIGN.md 4.10): the rows of
+        algo.fold_in(histories) with its defaults, ranked against the items as topk_recommendation ranks (pools, -1 / 0.0
+        padding).  exclude_seen: leave each row's history items out.  All on the device: the folded rows are bound as the
+        serve handle's queries and never reach the host.  Models with fold_in: ALS and PLSI."""
+        if not callable(getattr(self.algo, "_fold_in_device", None)):
+            raise NotImplementedError("fold_in_recommendation needs a model with fold_in (ALS, PLSI), not %s"
+                                      % type(self.algo).__name__)
+        topk = backend.Serve._check_k(topk)
+        if pool is not None:
+            pool = self.algo.get_index_pool(pool, group="item")
+            if len(pool) == 0:
+                raise RuntimeError("pool is empty")
+        tX, (indptr, keys, _) = self.algo._fold_in_device(histories)
+        n = tX.shape[0]
+        if n == 0:
+            return np.zeros((0, topk), np.int32), np.zeros((0, topk), np.float32)
+        import torch
+        h = self._serve_handle(np.ascontiguousarray(self.algo.Q, dtype=np.float32), None)
+        try:
+            h.bind_queries(tX)
+            h.set_pool(pool)
+            qidx = torch.arange(n, dtype=torch.int32, device=tX.device)
+            if exclude_seen:
+                idx, val = h.topk_seen_device(qidx, topk, indptr, keys)
+            else:
+                idx, val = h.topk_device(qidx, topk)
+            topks, scores = idx.cpu().numpy(), val.cpu().numpy()
+        finally:
+            # the folded rows are freed with this call; every query on the handle sets its own queries first
+            h._bound.pop("queries", None)
+            h.num_queries = 0
+        if repr:
+            topks = [[self.algo._idmanager.itemids[t] for t in tt if t != -1] for tt in topks]
+        return topks, scores
+
 
 class ParBPRMF(ParALS):
     _bias = True

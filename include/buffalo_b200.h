@@ -293,6 +293,16 @@ int bfl_plsi_update_items_device(bfl_plsi_t* h, int64_t item_begin, int64_t item
 int bfl_plsi_normalize_device(bfl_plsi_t* h, float alpha1, float alpha2, void* stream);
 /* copy the new item factors into dQ and zero the accumulator for the next iteration (no separate reset) */
 int bfl_plsi_swap_device(bfl_plsi_t* h, void* stream);
+/* Folding-in (DESIGN.md 4.10): `iters` EM iterations on each of `rows` user rows with the item factors fixed.  Per
+ * iteration a row becomes the row pass's sum of v * l / sum(l), l = max(x * q, 1e-10), then (acc + alpha1 / d) divided
+ * by its sum over the d columns, as bfl_plsi_normalize does (alpha1 is passed undivided, like there).  DEVICE arrays,
+ * stream-ordered: d_Q [Q_rows x vdim] and d_X [rows x vdim] 16-byte aligned, padding columns zero; d_indptr[rows] END
+ * offsets from 0, d_keys items in [0, Q_rows) (not checked), d_vals.  d_X holds the start rows in and the results out;
+ * rows without entries keep their start row.  Uses only the handle's options (d), not its factors or CSR; no atomics,
+ * so the same inputs give the same bits. */
+int bfl_plsi_fold_in_device(bfl_plsi_t* h, const float* d_Q, int64_t Q_rows, const int64_t* d_indptr,
+                            const int32_t* d_keys, const float* d_vals, int64_t rows, int64_t nnz, float* d_X, int iters,
+                            float alpha1, void* stream);
 
 /* =====================================================================================
  * Evaluation top-k (SURVEY.md 8(f-2)); replaces the host quickselect behind Evaluable.get_topk /
