@@ -4,13 +4,9 @@ BPRMF.prepare_sampling (bpr.py:99-111)."""
 import numpy as np
 import pytest
 
+from tests.sort_ref import numpy_csr
+
 pytestmark = pytest.mark.gpu
-
-
-def numpy_csr(major, minor, vals, num_major, stable_sort):
-    order = np.lexsort((minor, major)) if stable_sort else np.argsort(major, kind="stable")
-    indptr = np.cumsum(np.bincount(major, minlength=num_major)).astype(np.int64)
-    return indptr, minor[order].astype(np.int32), vals[order].astype(np.float32)
 
 
 @pytest.mark.parametrize("U,I,nnz,sort_minor", [(50, 30, 400, True), (3000, 70000, 250000, True), (100000, 900, 600000, True),
