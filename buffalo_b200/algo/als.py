@@ -109,11 +109,7 @@ class ALS(Algo, ALSOption, Evaluable, Serializable):
         if n:
             import torch
             try:
-                h.bind_factors(tX, st.Q)
-                if st.derived_key != st.key:            # the Gram of this Q, computed once
-                    st.derived_key = None
-                    h.precompute_device(0)
-                    st.derived_key = st.key
+                self._bind_fold_items(st, h, tX)
                 h.bind_csr(0, ind_t, keys_t, vals_t)
                 # the loss pair train() passes as well, so the solve is the very instantiation of the user half-epoch
                 loss = torch.zeros(2, dtype=torch.float64, device=tX.device)
@@ -124,6 +120,57 @@ class ALS(Algo, ALSOption, Evaluable, Serializable):
                 # before it solves); the holder keeps only its scratch, the resident Q is st.Q
                 h._keep = []
         return tX, (ind_t, keys_t, vals_t)
+
+    @staticmethod
+    def _bind_fold_items(st, h, X):
+        """Binds rows X and the state's resident Q to the fold-in holder h, with the Gram of this Q computed once."""
+        h.bind_factors(X, st.Q)
+        if st.derived_key != st.key:
+            st.derived_key = None
+            h.precompute_device(0)
+            st.derived_key = st.key
+
+    # ---- explanations (DESIGN.md 4.11) --------------------------------------------------------
+    EXPLAIN_DMAX, EXPLAIN_KMAX, EXPLAIN_TOPM_MAX = 256, 4096, 64
+
+    def explain(self, histories, items, topm=5):
+        """Why each target item scores what it does for each history row: Hu, Koren and Volinsky's section 5 split of
+        the score q_i . x_r into one term per history item j, (q_i' A_r^-1 q_j) * (1 + alpha v_j), where
+        A_r = Q'Q + alpha sum v_j q_j q_j' + reg_u kappa I and x_r = A_r^-1 sum (1 + alpha v_j) q_j is the exact
+        least-squares row of the user half-epoch (kappa = the row's entry count with adaptive_reg, else 1).  Entries of
+        one item are summed into one term.  x_r is the exact solve whatever the optimizer: it is fold_in(histories)'s
+        row for llt / ldlt at d < 128, while manual_cg and iALS++ (every d >= 128) only approach it, so P[u] . q_i
+        after train() is in general not this score.
+
+        histories: as fold_in takes them.  items: an (n, k) integer array of item indexes with -1 for no target (what
+        ParALS.topk_recommendation returns), or n lists of item ids (unknown ids become -1; rows padded with -1).
+        Returns (scores float32 [n, k], keys int32 [n, k, topm], contributions float32 [n, k, topm]): the topm items
+        with the largest contributions, descending, ties to the smaller item index; -1 / 0.0 pad.  A -1 target or an
+        empty history gives score 0.0 and keys -1; a row whose A_r meets a non-positive Cholesky pivot gets NaN scores
+        and keys -1.  On the GPU only: without one the backend's "no CPU fallback" error is raised."""
+        if self.opt._nrz_Q:
+            raise RuntimeError("Cannot explain scores with normalized item factors")
+        if isinstance(topm, bool) or not isinstance(topm, (int, np.integer)) or not 1 <= topm <= self.EXPLAIN_TOPM_MAX:
+            raise ValueError("topm must be an integer in [1, %d], got %r" % (self.EXPLAIN_TOPM_MAX, topm))
+        if self.opt.d > self.EXPLAIN_DMAX:
+            raise ValueError("explain supports d <= %d, got %d" % (self.EXPLAIN_DMAX, self.opt.d))
+        num_items = self.Q.shape[0]
+        indptr, keys, vals = fold_in.history_csr(self, histories, num_items)
+        targets = fold_in.target_matrix(self, items, len(indptr), num_items, self.EXPLAIN_KMAX)
+        st, h = fold_in.item_state(self, CuALS)
+        n, k = targets.shape
+        if n == 0 or k == 0:
+            return (np.zeros((n, k), np.float32), np.full((n, k, topm), -1, np.int32),
+                    np.zeros((n, k, topm), np.float32))
+        import torch
+        ind_t, keys_t, vals_t = fold_in.csr_to_device(indptr, keys, vals)
+        try:
+            # the explanation reads Q and its Gram only; the bound rows are a placeholder
+            self._bind_fold_items(st, h, torch.zeros((1, h.get_vdim()), dtype=torch.float32, device=ind_t.device))
+            out = h.explain_device(ind_t, keys_t, vals_t, torch.from_numpy(targets).to(ind_t.device), topm)
+        finally:
+            h._keep = []
+        return tuple(t.cpu().numpy() for t in out)
 
     # ---- training -----------------------------------------------------------------------------
     def _get_buffer(self):

@@ -1,4 +1,4 @@
-"""Folding-in (DESIGN.md 4.10): the host side that ALS.fold_in and PLSI.fold_in share.
+"""Folding-in (DESIGN.md 4.10): the host side that ALS.fold_in, PLSI.fold_in and ALS.explain (4.11) share.
 
 A fold-in computes user rows from their histories with the model's item factors held fixed.  This module turns the
 caller's histories and start rows into checked host arrays (before any device work), keeps the model's item factors on
@@ -40,6 +40,38 @@ def history_csr(algo, histories, num_items):
     lens = np.array([len(r) for r in rows], dtype=np.int64)
     keys = np.concatenate(rows).astype(np.int32) if rows else np.zeros(0, np.int32)
     return np.cumsum(lens).astype(np.int64), keys, np.ones(len(keys), dtype=np.float32)
+
+
+def target_matrix(algo, items, n, num_items, kmax):
+    """int32 (n, k) item indexes, -1 for no target, of explanation targets given as
+      * an (n, k) integer array of item indexes in [-1, num_items) (the shape ParALS.topk_recommendation returns),
+      * or n lists of item ids, mapped through the model's item-id map; unknown ids become -1 and the rows are padded
+        with -1 to the longest.
+    Raises ValueError on a wrong shape, an index out of range, k > kmax or another input type."""
+    if isinstance(items, np.ndarray):
+        if items.ndim != 2 or items.shape[0] != n or not np.issubdtype(items.dtype, np.integer):
+            raise ValueError("items must be an (%d, k) integer array, got %s %s" % (n, items.dtype, items.shape))
+        if items.size and (int(items.min()) < -1 or int(items.max()) >= num_items):
+            raise ValueError("items hold an index outside [-1, %d)" % num_items)
+        T = np.ascontiguousarray(items, dtype=np.int32)
+    elif isinstance(items, (list, tuple)):
+        if len(items) != n:
+            raise ValueError("items must hold one list per history row (%d), got %d" % (n, len(items)))
+        k = 0
+        for it in items:
+            if not isinstance(it, (list, tuple, np.ndarray)):
+                raise ValueError("every row of items must be a list of item ids, got %s" % type(it).__name__)
+            k = max(k, len(it))
+        T = np.full((n, k), -1, dtype=np.int32)
+        for r, it in enumerate(items):
+            idx = algo.get_index(list(it), group="item") if len(it) else []
+            T[r, :len(idx)] = [-1 if i is None else i for i in idx]
+    else:
+        raise ValueError("items must be an (n, k) integer array or a list of lists of item ids, got %s"
+                         % type(items).__name__)
+    if T.shape[1] > kmax:
+        raise ValueError("at most %d targets per row, got %d" % (kmax, T.shape[1]))
+    return T
 
 
 def start_rows(init, n, d, fill):
@@ -99,11 +131,16 @@ def begin(model, make, histories, init, fill):
     device arrays.  Returns (state, holder, (indptr, keys, vals, X) as to_device gives them)."""
     indptr, keys, vals = history_csr(model, histories, model.Q.shape[0])
     X0 = start_rows(init, len(indptr), model.opt.d, fill)
+    st, h = item_state(model, make)
+    return st, h, to_device(indptr, keys, vals, X0, h.get_vdim())
+
+
+def item_state(model, make):
+    """(the model's ItemState, its holder), refreshed for the model's current Q and options."""
     if getattr(model, "_fold_state", None) is None:
         model._fold_state = ItemState()
     st = model._fold_state
-    h = st.refresh(make, model.opt, model.Q)
-    return st, h, to_device(indptr, keys, vals, X0, h.get_vdim())
+    return st, st.refresh(make, model.opt, model.Q)
 
 
 def device():
@@ -115,10 +152,16 @@ def to_device(indptr, keys, vals, X0, vdim):
     """(indptr, keys, vals, X) torch CUDA tensors; keys / vals have at least one element, X is [n, vdim] with the start
     rows in its first d columns and zero padding."""
     import torch
+    X = torch.zeros((X0.shape[0], vdim), dtype=torch.float32, device=device())
+    X[:, :X0.shape[1]] = torch.from_numpy(np.ascontiguousarray(X0)).to(X.device)
+    return csr_to_device(indptr, keys, vals) + (X,)
+
+
+def csr_to_device(indptr, keys, vals):
+    """(indptr, keys, vals) torch CUDA tensors; keys / vals have at least one element."""
+    import torch
     dev = device()
     t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
     if not len(keys):
         keys, vals = np.zeros(1, np.int32), np.zeros(1, np.float32)
-    X = torch.zeros((X0.shape[0], vdim), dtype=torch.float32, device=dev)
-    X[:, :X0.shape[1]] = t(X0)
-    return t(indptr), t(keys), t(vals), X
+    return t(indptr), t(keys), t(vals)

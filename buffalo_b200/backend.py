@@ -165,6 +165,27 @@ class CuALS(_Holder):
         arr = (C.c_void_p * max(len(pointers), 1))(*[int(p) for p in pointers])
         _cabi.check(self._lib.bfl_als_set_peer_replicas(self._h, int(axis), len(pointers), arr), "set_peer_replicas")
 
+    def explain_device(self, indptr, keys, vals, targets, topm, stream=None):
+        """bfl_als_explain_device: (scores float32 [n, k], keys int32 [n, k, topm], contributions float32 [n, k, topm])
+        torch CUDA tensors explaining the exact row solve of each history row (indptr int64 [n] END offsets, keys int32
+        items in [0, Q_rows), ascending within a row, not checked here; vals float32) for the targets int32 [n, k], against
+        the bound Q and the Gram of precompute_device(0)."""
+        import torch
+        if targets.ndim != 2 or indptr.shape[0] != targets.shape[0]:
+            raise ValueError("targets must be [n, k] with one row per END offset (got %s for %d rows)"
+                             % (tuple(targets.shape), indptr.shape[0]))
+        n, k = targets.shape
+        dev = targets.device
+        scores = torch.empty((n, k), dtype=torch.float32, device=dev)
+        out_keys = torch.empty((n, k, int(topm)), dtype=torch.int32, device=dev)
+        contrib = torch.empty((n, k, int(topm)), dtype=torch.float32, device=dev)
+        if n:
+            _cabi.check(self._lib.bfl_als_explain_device(
+                self._h, _dev(indptr, "int64", "indptr"), _dev(keys, "int32", "keys"), _dev(vals, "float32", "vals"), n,
+                _dev(targets, "int32", "targets"), int(k), int(topm), scores.data_ptr(), out_keys.data_ptr(),
+                contrib.data_ptr(), _stream_ptr(stream)), "bfl_als_explain_device")
+        return scores, out_keys, contrib
+
     def gram_tensor(self):
         """View of the current d x d Gram matrix as a torch tensor (multi-GPU all-reduce, tests)."""
         ptr = self._lib.bfl_als_gram_device_mut(self._h)

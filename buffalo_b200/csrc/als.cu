@@ -3,6 +3,7 @@
 #include "als_fast.cuh"
 #include "als_generic.cuh"
 #include "bfl_common.cuh"
+#include "explain.cuh"
 
 using namespace bfl;
 
@@ -34,6 +35,7 @@ struct bfl_als : Holder {
     bool indptr_uploaded[2] = {false, false};   // own_indptr[axis] holds the caller's offsets (host-pointer path)
 
     DevBuf<float> G;          // d x d
+    int gram_axis = -1;       // axis whose full Gram G holds (the last precompute), -1 before one or after a partial one
     DevBuf<float> gram_part;  // partials of the two-stage Gram
     DevBuf<float> yui;        // generic ialspp scratch
     DevBuf<double> d_loss;    // 2 doubles
@@ -336,8 +338,10 @@ int bfl_als_precompute(bfl_als_t* h, int axis) {
     if (axis != 0 && axis != 1) BFL_FAIL(BFL_ERR_ARG, "axis must be 0 or 1");
     const float* F = axis == 0 ? h->dQ : h->dP;
     const int64_t rows = axis == 0 ? h->Q_rows : h->P_rows;
+    h->gram_axis = -1;
     int rc = gram(h, F, rows, h->stream);
     if (rc != BFL_OK) return rc;
+    h->gram_axis = axis;
     rc = note_factor_absmax(h, axis, h->stream);
     if (rc != BFL_OK) return rc;
     BFL_CUDA(cudaStreamSynchronize(h->stream));
@@ -452,8 +456,10 @@ int bfl_als_precompute_device(bfl_als_t* h, int axis, void* stream) {
     if (axis != 0 && axis != 1) BFL_FAIL(BFL_ERR_ARG, "axis must be 0 or 1");
     const float* F = axis == 0 ? h->dQ : h->dP;
     const int64_t rows = axis == 0 ? h->Q_rows : h->P_rows;
+    h->gram_axis = -1;
     int rc = gram(h, F, rows, (cudaStream_t)stream);
     if (rc != BFL_OK) return rc;
+    h->gram_axis = axis;
     return note_factor_absmax(h, axis, (cudaStream_t)stream);
 }
 
@@ -463,6 +469,7 @@ int bfl_als_precompute_rows_device(bfl_als_t* h, int axis, int64_t row_begin, in
     const float* F = axis == 0 ? h->dQ : h->dP;
     const int64_t rows = axis == 0 ? h->Q_rows : h->P_rows;
     if (row_begin < 0 || row_end > rows || row_end < row_begin) BFL_FAIL(BFL_ERR_ARG, "bad row range");
+    h->gram_axis = -1;
     // the operand scale needs max|Y| of the whole replica, not of the range (every rank gathers from all rows)
     int rc = note_factor_absmax(h, axis, (cudaStream_t)stream);
     if (rc != BFL_OK) return rc;
@@ -512,6 +519,38 @@ int bfl_als_set_peer_replicas(bfl_als_t* h, int axis, int n_peers, float* const*
     }
     h->n_peer[axis] = n_peers;
     return BFL_OK;
+}
+
+int bfl_als_explain_device(bfl_als_t* h, const int64_t* d_indptr, const int32_t* d_keys, const float* d_vals, int64_t n,
+                           const int32_t* d_targets, int k, int topm, float* d_scores, int32_t* d_out_keys,
+                           float* d_out_contrib, void* stream) {
+    if (!h || !h->factors_ready) BFL_FAIL(BFL_ERR_STATE, "factors not bound");
+    if (h->gram_axis != 0) BFL_FAIL(BFL_ERR_STATE, "explain needs the Gram of Q: bfl_als_precompute_device(axis 0) first");
+    if (h->d > EXPLAIN_DMAX) BFL_FAIL(BFL_ERR_ARG, "explain supports d <= " + std::to_string(EXPLAIN_DMAX));
+    if (k < 1 || k > EXPLAIN_KMAX) BFL_FAIL(BFL_ERR_ARG, "k must be in [1, " + std::to_string(EXPLAIN_KMAX) + "]");
+    if (topm < 1 || topm > EXPLAIN_TOPM_MAX) BFL_FAIL(BFL_ERR_ARG, "topm must be in [1, " + std::to_string(EXPLAIN_TOPM_MAX) + "]");
+    if (n < 0 || (n > 0 && (!d_indptr || !d_keys || !d_vals || !d_targets || !d_scores || !d_out_keys || !d_out_contrib)))
+        BFL_FAIL(BFL_ERR_ARG, "bad explain arguments");
+    ExplainArgs a;
+    a.G = h->G.p;
+    a.Q = h->dQ;
+    a.Q_rows = h->Q_rows;
+    a.D = h->d;
+    a.ld = h->vdim;
+    a.alpha = h->alpha;
+    a.reg = h->reg_u;
+    a.adaptive_reg = h->adaptive_reg;
+    a.indptr = d_indptr;
+    a.keys = d_keys;
+    a.vals = d_vals;
+    a.n = n;
+    a.targets = d_targets;
+    a.k = k;
+    a.topm = topm;
+    a.scores = d_scores;
+    a.out_keys = d_out_keys;
+    a.out_contrib = d_out_contrib;
+    return explain_launch(a, h->num_sms, (cudaStream_t)stream);
 }
 
 const float* bfl_als_gram_device(bfl_als_t* h) { return h ? h->G.p : nullptr; }

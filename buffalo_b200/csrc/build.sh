@@ -13,6 +13,7 @@ SRCS="$HERE/bfl_common.cu $HERE/als.cu"
 [ -f "$HERE/plsi.cu" ] && SRCS="$SRCS $HERE/plsi.cu"
 [ -f "$HERE/mm_ingest.cu" ] && SRCS="$SRCS $HERE/mm_ingest.cu"
 [ -f "$HERE/stream_ingest.cu" ] && SRCS="$SRCS $HERE/stream_ingest.cu"
+[ -f "$HERE/explain.cu" ] && SRCS="$SRCS $HERE/explain.cu"
 "$NVCC" -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 \
     -ccbin /usr/bin/g++ -Xcompiler -fPIC,-O3,-Wall -shared \
     ${BFL_PTXAS_V:+-Xptxas -v} -o "$OUT" $SRCS

@@ -215,6 +215,42 @@ class ParALS(Parallel):
             topks = [[self.algo._idmanager.itemids[t] for t in tt if t != -1] for tt in topks]
         return topks, scores
 
+    def explain(self, keys, items, topm=5, repr=False):
+        """(scores, keys, contributions) of algo.explain (DESIGN.md 4.11) for trained users: their histories are their
+        rows of the training data ("rowwise" group, keys and values).  keys: user ids (a list) or user indexes (an
+        array); every one must resolve.  items as algo.explain takes them, so the keys and topks that
+        topk_recommendation returns can be passed straight in.  repr=True returns the explaining items as item ids,
+        without the -1 padding.  Models with explain: ALS (a score is a sum of per-item terms only for least-squares
+        rows)."""
+        if not callable(getattr(self.algo, "explain", None)):
+            raise NotImplementedError("explain needs a least-squares model (ALS), not %s" % type(self.algo).__name__)
+        num_users = self.algo.P.shape[0]
+        if isinstance(keys, list):
+            idx = self.algo.get_index(keys, group="user") if keys else []
+            missing = [k for k, i in zip(keys, idx) if i is None]
+            if missing:
+                raise ValueError("unknown user keys: %s" % missing[:5])
+            idx = np.asarray(idx, dtype=np.int64)
+        else:
+            idx = np.asarray(keys)
+            if idx.ndim != 1 or (idx.size and not np.issubdtype(idx.dtype, np.integer)):
+                raise ValueError("keys must be a list of user ids or a 1-d array of user indexes")
+            if idx.size and (int(idx.min()) < 0 or int(idx.max()) >= num_users):
+                raise ValueError("user index outside [0, %d)" % num_users)
+        data = getattr(self.algo, "data", None)
+        if data is None:
+            raise ValueError("explain needs the training data attached to the model")
+        grp = data.get_group("rowwise")
+        ends = np.asarray(grp["indptr"][:], dtype=np.int64)
+        nnz = int(ends[-1]) if len(ends) else 0
+        rows = scipy.sparse.csr_matrix((np.asarray(grp["val"][:nnz], dtype=np.float32), np.asarray(grp["key"][:nnz]),
+                                        np.concatenate([[0], ends])), shape=(len(ends), self.algo.Q.shape[0]))
+        scores, out_keys, contrib = self.algo.explain(rows[idx.astype(np.int64)], items, topm)
+        if repr:
+            names = self.algo._idmanager.itemids
+            out_keys = [[[names[t] for t in tt if t != -1] for tt in row] for row in out_keys]
+        return scores, out_keys, contrib
+
 
 class ParBPRMF(ParALS):
     _bias = True

@@ -127,6 +127,23 @@ int bfl_als_update_device(bfl_als_t* h, int axis, int64_t row_begin, int64_t row
  * all-gather of the updated shard overlaps the solve row by row; the caller only needs a stream-ordered barrier
  * between half-epochs.  n_peers = 0 switches the fused exchange off.  At most 15 peers. */
 int bfl_als_set_peer_replicas(bfl_als_t* h, int axis, int n_peers, float* const* peer_ptrs);
+
+/* Explanations of the exact row solve (csrc/explain.cu, DESIGN.md 4.11).  For n history rows (DEVICE CSR: d_indptr
+ * int64 END offsets, d_keys int32 items in [0, Q_rows) ascending within a row (not checked), d_vals float32) and d_targets
+ * int32 [n, k] (item indexes; -1 for no target), with A_r = Q'Q + alpha sum v_j q_j q_j' + reg_u kappa I and
+ * b_r = sum (1 + alpha v_j) q_j (kappa = the row's entry count with adaptive_reg, else 1), writes
+ *   d_scores [n, k]            q_i' A_r^-1 b_r,
+ *   d_out_keys [n, k, topm]    the topm history items with the largest (q_i' A_r^-1 q_j)(1 + alpha v_j), entries of
+ *                              one item summed, descending, ties to the smaller item; -1 pads,
+ *   d_out_contrib [n, k, topm] those contributions; 0.0 pads.
+ * A -1 target or an empty row gives score 0.0 and keys -1.  A non-positive Cholesky pivot of A_r gives NaN scores and
+ * keys -1 for that row only.  Reads the bound Q, the Gram of the last bfl_als_precompute_device(axis 0) (else
+ * BFL_ERR_STATE), alpha, reg_u and adaptive_reg.  k in [1, 4096], topm in [1, 64], d <= 256, else BFL_ERR_ARG.  No
+ * atomics: a row's outputs do not depend on the other rows of the call. */
+int bfl_als_explain_device(bfl_als_t* h, const int64_t* d_indptr, const int32_t* d_keys, const float* d_vals, int64_t n,
+                           const int32_t* d_targets, int k, int topm, float* d_scores, int32_t* d_out_keys,
+                           float* d_out_contrib, void* stream);
+
 /* device pointer of the current Gram matrix [d x d] (tests) */
 const float* bfl_als_gram_device(bfl_als_t* h);
 /* multi-GPU: when several ranks each computed the Gram of their shard of Y, the host
