@@ -774,25 +774,31 @@ def csr_from_triples_host(major, minor, vals, num_major, num_minor, sort_minor=T
     return indptr, key[:n], val[:n]
 
 
-class MMIngest(object):
-    """Handle of the device MatrixMarket parser (csrc/mm_ingest.cu, bfl_mm_ingest_*): stream the text after the header
-    through two pinned staging buffers, then split and build both CSR orientations on the device."""
+class _TextIngest(object):
+    """Handle of a device text parser (bfl_<prefix>_*): the text is fed through two pinned staging buffers of
+    block_bytes, then the CSR groups are built on the device and copied out.  STAGES names the entries of stats()."""
 
-    STAGES = ("h2d", "parse", "patch", "split", "csr_rowwise", "csr_colwise", "d2h")
+    STAGES = ()
 
-    def __init__(self, num_rows, num_cols, nnz_hint, block_bytes, header_lines, slow_cap):
+    def __init__(self, prefix, block_bytes, *create_args):
         self._lib = _cabi.lib()
-        self._h = self._lib.bfl_mm_ingest_create(int(num_rows), int(num_cols), int(nnz_hint), int(block_bytes),
-                                                 int(header_lines), int(slow_cap))
+        self._prefix = prefix
+        self._h = self._fn("create")(*create_args)
         if not self._h:
-            raise _cabi.BackendError("bfl_mm_ingest_create failed: " +
-                                     self._lib.bfl_last_error().decode("utf-8", "replace"))
+            err = self._lib.bfl_last_error().decode("utf-8", "replace")
+            raise _cabi.BackendError("bfl_%s_create failed: %s" % (prefix, err))
         self.block_bytes = int(block_bytes)
+
+    def _fn(self, name):
+        return getattr(self._lib, "bfl_%s_%s" % (self._prefix, name))
+
+    def _call(self, name, *args):
+        _cabi.check(self._fn(name)(self._h, *args), "bfl_%s_%s" % (self._prefix, name))
 
     def close(self):
         h, self._h = getattr(self, "_h", None), None
         if h:
-            self._lib.bfl_mm_ingest_destroy(h)
+            self._fn("destroy")(h)
 
     __del__ = close
 
@@ -805,139 +811,103 @@ class MMIngest(object):
     def staging(self, slot):
         """uint8 view of pinned staging buffer `slot`, free for writing (its previous upload has finished)."""
         p = C.c_void_p()
-        _cabi.check(self._lib.bfl_mm_ingest_staging(self._h, int(slot), C.byref(p)), "bfl_mm_ingest_staging")
+        self._call("staging", int(slot), C.byref(p))
         return np.ctypeslib.as_array((C.c_uint8 * self.block_bytes).from_address(p.value))
 
     def feed(self, slot, n, is_last):
-        _cabi.check(self._lib.bfl_mm_ingest_feed(self._h, int(slot), int(n), int(bool(is_last))), "bfl_mm_ingest_feed")
+        self._call("feed", int(slot), int(n), int(bool(is_last)))
+
+    def build(self, orientation, num_major, nnz):
+        """-> (indptr int64[num_major] END offsets, key int32[nnz], val float32[nnz]); 0 = rowwise, 1 = colwise"""
+        indptr = np.empty(int(num_major), np.int64)
+        key, val = np.empty(max(nnz, 1), np.int32), np.empty(max(nnz, 1), np.float32)
+        self._call("build", int(orientation), indptr.ctypes.data, key.ctypes.data, val.ctypes.data)
+        return indptr, key[:nnz], val[:nnz]
+
+    def stats(self):
+        """-> ({stage: device ms}, peak device bytes of the default memory pool)"""
+        ms, peak = (C.c_double * len(self.STAGES))(), C.c_int64(0)
+        self._call("stats", ms, C.byref(peak))
+        return dict(zip(self.STAGES, list(ms))), peak.value
+
+
+class MMIngest(_TextIngest):
+    """Handle of the device MatrixMarket parser (csrc/mm_ingest.cu, bfl_mm_ingest_*): stream the text after the header
+    through two pinned staging buffers, then split and build both CSR orientations on the device."""
+
+    STAGES = ("h2d", "parse", "patch", "split", "csr_rowwise", "csr_colwise", "d2h")
+
+    def __init__(self, num_rows, num_cols, nnz_hint, block_bytes, header_lines, slow_cap):
+        super().__init__("mm_ingest", block_bytes, int(num_rows), int(num_cols), int(nnz_hint), int(block_bytes),
+                         int(header_lines), int(slow_cap))
 
     def finish(self):
         """-> dict(nnz, tokmask, reject_line, range_line, n_slow)"""
         v = [C.c_int64(0), C.c_int32(0), C.c_int64(0), C.c_int64(0), C.c_int64(0)]
-        _cabi.check(self._lib.bfl_mm_ingest_finish(self._h, *[C.byref(x) for x in v]), "bfl_mm_ingest_finish")
+        self._call("finish", *[C.byref(x) for x in v])
         return dict(zip(("nnz", "tokmask", "reject_line", "range_line", "n_slow"), [x.value for x in v]))
 
     def slow_tokens(self, n):
         """-> (ordinal int64, offset from the first fed byte int64, length int32) of n slow value tokens"""
         o, off, ln = np.empty(n, np.int64), np.empty(n, np.int64), np.empty(n, np.int32)
-        _cabi.check(self._lib.bfl_mm_ingest_slow_tokens(self._h, int(n), o.ctypes.data, off.ctypes.data, ln.ctypes.data),
-                    "bfl_mm_ingest_slow_tokens")
+        self._call("slow_tokens", int(n), o.ctypes.data, off.ctypes.data, ln.ctypes.data)
         return o, off, ln
 
     def patch_values(self, ordinal, vals):
         o = np.ascontiguousarray(ordinal, dtype=np.int64)
         v = np.ascontiguousarray(vals, dtype=np.float32)
-        _cabi.check(self._lib.bfl_mm_ingest_patch_values(self._h, o.ctypes.data, v.ctypes.data, len(o)),
-                    "bfl_mm_ingest_patch_values")
+        self._call("patch_values", o.ctypes.data, v.ctypes.data, len(o))
 
     def split(self, sample_idx):
         """-> (row int32, col int32, val float32) of the sampled data-line ordinals (strictly increasing)"""
         idx = np.ascontiguousarray(sample_idx, dtype=np.int64)
         n = len(idx)
         r, c, v = np.empty(n, np.int32), np.empty(n, np.int32), np.empty(n, np.float32)
-        _cabi.check(self._lib.bfl_mm_ingest_split(self._h, idx.ctypes.data, n, r.ctypes.data, c.ctypes.data,
-                                                  v.ctypes.data), "bfl_mm_ingest_split")
+        self._call("split", idx.ctypes.data, n, r.ctypes.data, c.ctypes.data, v.ctypes.data)
         return r, c, v
 
-    def build(self, orientation, num_major, nnz):
-        """-> (indptr int64[num_major] END offsets, key int32[nnz], val float32[nnz]); 0 = rowwise, 1 = colwise"""
-        indptr = np.empty(int(num_major), np.int64)
-        key, val = np.empty(max(nnz, 1), np.int32), np.empty(max(nnz, 1), np.float32)
-        _cabi.check(self._lib.bfl_mm_ingest_build(self._h, int(orientation), indptr.ctypes.data, key.ctypes.data,
-                                                  val.ctypes.data), "bfl_mm_ingest_build")
-        return indptr, key[:nnz], val[:nnz]
 
-    def stats(self):
-        """-> ({stage: device ms}, peak device bytes of the default memory pool)"""
-        ms, peak = (C.c_double * len(self.STAGES))(), C.c_int64(0)
-        _cabi.check(self._lib.bfl_mm_ingest_stats(self._h, ms, C.byref(peak)), "bfl_mm_ingest_stats")
-        return dict(zip(self.STAGES, list(ms))), peak.value
-
-
-class StreamIngest(object):
+class StreamIngest(_TextIngest):
     """Handle of the device Stream parser (csrc/stream_ingest.cu, bfl_stream_ingest_*): stream the text through two
     pinned staging buffers, intern the item tokens on the device, then split and build the CSR groups there."""
 
     STAGES = ("h2d", "parse", "intern", "number", "split", "csr_rowwise", "csr_colwise", "d2h")
 
     def __init__(self, block_bytes, whitespace, hash_bits=64):
-        self._lib = _cabi.lib()
         ascii_ws = sum(1 << c for c in whitespace if c < 64)
         usp = np.ascontiguousarray([c for c in whitespace if c >= 0x80], dtype=np.int32)
-        self._h = self._lib.bfl_stream_ingest_create(int(block_bytes), ascii_ws, usp.ctypes.data, len(usp), int(hash_bits))
-        if not self._h:
-            raise _cabi.BackendError("bfl_stream_ingest_create failed: " +
-                                     self._lib.bfl_last_error().decode("utf-8", "replace"))
-        self.block_bytes = int(block_bytes)
-
-    def close(self):
-        h, self._h = getattr(self, "_h", None), None
-        if h:
-            self._lib.bfl_stream_ingest_destroy(h)
-
-    __del__ = close
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.close()
-
-    def staging(self, slot):
-        p = C.c_void_p()
-        _cabi.check(self._lib.bfl_stream_ingest_staging(self._h, int(slot), C.byref(p)), "bfl_stream_ingest_staging")
-        return np.ctypeslib.as_array((C.c_uint8 * self.block_bytes).from_address(p.value))
+        super().__init__("stream_ingest", block_bytes, int(block_bytes), ascii_ws, usp.ctypes.data, len(usp),
+                         int(hash_bits))
 
     def load_iid(self, names):
         """names: list of bytes (UTF-8 item names, in id order)"""
         offs = np.zeros(len(names) + 1, np.int64)
         np.cumsum([len(x) for x in names], out=offs[1:])
         buf = np.frombuffer(b"".join(names) or b"\0", np.uint8)
-        _cabi.check(self._lib.bfl_stream_ingest_load_iid(self._h, buf.ctypes.data, offs.ctypes.data, len(names)),
-                    "bfl_stream_ingest_load_iid")
-
-    def feed(self, slot, n, is_last):
-        _cabi.check(self._lib.bfl_stream_ingest_feed(self._h, int(slot), int(n), int(bool(is_last))),
-                    "bfl_stream_ingest_feed")
+        self._call("load_iid", buf.ctypes.data, offs.ctypes.data, len(names))
 
     def finish(self):
         """-> dict(tokens, lines, items, decline, decline_line)"""
         v = [C.c_int64(0), C.c_int64(0), C.c_int32(0), C.c_int32(0), C.c_int64(0)]
-        _cabi.check(self._lib.bfl_stream_ingest_finish(self._h, *[C.byref(x) for x in v]), "bfl_stream_ingest_finish")
+        self._call("finish", *[C.byref(x) for x in v])
         return dict(zip(("tokens", "lines", "items", "decline", "decline_line"), [x.value for x in v]))
 
     def names(self, n):
         """-> (offset int64, length int32) of the first occurrence of each of the n items"""
         off, ln = np.empty(max(n, 1), np.int64), np.empty(max(n, 1), np.int32)
-        _cabi.check(self._lib.bfl_stream_ingest_names(self._h, off.ctypes.data, ln.ctypes.data), "bfl_stream_ingest_names")
+        self._call("names", off.ctypes.data, ln.ctypes.data)
         return off[:n], ln[:n]
 
     def split(self, num_users, method, newest_n, sample_idx, as_matrix):
         """method: 0 none, 1 newest, 2 sample -> (n_train, (row int32, col int32, val float32) of the vali triples)"""
         idx = np.ascontiguousarray(sample_idx, dtype=np.int64)
         nv, nt = C.c_int64(0), C.c_int64(0)
-        _cabi.check(self._lib.bfl_stream_ingest_split(self._h, int(num_users), int(method), int(newest_n), idx.ctypes.data,
-                                                      len(idx), int(bool(as_matrix)), C.byref(nv), C.byref(nt)),
-                    "bfl_stream_ingest_split")
+        self._call("split", int(num_users), int(method), int(newest_n), idx.ctypes.data, len(idx), int(bool(as_matrix)),
+                   C.byref(nv), C.byref(nt))
         n = nv.value
         r, c, v = np.empty(max(n, 1), np.int32), np.empty(max(n, 1), np.int32), np.empty(max(n, 1), np.float32)
-        _cabi.check(self._lib.bfl_stream_ingest_vali(self._h, r.ctypes.data, c.ctypes.data, v.ctypes.data),
-                    "bfl_stream_ingest_vali")
+        self._call("vali", r.ctypes.data, c.ctypes.data, v.ctypes.data)
         return nt.value, (r[:n], c[:n], v[:n])
-
-    def build(self, orientation, num_major, nnz):
-        """-> (indptr int64[num_major] END offsets, key int32[nnz], val float32[nnz]); 0 = rowwise, 1 = colwise"""
-        indptr = np.empty(int(num_major), np.int64)
-        key, val = np.empty(max(nnz, 1), np.int32), np.empty(max(nnz, 1), np.float32)
-        _cabi.check(self._lib.bfl_stream_ingest_build(self._h, int(orientation), indptr.ctypes.data, key.ctypes.data,
-                                                      val.ctypes.data), "bfl_stream_ingest_build")
-        return indptr, key[:nnz], val[:nnz]
-
-    def stats(self):
-        """-> ({stage: device ms}, peak device bytes of the default memory pool)"""
-        ms, peak = (C.c_double * len(self.STAGES))(), C.c_int64(0)
-        _cabi.check(self._lib.bfl_stream_ingest_stats(self._h, ms, C.byref(peak)), "bfl_stream_ingest_stats")
-        return dict(zip(self.STAGES, list(ms))), peak.value
 
 
 def device_free_bytes():

@@ -5,6 +5,8 @@
 //     Replaces the text -> temp files -> parallel sort pipeline's sort/compress stage (fileio.hpp:263-419, mm.py:236-279).
 //   * cumulative popularity table of BPRMF.prepare_sampling (buffalo/algo/bpr.py:99-111): histogram of the item keys,
 //     integer power, inclusive scan.
+//   * the core the two device text parsers share (text_ingest.cuh): handle setup, staging, the stage clock and the
+//     CSR build into host arrays.
 // Sort pass = per-warp digit histograms over contiguous sub-tiles, one exclusive scan of the digit-major counter
 // matrix, and a stable scatter in which every warp walks its sub-tile in order and ranks equal digits with
 // __match_any_sync -- no atomics on the data path, so the result is deterministic.
@@ -12,6 +14,7 @@
 #include <vector>
 
 #include "bfl_common.cuh"
+#include "text_ingest.cuh"
 
 using namespace bfl;
 
@@ -190,29 +193,17 @@ int bits_for(long long v) {
 extern "C" {
 
 // Cumulative popularity table on the device: cum[i] = sum_{j <= i} count(j)^power (int64), bpr.py:99-111.
-// grid cap of the grid-stride helper kernels: 16 CTAs of 256 threads per SM of the current device
-static int ingest_grid_cap() {
-    int dev = 0, sms = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
-        sms <= 0)
-        sms = 1;
-    return sms * 16;
-}
-
 int bfl_popularity_table_device(const int32_t* d_keys, int64_t nnz, int32_t n_items, int power, int64_t* d_cum, void* stream) {
     if (BFL_OK != require_device()) return BFL_ERR_CUDA;
-    const int cap = ingest_grid_cap();
     if (!d_cum || n_items <= 0 || nnz < 0 || (nnz > 0 && !d_keys) || power < 0) BFL_FAIL(BFL_ERR_ARG, "bad popularity-table arguments");
     cudaStream_t st = (cudaStream_t)stream;
     BFL_CUDA(cudaMemsetAsync(d_cum, 0, sizeof(int64_t) * n_items, st));
     if (nnz > 0) {
-        hist_i32_kernel<<<(unsigned)std::min<int64_t>((nnz + 255) / 256, cap), 256, 0, st>>>(
-            d_keys, nnz, reinterpret_cast<long long*>(d_cum), n_items);
+        hist_i32_kernel<<<grid_for(nnz), 256, 0, st>>>(d_keys, nnz, reinterpret_cast<long long*>(d_cum), n_items);
         BFL_LAUNCHED();
     }
     if (power != 1) {
-        ipow_kernel<<<(unsigned)std::min<int64_t>((n_items + 255) / 256, cap), 256, 0, st>>>(
-            reinterpret_cast<long long*>(d_cum), n_items, power);
+        ipow_kernel<<<grid_for(n_items), 256, 0, st>>>(reinterpret_cast<long long*>(d_cum), n_items, power);
         BFL_LAUNCHED();
     }
     return inclusive_scan_i64(reinterpret_cast<long long*>(d_cum), reinterpret_cast<long long*>(d_cum), n_items, st);
@@ -245,7 +236,7 @@ int bfl_csr_from_triples_device(const int32_t* d_major, const int32_t* d_minor, 
     // indptr: histogram of the major index + inclusive scan
     BFL_CUDA(cudaMemsetAsync(d_indptr, 0, sizeof(int64_t) * num_major, st));
     if (nnz == 0) return BFL_OK;
-    const unsigned g = (unsigned)std::min<int64_t>((nnz + 255) / 256, ingest_grid_cap());
+    const int g = grid_for(nnz);
     hist_i32_kernel<<<g, 256, 0, st>>>(d_major, nnz, reinterpret_cast<long long*>(d_indptr), num_major);
     BFL_LAUNCHED();
     int rc = inclusive_scan_i64(reinterpret_cast<long long*>(d_indptr), reinterpret_cast<long long*>(d_indptr), num_major, st);
@@ -318,3 +309,114 @@ int bfl_csr_from_triples_host(const int32_t* major, const int32_t* minor, const 
 }
 
 }  // extern "C"
+
+// ---- core of the device text parsers (text_ingest.cuh) ------------------------------------------
+namespace bfl {
+
+int grid_for(long long n) {
+    int dev = 0, sms = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+        sms <= 0)
+        sms = 1;
+    return (int)std::max<long long>(1, std::min<long long>((n + 255) / 256, (long long)sms * 16));
+}
+
+TextIngest::~TextIngest() {
+    if (comp) cudaStreamSynchronize(comp);
+    for (int i = 0; i < 2; ++i) {
+        if (host[i]) cudaFreeHost(host[i]);
+        if (copied[i]) cudaEventDestroy(copied[i]);
+    }
+    for (auto& v : marks)
+        for (cudaEvent_t e : v) cudaEventDestroy(e);
+    if (comp) cudaStreamDestroy(comp);
+}
+
+bool setup(TextIngest* h, long long block_bytes, int stages) {
+    h->block_bytes = block_bytes;
+    h->marks.resize((size_t)stages);
+    int dev = 0;
+    uint64_t zero = 0;
+    bool ok = cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetDefaultMemPool(&h->mem_pool, dev) == cudaSuccess &&
+              cudaMemPoolSetAttribute(h->mem_pool, cudaMemPoolAttrUsedMemHigh, &zero) == cudaSuccess &&
+              cudaStreamCreateWithFlags(&h->comp, cudaStreamNonBlocking) == cudaSuccess;
+    for (int i = 0; ok && i < 2; ++i)
+        ok = cudaHostAlloc(&h->host[i], (size_t)block_bytes, cudaHostAllocDefault) == cudaSuccess &&
+             cudaEventCreateWithFlags(&h->copied[i], cudaEventDisableTiming) == cudaSuccess;
+    return ok;
+}
+
+int mark(TextIngest* h, int stage, cudaStream_t st) {
+    cudaEvent_t e;
+    BFL_CUDA(cudaEventCreate(&e));
+    h->marks[stage].push_back(e);
+    BFL_CUDA(cudaEventRecord(e, st));
+    return BFL_OK;
+}
+
+int staging(TextIngest* h, int slot, void** host_ptr) {
+    if (!h || slot < 0 || slot > 1 || !host_ptr) BFL_FAIL(BFL_ERR_ARG, "bad staging arguments");
+    if (h->copy_pending[slot]) BFL_CUDA(cudaEventSynchronize(h->copied[slot]));
+    h->copy_pending[slot] = false;
+    *host_ptr = h->host[slot];
+    return BFL_OK;
+}
+
+int check_feed(TextIngest* h, int slot, long long n, int is_last) {
+    if (!h || slot < 0 || slot > 1 || n < 0 || n > h->block_bytes) BFL_FAIL(BFL_ERR_ARG, "bad feed arguments");
+    if (h->last_fed) BFL_FAIL(BFL_ERR_STATE, "feed after the last block");
+    if (!is_last && (n == 0 || h->host[slot][n - 1] != '\n')) BFL_FAIL(BFL_ERR_ARG, "a block that is not the last must end with '\\n'");
+    h->last_fed = is_last != 0;
+    return BFL_OK;
+}
+
+int build_to_host(TextIngest* h, int orientation, const int32_t* row, const int32_t* col, const float* val, long long nnz,
+                  int32_t num_rows, int32_t num_cols, int sort_minor, int csr_stage, int d2h_stage, int64_t* indptr,
+                  int32_t* key, float* out_val) {
+    const int32_t nmaj = orientation ? num_cols : num_rows, nmin = orientation ? num_rows : num_cols;
+    int64_t* d_ind = nullptr;
+    int32_t* d_key = nullptr;
+    float* d_val = nullptr;
+    const size_t m = (size_t)std::max<long long>(nnz, 1);
+    BFL_CUDA(cudaMallocAsync(&d_ind, sizeof(int64_t) * nmaj, h->comp));
+    BFL_CUDA(cudaMallocAsync(&d_key, sizeof(int32_t) * m, h->comp));
+    BFL_CUDA(cudaMallocAsync(&d_val, sizeof(float) * m, h->comp));
+    if (int rc = mark(h, csr_stage, h->comp)) return rc;
+    int rc = bfl_csr_from_triples_device(orientation ? col : row, orientation ? row : col, val, nnz, nmaj, std::max(nmin, 1),
+                                         sort_minor, d_ind, d_key, d_val, h->comp);
+    if (rc != BFL_OK) return rc;
+    if ((rc = mark(h, csr_stage, h->comp))) return rc;
+    h->built[orientation] = true;
+    if ((rc = mark(h, d2h_stage, h->comp))) return rc;
+    BFL_CUDA(cudaMemcpyAsync(indptr, d_ind, sizeof(int64_t) * nmaj, cudaMemcpyDeviceToHost, h->comp));
+    if (nnz) {
+        BFL_CUDA(cudaMemcpyAsync(key, d_key, sizeof(int32_t) * nnz, cudaMemcpyDeviceToHost, h->comp));
+        BFL_CUDA(cudaMemcpyAsync(out_val, d_val, sizeof(float) * nnz, cudaMemcpyDeviceToHost, h->comp));
+    }
+    if ((rc = mark(h, d2h_stage, h->comp))) return rc;
+    BFL_CUDA(cudaFreeAsync(d_ind, h->comp));
+    BFL_CUDA(cudaFreeAsync(d_key, h->comp));
+    BFL_CUDA(cudaFreeAsync(d_val, h->comp));
+    BFL_CUDA(cudaStreamSynchronize(h->comp));
+    return BFL_OK;
+}
+
+int stats(TextIngest* h, double* stage_ms, int64_t* peak_bytes) {
+    if (!h || !stage_ms || !peak_bytes) BFL_FAIL(BFL_ERR_ARG, "bad stats arguments");
+    BFL_CUDA(cudaStreamSynchronize(h->comp));
+    for (size_t s = 0; s < h->marks.size(); ++s) {
+        double tot = 0.0;
+        for (size_t i = 0; i + 1 < h->marks[s].size(); i += 2) {
+            float ms = 0.f;
+            BFL_CUDA(cudaEventElapsedTime(&ms, h->marks[s][i], h->marks[s][i + 1]));
+            tot += ms;
+        }
+        stage_ms[s] = tot;
+    }
+    uint64_t hi = 0;
+    BFL_CUDA(cudaMemPoolGetAttribute(h->mem_pool, cudaMemPoolAttrUsedMemHigh, &hi));
+    *peak_bytes = (int64_t)hi;
+    return BFL_OK;
+}
+
+}  // namespace bfl

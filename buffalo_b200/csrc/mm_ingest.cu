@@ -17,6 +17,7 @@
 #include <vector>
 
 #include "bfl_common.cuh"
+#include "text_ingest.cuh"
 
 using namespace bfl;
 
@@ -326,46 +327,39 @@ __global__ void mm_compact_kernel(const long long* __restrict__ idx, long long n
     }
 }
 
-int grid_for(long long n) {
-    int dev = 0, sms = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
-        sms <= 0)
-        sms = 1;
-    return (int)std::max<long long>(1, std::min<long long>((n + 255) / 256, (long long)sms * 16));
-}
-
 enum { ST_H2D = 0, ST_PARSE, ST_PATCH, ST_SPLIT, ST_CSR_ROW, ST_CSR_COL, ST_D2H, ST_COUNT };
 
 }  // namespace
 
-struct bfl_mm_ingest {
+struct bfl_mm_ingest : TextIngest {
     int32_t num_rows = 0, num_cols = 0;
-    long long cap = 0, block_bytes = 0, buf_bytes = 0, header_lines = 0, slow_cap = 0;
-    cudaStream_t copy = nullptr, comp = nullptr;
-    unsigned char* host[2] = {nullptr, nullptr};           // pinned staging buffers
+    long long cap = 0, buf_bytes = 0, header_lines = 0, slow_cap = 0;
+    cudaStream_t copy = nullptr;                           // uploads of the staging buffers
     unsigned char* dev[2] = {nullptr, nullptr};            // device text buffers (16-byte front pad)
-    cudaEvent_t copied[2] = {nullptr, nullptr}, parsed[2] = {nullptr, nullptr};
-    bool copy_pending[2] = {false, false}, parse_pending[2] = {false, false};
-    long long fed = 0, nnz = -1;
-    bool last_fed = false, split_done = false, built[2] = {false, false};
+    cudaEvent_t parsed[2] = {nullptr, nullptr};
+    bool parse_pending[2] = {false, false};
+    long long nnz = -1;
+    bool split_done = false;
     MMState* state = nullptr;
     long long* counts = nullptr;
     int32_t *row = nullptr, *col = nullptr;
     float* val = nullptr;
     long long *slow_ord = nullptr, *slow_pos = nullptr;
-    std::vector<cudaEvent_t> marks[ST_COUNT];              // (begin, end) pairs per stage
-    cudaMemPool_t pool = nullptr;
+
+    ~bfl_mm_ingest() override {
+        if (comp) cudaStreamSynchronize(comp);
+        if (copy) cudaStreamSynchronize(copy);
+        for (int i = 0; i < 2; ++i) {
+            if (dev[i]) cudaFree(dev[i]);
+            if (parsed[i]) cudaEventDestroy(parsed[i]);
+        }
+        for (void* p : {(void*)state, (void*)counts, (void*)row, (void*)col, (void*)val, (void*)slow_ord, (void*)slow_pos})
+            if (p) cudaFree(p);
+        if (copy) cudaStreamDestroy(copy);
+    }
 };
 
 namespace {
-
-int mark(bfl_mm_ingest* h, int stage, cudaStream_t st) {
-    cudaEvent_t e;
-    BFL_CUDA(cudaEventCreate(&e));
-    h->marks[stage].push_back(e);
-    BFL_CUDA(cudaEventRecord(e, st));
-    return BFL_OK;
-}
 
 void free_triples(bfl_mm_ingest* h) {
     if (h->row) cudaFreeAsync(h->row, h->comp);
@@ -391,24 +385,14 @@ bfl_mm_ingest_t* bfl_mm_ingest_create(int32_t num_rows, int32_t num_cols, int64_
     h->num_rows = num_rows;
     h->num_cols = num_cols;
     h->cap = nnz_hint;
-    h->block_bytes = block_bytes;
     h->header_lines = header_lines;
     h->slow_cap = std::max<int64_t>(slow_cap, 1);
     // the last tile of a block stages MM_SMEM bytes from 16 before its start
     h->buf_bytes = (block_bytes + MM_TILE - 1) / MM_TILE * MM_TILE + MM_SMEM;
-    int dev = 0;
-    bool ok = cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetDefaultMemPool(&h->pool, dev) == cudaSuccess;
-    if (ok) {
-        uint64_t zero = 0;
-        ok = cudaMemPoolSetAttribute(h->pool, cudaMemPoolAttrUsedMemHigh, &zero) == cudaSuccess &&
-             cudaStreamCreateWithFlags(&h->copy, cudaStreamNonBlocking) == cudaSuccess &&
-             cudaStreamCreateWithFlags(&h->comp, cudaStreamNonBlocking) == cudaSuccess;
-    }
+    bool ok = setup(h, block_bytes, ST_COUNT) && cudaStreamCreateWithFlags(&h->copy, cudaStreamNonBlocking) == cudaSuccess;
     for (int i = 0; ok && i < 2; ++i)
-        ok = cudaHostAlloc(&h->host[i], (size_t)block_bytes, cudaHostAllocDefault) == cudaSuccess &&
-             cudaMallocAsync(&h->dev[i], (size_t)h->buf_bytes, h->comp) == cudaSuccess &&
+        ok = cudaMallocAsync(&h->dev[i], (size_t)h->buf_bytes, h->comp) == cudaSuccess &&
              cudaMemsetAsync(h->dev[i], 0, (size_t)h->buf_bytes, h->comp) == cudaSuccess &&
-             cudaEventCreateWithFlags(&h->copied[i], cudaEventDisableTiming) == cudaSuccess &&
              cudaEventCreateWithFlags(&h->parsed[i], cudaEventDisableTiming) == cudaSuccess;
     const long long tiles = (block_bytes + MM_TILE - 1) / MM_TILE;
     ok = ok && cudaMallocAsync(&h->state, sizeof(MMState), h->comp) == cudaSuccess &&
@@ -423,47 +407,15 @@ bfl_mm_ingest_t* bfl_mm_ingest_create(int32_t num_rows, int32_t num_cols, int64_
         ok = cudaMemcpyAsync(h->state, &s0, sizeof(s0), cudaMemcpyHostToDevice, h->comp) == cudaSuccess &&
              cudaStreamSynchronize(h->comp) == cudaSuccess;
     }
-    if (!ok) {
-        set_error(std::string("MatrixMarket ingest setup failed: ") + cudaGetErrorString(cudaGetLastError()));
-        bfl_mm_ingest_destroy(h);
-        return nullptr;
-    }
-    return h;
+    return setup_done(h, ok, "MatrixMarket");
 }
 
-void bfl_mm_ingest_destroy(bfl_mm_ingest_t* h) {
-    if (!h) return;
-    if (h->comp) cudaStreamSynchronize(h->comp);
-    if (h->copy) cudaStreamSynchronize(h->copy);
-    for (int i = 0; i < 2; ++i) {
-        if (h->host[i]) cudaFreeHost(h->host[i]);
-        if (h->dev[i]) cudaFree(h->dev[i]);
-        if (h->copied[i]) cudaEventDestroy(h->copied[i]);
-        if (h->parsed[i]) cudaEventDestroy(h->parsed[i]);
-    }
-    for (void* p : {(void*)h->state, (void*)h->counts, (void*)h->row, (void*)h->col, (void*)h->val, (void*)h->slow_ord,
-                    (void*)h->slow_pos})
-        if (p) cudaFree(p);
-    for (auto& v : h->marks)
-        for (cudaEvent_t e : v) cudaEventDestroy(e);
-    if (h->copy) cudaStreamDestroy(h->copy);
-    if (h->comp) cudaStreamDestroy(h->comp);
-    delete h;
-}
+void bfl_mm_ingest_destroy(bfl_mm_ingest_t* h) { delete h; }
 
-int bfl_mm_ingest_staging(bfl_mm_ingest_t* h, int slot, void** host_ptr) {
-    if (!h || slot < 0 || slot > 1 || !host_ptr) BFL_FAIL(BFL_ERR_ARG, "bad staging arguments");
-    if (h->copy_pending[slot]) BFL_CUDA(cudaEventSynchronize(h->copied[slot]));
-    h->copy_pending[slot] = false;
-    *host_ptr = h->host[slot];
-    return BFL_OK;
-}
+int bfl_mm_ingest_staging(bfl_mm_ingest_t* h, int slot, void** host_ptr) { return staging(h, slot, host_ptr); }
 
 int bfl_mm_ingest_feed(bfl_mm_ingest_t* h, int slot, int64_t n, int is_last) {
-    if (!h || slot < 0 || slot > 1 || n < 0 || n > h->block_bytes) BFL_FAIL(BFL_ERR_ARG, "bad feed arguments");
-    if (h->last_fed) BFL_FAIL(BFL_ERR_STATE, "feed after the last block");
-    if (!is_last && (n == 0 || h->host[slot][n - 1] != '\n')) BFL_FAIL(BFL_ERR_ARG, "a block that is not the last must end with '\\n'");
-    h->last_fed = is_last != 0;
+    if (int rc = check_feed(h, slot, n, is_last)) return rc;
     if (n == 0) return BFL_OK;
     unsigned char* d = h->dev[slot] + 16;
     // the device buffer is free once the parse that last read it has finished
@@ -611,56 +563,18 @@ int bfl_mm_ingest_build(bfl_mm_ingest_t* h, int orientation, int64_t* indptr, in
     if (!h || !h->split_done || orientation < 0 || orientation > 1 || h->built[orientation] || !indptr ||
         (h->nnz && (!key || !val)))
         BFL_FAIL(BFL_ERR_ARG, "bad build arguments (split first, each orientation once)");
-    const int32_t nmaj = orientation ? h->num_cols : h->num_rows, nmin = orientation ? h->num_rows : h->num_cols;
-    const long long nnz = h->nnz;
-    int64_t* d_ind = nullptr;
-    int32_t* d_key = nullptr;
-    float* d_val = nullptr;
-    const size_t m = (size_t)std::max<long long>(nnz, 1);
-    BFL_CUDA(cudaMallocAsync(&d_ind, sizeof(int64_t) * nmaj, h->comp));
-    BFL_CUDA(cudaMallocAsync(&d_key, sizeof(int32_t) * m, h->comp));
-    BFL_CUDA(cudaMallocAsync(&d_val, sizeof(float) * m, h->comp));
-    const int st = orientation ? ST_CSR_COL : ST_CSR_ROW;
-    if (int rc = mark(h, st, h->comp)) return rc;
-    int rc = bfl_csr_from_triples_device(orientation ? h->col : h->row, orientation ? h->row : h->col, h->val, nnz, nmaj, nmin,
-                                         1, d_ind, d_key, d_val, h->comp);
-    if (rc != BFL_OK) return rc;
-    if ((rc = mark(h, st, h->comp))) return rc;
-    h->built[orientation] = true;
+    if (int rc = build_to_host(h, orientation, h->row, h->col, h->val, h->nnz, h->num_rows, h->num_cols, 1,
+                               orientation ? ST_CSR_COL : ST_CSR_ROW, ST_D2H, indptr, key, val))
+        return rc;
     if (h->built[0] && h->built[1]) free_triples(h);       // the sort's inputs are not needed any more
-    if ((rc = mark(h, ST_D2H, h->comp))) return rc;
-    BFL_CUDA(cudaMemcpyAsync(indptr, d_ind, sizeof(int64_t) * nmaj, cudaMemcpyDeviceToHost, h->comp));
-    if (nnz) {
-        BFL_CUDA(cudaMemcpyAsync(key, d_key, sizeof(int32_t) * nnz, cudaMemcpyDeviceToHost, h->comp));
-        BFL_CUDA(cudaMemcpyAsync(val, d_val, sizeof(float) * nnz, cudaMemcpyDeviceToHost, h->comp));
-    }
-    if ((rc = mark(h, ST_D2H, h->comp))) return rc;
-    BFL_CUDA(cudaFreeAsync(d_ind, h->comp));
-    BFL_CUDA(cudaFreeAsync(d_key, h->comp));
-    BFL_CUDA(cudaFreeAsync(d_val, h->comp));
-    BFL_CUDA(cudaStreamSynchronize(h->comp));
     return BFL_OK;
 }
 
 // stage_ms[7]: H2D, parse, patch, split, rowwise CSR, colwise CSR, D2H (summed device time of each stage);
 // *peak_bytes: high-water mark of the device's default memory pool since create
 int bfl_mm_ingest_stats(bfl_mm_ingest_t* h, double* stage_ms, int64_t* peak_bytes) {
-    if (!h || !stage_ms || !peak_bytes) BFL_FAIL(BFL_ERR_ARG, "bad stats arguments");
-    BFL_CUDA(cudaStreamSynchronize(h->copy));
-    BFL_CUDA(cudaStreamSynchronize(h->comp));
-    for (int s = 0; s < ST_COUNT; ++s) {
-        double tot = 0.0;
-        for (size_t i = 0; i + 1 < h->marks[s].size(); i += 2) {
-            float ms = 0.f;
-            BFL_CUDA(cudaEventElapsedTime(&ms, h->marks[s][i], h->marks[s][i + 1]));
-            tot += ms;
-        }
-        stage_ms[s] = tot;
-    }
-    uint64_t hi = 0;
-    BFL_CUDA(cudaMemPoolGetAttribute(h->pool, cudaMemPoolAttrUsedMemHigh, &hi));
-    *peak_bytes = (int64_t)hi;
-    return BFL_OK;
+    if (h) BFL_CUDA(cudaStreamSynchronize(h->copy));
+    return stats(h, stage_ms, peak_bytes);
 }
 
 }  // extern "C"

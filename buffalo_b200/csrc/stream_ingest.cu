@@ -21,6 +21,7 @@
 #include <vector>
 
 #include "bfl_common.cuh"
+#include "text_ingest.cuh"
 
 using namespace bfl;
 
@@ -509,24 +510,14 @@ __global__ void remap_kernel(int32_t* __restrict__ item, long long n, const int3
         item[i] = e_item[item[i]];
 }
 
-int grid_for(long long n) {
-    int dev = 0, sms = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
-        sms <= 0)
-        sms = 1;
-    return (int)std::max<long long>(1, std::min<long long>((n + 255) / 256, (long long)sms * 16));
-}
-
 enum { ST_H2D = 0, ST_PARSE, ST_INTERN, ST_NUMBER, ST_SPLIT, ST_CSR_ROW, ST_CSR_COL, ST_D2H, ST_COUNT };
 
 }  // namespace
 
-struct bfl_stream_ingest {
-    long long block_bytes = 0, buf_bytes = 0, tmp_cap = 0;
+struct bfl_stream_ingest : TextIngest {
+    long long buf_bytes = 0, tmp_cap = 0;
     int hash_bits = 64;
     Grammar g{};
-    cudaStream_t comp = nullptr;
-    unsigned char* host[2] = {nullptr, nullptr};           // pinned staging buffers
     unsigned char* dev = nullptr;                          // device text buffer (16-byte front pad)
     STState* state = nullptr;
     long long* counts = nullptr;
@@ -535,7 +526,7 @@ struct bfl_stream_ingest {
     int32_t *blen = nullptr, *slot_of = nullptr;
     unsigned long long* bhash = nullptr;
     // per token (ordinal)
-    long long tok_cap = 0, tokens = 0, lines = 0, fed = 0;
+    long long tok_cap = 0, tokens = 0, lines = 0;
     bool open_line = false;                                // the input does not end with '\n'
     int32_t *user = nullptr, *item = nullptr;
     unsigned char* flag = nullptr;                         // first occurrence, then held for validation
@@ -547,7 +538,7 @@ struct bfl_stream_ingest {
     long long iid_count = -1;                              // >= 0: frozen table of that many names
     unsigned decline = 0;
     long long decline_line = -1;
-    bool last_fed = false, finished = false, split_done = false, built[2] = {false, false}, as_matrix = false;
+    bool finished = false, split_done = false, as_matrix = false;
     int32_t num_items = 0, num_users = 0;
     std::vector<long long> name_off;
     std::vector<int32_t> name_len;
@@ -555,19 +546,18 @@ struct bfl_stream_ingest {
     long long n_vali = 0, n_train = 0;
     int32_t *vr = nullptr, *vc = nullptr, *tu = nullptr, *ti = nullptr;
     float *vv = nullptr, *tv = nullptr;
-    std::vector<cudaEvent_t> marks[ST_COUNT];
-    cudaMemPool_t mpool = nullptr;
+
+    ~bfl_stream_ingest() override {
+        if (comp) cudaStreamSynchronize(comp);
+        for (void* p : {(void*)dev, (void*)state, (void*)counts, (void*)boff, (void*)blen, (void*)slot_of, (void*)bhash,
+                        (void*)user, (void*)item, (void*)flag, (void*)t.key, (void*)t.first, (void*)t.entry, (void*)E.off,
+                        (void*)E.first, (void*)E.foff, (void*)E.len, (void*)pool, (void*)vr, (void*)vc, (void*)vv, (void*)tu,
+                        (void*)ti, (void*)tv})
+            if (p) cudaFree(p);
+    }
 };
 
 namespace {
-
-int mark(bfl_stream_ingest* h, int stage) {
-    cudaEvent_t e;
-    BFL_CUDA(cudaEventCreate(&e));
-    h->marks[stage].push_back(e);
-    BFL_CUDA(cudaEventRecord(e, h->comp));
-    return BFL_OK;
-}
 
 template <class T>
 void dfree(bfl_stream_ingest* h, T*& p) {
@@ -708,59 +698,28 @@ bfl_stream_ingest_t* bfl_stream_ingest_create(int64_t block_bytes, uint64_t asci
         return nullptr;
     }
     auto* h = new bfl_stream_ingest();
-    h->block_bytes = block_bytes;
     h->hash_bits = hash_bits;
     h->g.ascii_ws = ascii_ws;
     h->g.n_uspace = n_uspace;
     for (int i = 0; i < n_uspace; ++i) h->g.uspace[i] = uspace[i];
     h->buf_bytes = (block_bytes + ST_TILE - 1) / ST_TILE * ST_TILE + 16;
-    int dev = 0;
-    bool ok = cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetDefaultMemPool(&h->mpool, dev) == cudaSuccess;
-    if (ok) {
-        uint64_t zero = 0;
-        ok = cudaMemPoolSetAttribute(h->mpool, cudaMemPoolAttrUsedMemHigh, &zero) == cudaSuccess &&
-             cudaStreamCreateWithFlags(&h->comp, cudaStreamNonBlocking) == cudaSuccess;
-    }
-    for (int i = 0; ok && i < 2; ++i) ok = cudaHostAlloc(&h->host[i], (size_t)block_bytes, cudaHostAllocDefault) == cudaSuccess;
     const long long tiles = (block_bytes + ST_TILE - 1) / ST_TILE;
-    ok = ok && cudaMallocAsync(&h->dev, (size_t)h->buf_bytes, h->comp) == cudaSuccess &&
-         cudaMemsetAsync(h->dev, 0, (size_t)h->buf_bytes, h->comp) == cudaSuccess &&
-         cudaMallocAsync(&h->state, sizeof(STState), h->comp) == cudaSuccess &&
-         cudaMallocAsync(&h->counts, sizeof(long long) * tiles, h->comp) == cudaSuccess && alloc_table(h, &h->t, 1 << 16) == BFL_OK;
+    bool ok = setup(h, block_bytes, ST_COUNT) && cudaMallocAsync(&h->dev, (size_t)h->buf_bytes, h->comp) == cudaSuccess &&
+              cudaMemsetAsync(h->dev, 0, (size_t)h->buf_bytes, h->comp) == cudaSuccess &&
+              cudaMallocAsync(&h->state, sizeof(STState), h->comp) == cudaSuccess &&
+              cudaMallocAsync(&h->counts, sizeof(long long) * tiles, h->comp) == cudaSuccess &&
+              alloc_table(h, &h->t, 1 << 16) == BFL_OK;
     if (ok) {
         STState s0 = {~0ull, 0u, 0u, 0ull, 0ull};
         ok = cudaMemcpyAsync(h->state, &s0, sizeof(s0), cudaMemcpyHostToDevice, h->comp) == cudaSuccess &&
              cudaStreamSynchronize(h->comp) == cudaSuccess;
     }
-    if (!ok) {
-        set_error(std::string("Stream ingest setup failed: ") + cudaGetErrorString(cudaGetLastError()));
-        bfl_stream_ingest_destroy(h);
-        return nullptr;
-    }
-    return h;
+    return setup_done(h, ok, "Stream");
 }
 
-void bfl_stream_ingest_destroy(bfl_stream_ingest_t* h) {
-    if (!h) return;
-    if (h->comp) cudaStreamSynchronize(h->comp);
-    for (int i = 0; i < 2; ++i)
-        if (h->host[i]) cudaFreeHost(h->host[i]);
-    for (void* p : {(void*)h->dev, (void*)h->state, (void*)h->counts, (void*)h->boff, (void*)h->blen, (void*)h->slot_of,
-                    (void*)h->bhash, (void*)h->user, (void*)h->item, (void*)h->flag, (void*)h->t.key, (void*)h->t.first,
-                    (void*)h->t.entry, (void*)h->E.off, (void*)h->E.first, (void*)h->E.foff, (void*)h->E.len, (void*)h->pool,
-                    (void*)h->vr, (void*)h->vc, (void*)h->vv, (void*)h->tu, (void*)h->ti, (void*)h->tv})
-        if (p) cudaFree(p);
-    for (auto& v : h->marks)
-        for (cudaEvent_t e : v) cudaEventDestroy(e);
-    if (h->comp) cudaStreamDestroy(h->comp);
-    delete h;
-}
+void bfl_stream_ingest_destroy(bfl_stream_ingest_t* h) { delete h; }
 
-int bfl_stream_ingest_staging(bfl_stream_ingest_t* h, int slot, void** host_ptr) {
-    if (!h || slot < 0 || slot > 1 || !host_ptr) BFL_FAIL(BFL_ERR_ARG, "bad staging arguments");
-    *host_ptr = h->host[slot];
-    return BFL_OK;
-}
+int bfl_stream_ingest_staging(bfl_stream_ingest_t* h, int slot, void** host_ptr) { return staging(h, slot, host_ptr); }
 
 int bfl_stream_ingest_load_iid(bfl_stream_ingest_t* h, const char* names, const int64_t* offsets, int64_t n) {
     if (!h || n <= 0 || !offsets || (offsets[n] && !names) || offsets[0] != 0) BFL_FAIL(BFL_ERR_ARG, "bad iid arguments");
@@ -779,12 +738,12 @@ int bfl_stream_ingest_load_iid(bfl_stream_ingest_t* h, const char* names, const 
     BFL_CUDA(cudaMallocAsync(&d_offs, sizeof(long long) * (n + 1), h->comp));
     if (bytes) BFL_CUDA(cudaMemcpyAsync(d_names, names, (size_t)bytes, cudaMemcpyHostToDevice, h->comp));
     BFL_CUDA(cudaMemcpyAsync(d_offs, offsets, sizeof(long long) * (n + 1), cudaMemcpyHostToDevice, h->comp));
-    if (int rc = mark(h, ST_INTERN)) return rc;
+    if (int rc = mark(h, ST_INTERN, h->comp)) return rc;
     st_name_kernel<<<grid_for(n), 256, 0, h->comp>>>(d_names, d_offs, n, h->hash_bits, h->boff, h->blen, h->bhash);
     BFL_LAUNCHED();
     // name i gets ordinal n - 1 - i: the slot's minimum is the name's LAST index (a dict comprehension keeps the last)
     if (int rc = intern(h, d_names, n, n - 1, -1, 0, false, nullptr, nullptr, nullptr)) return rc;
-    if (int rc = mark(h, ST_INTERN)) return rc;
+    if (int rc = mark(h, ST_INTERN, h->comp)) return rc;
     BFL_CUDA(cudaFreeAsync(d_names, h->comp));
     BFL_CUDA(cudaFreeAsync(d_offs, h->comp));
     h->iid_count = n;
@@ -792,17 +751,14 @@ int bfl_stream_ingest_load_iid(bfl_stream_ingest_t* h, const char* names, const 
 }
 
 int bfl_stream_ingest_feed(bfl_stream_ingest_t* h, int slot, int64_t n, int is_last) {
-    if (!h || slot < 0 || slot > 1 || n < 0 || n > h->block_bytes) BFL_FAIL(BFL_ERR_ARG, "bad feed arguments");
-    if (h->last_fed) BFL_FAIL(BFL_ERR_STATE, "feed after the last block");
-    if (!is_last && (n == 0 || h->host[slot][n - 1] != '\n')) BFL_FAIL(BFL_ERR_ARG, "a block that is not the last must end with '\\n'");
-    h->last_fed = is_last != 0;
+    if (int rc = check_feed(h, slot, n, is_last)) return rc;
     if (n) h->open_line = h->host[slot][n - 1] != '\n';
     if (n == 0 || h->decline) return BFL_OK;
     unsigned char* d = h->dev + 16;
-    if (int rc = mark(h, ST_H2D)) return rc;
+    if (int rc = mark(h, ST_H2D, h->comp)) return rc;
     BFL_CUDA(cudaMemcpyAsync(d, h->host[slot], (size_t)n, cudaMemcpyHostToDevice, h->comp));
-    if (int rc = mark(h, ST_H2D)) return rc;
-    if (int rc = mark(h, ST_PARSE)) return rc;
+    if (int rc = mark(h, ST_H2D, h->comp)) return rc;
+    if (int rc = mark(h, ST_PARSE, h->comp)) return rc;
     const long long tiles = (n + ST_TILE - 1) / ST_TILE;
     st_count_kernel<<<(unsigned)tiles, ST_THREADS, 0, h->comp>>>(d, n, h->g.ascii_ws, h->counts);
     BFL_LAUNCHED();
@@ -835,10 +791,10 @@ int bfl_stream_ingest_feed(bfl_stream_ingest_t* h, int slot, int64_t n, int is_l
     a.bhash = h->bhash;
     st_write_kernel<<<(unsigned)tiles, ST_THREADS, 0, h->comp>>>(a);
     BFL_LAUNCHED();
-    if (int rc = mark(h, ST_PARSE)) return rc;
-    if (int rc = mark(h, ST_INTERN)) return rc;
+    if (int rc = mark(h, ST_PARSE, h->comp)) return rc;
+    if (int rc = mark(h, ST_INTERN, h->comp)) return rc;
     if (int rc = intern(h, d, nb, h->tokens, 1, h->fed, frozen, h->user, h->item, frozen ? nullptr : h->flag)) return rc;
-    if (int rc = mark(h, ST_INTERN)) return rc;
+    if (int rc = mark(h, ST_INTERN, h->comp)) return rc;
     STState s;
     if (int rc = read_state(h, &s)) return rc;
     h->decline |= s.decline;
@@ -869,7 +825,7 @@ int bfl_stream_ingest_finish(bfl_stream_ingest_t* h, int64_t* num_tokens, int64_
     *decline_line = s.decline_line == ~0ull ? -1 : (int64_t)s.decline_line;
     *num_items = 0;
     if (h->decline) return BFL_OK;
-    if (int rc = mark(h, ST_NUMBER)) return rc;
+    if (int rc = mark(h, ST_NUMBER, h->comp)) return rc;
     const long long m = h->n_entries;
     int32_t* e_item = nullptr;
     BFL_CUDA(cudaMallocAsync(&e_item, sizeof(int32_t) * std::max<long long>(m, 1), h->comp));
@@ -910,7 +866,7 @@ int bfl_stream_ingest_finish(bfl_stream_ingest_t* h, int64_t* num_tokens, int64_
         if (*p) BFL_CUDA(cudaFreeAsync(*p, h->comp));
         *p = nullptr;
     }
-    if (int rc = mark(h, ST_NUMBER)) return rc;
+    if (int rc = mark(h, ST_NUMBER, h->comp)) return rc;
     BFL_CUDA(cudaStreamSynchronize(h->comp));
     *num_items = h->num_items;
     return BFL_OK;
@@ -941,7 +897,7 @@ int bfl_stream_ingest_split(bfl_stream_ingest_t* h, int32_t num_users, int metho
     h->num_users = num_users;
     h->as_matrix = as_matrix != 0;
     cudaStream_t st = h->comp;
-    if (int rc = mark(h, ST_SPLIT)) return rc;
+    if (int rc = mark(h, ST_SPLIT, h->comp)) return rc;
     long long *ustart = nullptr, *hpos = nullptr, *hstart = nullptr, *vcnt = nullptr;
     int32_t *hu = nullptr, *hi = nullptr;
     const size_t T1 = (size_t)std::max<long long>(T, 1);
@@ -1039,7 +995,7 @@ int bfl_stream_ingest_split(bfl_stream_ingest_t* h, int32_t num_users, int metho
         for (void* p : {(void*)rpos, (void*)ku, (void*)skey}) BFL_CUDA(cudaFreeAsync(p, st));
         h->n_train = m;
     }
-    if (int rc = mark(h, ST_SPLIT)) return rc;
+    if (int rc = mark(h, ST_SPLIT, h->comp)) return rc;
     BFL_CUDA(cudaStreamSynchronize(st));
     *n_vali = h->n_vali;
     *n_train = h->n_train;
@@ -1062,54 +1018,14 @@ int bfl_stream_ingest_build(bfl_stream_ingest_t* h, int orientation, int64_t* in
     if (!h || !h->split_done || orientation < 0 || orientation > 1 || (orientation && !h->as_matrix) || h->built[orientation] ||
         !indptr || (h->n_train && (!key || !val)))
         BFL_FAIL(BFL_ERR_ARG, "bad build arguments (split first, each orientation once, colwise in matrix mode)");
-    const int32_t nmaj = orientation ? h->num_items : h->num_users, nmin = orientation ? h->num_users : h->num_items;
-    const long long nnz = h->n_train;
-    int64_t* d_ind = nullptr;
-    int32_t* d_key = nullptr;
-    float* d_val = nullptr;
-    const size_t m = (size_t)std::max<long long>(nnz, 1);
-    BFL_CUDA(cudaMallocAsync(&d_ind, sizeof(int64_t) * nmaj, h->comp));
-    BFL_CUDA(cudaMallocAsync(&d_key, sizeof(int32_t) * m, h->comp));
-    BFL_CUDA(cudaMallocAsync(&d_val, sizeof(float) * m, h->comp));
-    const int stg = orientation ? ST_CSR_COL : ST_CSR_ROW;
-    if (int rc = mark(h, stg)) return rc;
-    int rc = bfl_csr_from_triples_device(orientation ? h->ti : h->tu, orientation ? h->tu : h->ti, h->tv, nnz, nmaj,
-                                         std::max(nmin, 1), h->as_matrix ? 1 : 0, d_ind, d_key, d_val, h->comp);
-    if (rc != BFL_OK) return rc;
-    if ((rc = mark(h, stg))) return rc;
-    h->built[orientation] = true;
-    if ((rc = mark(h, ST_D2H))) return rc;
-    BFL_CUDA(cudaMemcpyAsync(indptr, d_ind, sizeof(int64_t) * nmaj, cudaMemcpyDeviceToHost, h->comp));
-    if (nnz) {
-        BFL_CUDA(cudaMemcpyAsync(key, d_key, sizeof(int32_t) * nnz, cudaMemcpyDeviceToHost, h->comp));
-        BFL_CUDA(cudaMemcpyAsync(val, d_val, sizeof(float) * nnz, cudaMemcpyDeviceToHost, h->comp));
-    }
-    if ((rc = mark(h, ST_D2H))) return rc;
-    BFL_CUDA(cudaFreeAsync(d_ind, h->comp));
-    BFL_CUDA(cudaFreeAsync(d_key, h->comp));
-    BFL_CUDA(cudaFreeAsync(d_val, h->comp));
-    BFL_CUDA(cudaStreamSynchronize(h->comp));
-    return BFL_OK;
+    return build_to_host(h, orientation, h->tu, h->ti, h->tv, h->n_train, h->num_users, h->num_items, h->as_matrix ? 1 : 0,
+                         orientation ? ST_CSR_COL : ST_CSR_ROW, ST_D2H, indptr, key, val);
 }
 
 // stage_ms[8]: H2D, parse, intern, number, split, rowwise CSR, colwise CSR, D2H (summed device time of each stage);
 // *peak_bytes: high-water mark of the device's default memory pool since create
 int bfl_stream_ingest_stats(bfl_stream_ingest_t* h, double* stage_ms, int64_t* peak_bytes) {
-    if (!h || !stage_ms || !peak_bytes) BFL_FAIL(BFL_ERR_ARG, "bad stats arguments");
-    BFL_CUDA(cudaStreamSynchronize(h->comp));
-    for (int s = 0; s < ST_COUNT; ++s) {
-        double tot = 0.0;
-        for (size_t i = 0; i + 1 < h->marks[s].size(); i += 2) {
-            float ms = 0.f;
-            BFL_CUDA(cudaEventElapsedTime(&ms, h->marks[s][i], h->marks[s][i + 1]));
-            tot += ms;
-        }
-        stage_ms[s] = tot;
-    }
-    uint64_t hi = 0;
-    BFL_CUDA(cudaMemPoolGetAttribute(h->mpool, cudaMemPoolAttrUsedMemHigh, &hi));
-    *peak_bytes = (int64_t)hi;
-    return BFL_OK;
+    return stats(h, stage_ms, peak_bytes);
 }
 
 }  // extern "C"

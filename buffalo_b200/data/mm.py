@@ -1,5 +1,4 @@
 """MatrixMarket ingest (buffalo/data/mm.py): text file, scipy sparse or dense 2-D array -> database."""
-import mmap
 import os
 
 import numpy as np
@@ -7,6 +6,7 @@ import scipy.sparse
 
 from buffalo_b200.data.base import Data, DataOption, DataReader
 from buffalo_b200.data import prepro
+from buffalo_b200.data.text_ingest import _Fallback, feed_blocks, read_ranges
 from buffalo_b200.misc import aux, log
 
 
@@ -97,10 +97,6 @@ MAX_LINE = 1024                          # BFL_MM_MAX_LINE: longer lines are gra
 _DEVICE_BYTES_PER_NNZ = 40               # peak of the device build: triples, CSR output and radix-sort scratch
 
 
-class _Fallback(Exception):
-    """The device path declines the file; the host path builds it instead."""
-
-
 def _data_offset(path, skip):
     """Byte offset of the first line after the header, or None when the header lines use a bare '\r' line end
     (text mode counts those as line ends, a byte split on '\n' would not)."""
@@ -133,32 +129,7 @@ def _device_ingest(path, U, I, nnz_hint, skip, vopt, logger, block_bytes=None):
     slow_cap = min(nnz_hint, DEVICE_INGEST_MAX_SLOW)
     with backend.MMIngest(U, I, nnz_hint, block, skip, slow_cap) as ing, open(path, "rb", buffering=0) as fin:
         fin.seek(data_off)
-        carry, slot = b"", 0
-        while True:
-            buf = ing.staging(slot)
-            k = len(carry)
-            buf[:k] = np.frombuffer(carry, np.uint8)
-            view, total = memoryview(buf), k
-            t0 = time.perf_counter()
-            while total < block:
-                got = fin.readinto(view[total:])
-                if not got:
-                    break
-                total += got
-            host_ms["read"] += 1e3 * (time.perf_counter() - t0)
-            last = total < block
-            cut = total
-            if not last:
-                lo = max(0, total - MAX_LINE - 1)
-                nl = np.flatnonzero(buf[lo:total] == 10)
-                if not len(nl):
-                    raise _Fallback("a line longer than %d bytes" % min(MAX_LINE, block - 1))
-                cut = lo + int(nl[-1]) + 1
-                carry = bytes(buf[cut:total])
-            ing.feed(slot, cut, last)
-            if last:
-                break
-            slot ^= 1
+        feed_blocks(ing, fin, block, MAX_LINE, host_ms)
         r = ing.finish()
         if r["reject_line"] >= 0:
             raise _Fallback("line %d is outside the device grammar" % r["reject_line"])
@@ -174,10 +145,8 @@ def _device_ingest(path, U, I, nnz_hint, skip, vopt, logger, block_bytes=None):
         if r["n_slow"]:
             t0 = time.perf_counter()
             ordinal, offset, length = ing.slow_tokens(r["n_slow"])
-            with open(path, "rb") as f, mmap.mmap(f.fileno(), 0, access=mmap.ACCESS_READ) as text:
-                toks = [text[data_off + o:data_off + o + n] for o, n in zip(offset.tolist(), length.tolist())]
             try:
-                vals = _parse_value_tokens(toks)
+                vals = _parse_value_tokens(read_ranges(path, offset + data_off, length))
             except ValueError as e:
                 raise _Fallback("a value the host parser rejects (%s)" % e)
             host_ms["slow_parse"] = 1e3 * (time.perf_counter() - t0)

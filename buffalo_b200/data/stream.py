@@ -5,7 +5,6 @@ newest.  API-compatible container; the three MF trainers only consume data_type 
 split on the GPU (csrc/stream_ingest.cu) into the same database; files the device path declines go to the host loop."""
 import codecs
 import locale
-import mmap
 import os
 import time
 from collections import Counter
@@ -13,6 +12,7 @@ from collections import Counter
 import numpy as np
 
 from buffalo_b200.data.base import Data, DataOption
+from buffalo_b200.data.text_ingest import _Fallback, feed_blocks, find_cut, read_ranges
 from buffalo_b200.misc import aux, log
 
 
@@ -52,20 +52,9 @@ _DECLINE = ((1, "a bare '\\r' line end"), (2, "bytes that are not UTF-8"), (4, "
             (32, "too little device memory"), (64, "more than 2^31 - 2 lines or items"))
 
 
-class _Fallback(Exception):
-    """The device path declines the file; the host path builds it instead."""
-
-
 def _find_cut(buf, total, block):
-    """End of the last line in buf[:total]: one past its line feed."""
-    hi = total
-    while hi > 0:
-        lo = max(0, hi - (1 << 20))
-        nl = np.flatnonzero(buf[lo:hi] == 10)
-        if len(nl):
-            return lo + int(nl[-1]) + 1
-        hi = lo
-    raise _Fallback("a line longer than the %d-byte block" % block)
+    """Stream's cut: the end of the last line anywhere in buf[:total]; a line longer than the block declines the file."""
+    return find_cut(buf, total, block)
 
 
 def _device_ingest(path, uids, names, vopt, as_matrix, block_bytes=None):
@@ -80,32 +69,10 @@ def _device_ingest(path, uids, names, vopt, as_matrix, block_bytes=None):
     free = backend.device_free_bytes()
     if need > free:
         raise _Fallback("estimated %.1f GB of device memory for the parse, %.1f GB free" % (need / 1e9, free / 1e9))
-    size = os.path.getsize(path)
     with backend.StreamIngest(block, WHITESPACE, _HASH_BITS) as ing, open(path, "rb", buffering=0) as fin:
         if names is not None:
             ing.load_iid([s.encode("utf-8") for s in names])
-        carry, slot, last_byte = b"", 0, b"\n"
-        while True:
-            buf = ing.staging(slot)
-            k = len(carry)
-            buf[:k] = np.frombuffer(carry, np.uint8)
-            view, total = memoryview(buf), k
-            t0 = time.perf_counter()
-            while total < block:
-                got = fin.readinto(view[total:])
-                if not got:
-                    break
-                total += got
-            host_ms["read"] += 1e3 * (time.perf_counter() - t0)
-            last = total < block or fin.tell() == size
-            cut = total if last else _find_cut(buf, total, block)
-            carry = b"" if last else bytes(buf[cut:total])
-            if cut:
-                last_byte = bytes(buf[cut - 1:cut])
-            ing.feed(slot, cut, last)
-            if last:
-                break
-            slot ^= 1
+        last_byte = feed_blocks(ing, fin, block, block, host_ms)
         r = ing.finish()
         if r["decline"]:
             why = [s for b, s in _DECLINE if r["decline"] & b]
@@ -124,8 +91,7 @@ def _device_ingest(path, uids, names, vopt, as_matrix, block_bytes=None):
         if names is None:
             t0 = time.perf_counter()
             off, ln = ing.names(num_items)
-            with open(path, "rb") as f, mmap.mmap(f.fileno(), 0, access=mmap.ACCESS_READ) as text:
-                names = [text[o:o + n].decode("utf-8") for o, n in zip(off.tolist(), ln.tolist())]
+            names = [b.decode("utf-8") for b in read_ranges(path, off, ln)]
             host_ms["names"] = 1e3 * (time.perf_counter() - t0)
         method = vopt.name if vopt else None
         vali_n = vopt.get("n", 0) if method == "newest" else 0

@@ -1,5 +1,5 @@
-"""Host side of the device MatrixMarket parser (data/mm.py): routing, header parsing, the block/carry protocol and the
-host re-parse of the value tokens the device leaves to it.  No GPU needed: the device handle is replaced by a fake."""
+"""Host side of the device MatrixMarket parser (data/mm.py): routing, header parsing and the host re-parse of the value
+tokens the device leaves to it.  No GPU needed (the block/carry protocol is in test_text_ingest_cpu.py)."""
 import numpy as np
 import pytest
 
@@ -79,50 +79,3 @@ def test_value_tokens_match_host_reader(tmp_path):
     assert got.dtype == np.float32 and got.tobytes() == want.tobytes()
     with pytest.raises(ValueError):
         mmmod._parse_value_tokens([b"1.5x"])
-
-
-class _FakeIngest(object):
-    """Stands in for backend.MMIngest: records the fed blocks and declines the file at finish()."""
-    blocks = []
-
-    def __init__(self, U, I, nnz_hint, block, header_lines, slow_cap):
-        self.block = block
-        self.bufs = [np.zeros(block, np.uint8), np.zeros(block, np.uint8)]
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        pass
-
-    def staging(self, slot):
-        return self.bufs[slot]
-
-    def feed(self, slot, n, is_last):
-        b = self.bufs[slot][:n].tobytes()
-        assert is_last or b.endswith(b"\n")
-        _FakeIngest.blocks.append((b, is_last))
-
-    def finish(self):
-        return dict(nnz=0, tokmask=0, reject_line=1, range_line=-1, n_slow=0)
-
-
-@pytest.mark.parametrize("block", [16, 64, 100, 4096])
-@pytest.mark.parametrize("final_eol", [True, False])
-def test_blocks_end_on_line_ends(tmp_path, monkeypatch, block, final_eol):
-    """The caller carries the partial last line of a block into the next one: every block but the last ends with
-    '\\n', and the blocks concatenate to the text after the header."""
-    from buffalo_b200 import backend
-    monkeypatch.setattr(backend, "MMIngest", _FakeIngest)
-    monkeypatch.setattr(backend, "device_free_bytes", lambda: 1 << 40)
-    body = "".join("%d %d %s\n" % (i % 7 + 1, i % 5 + 1, "1" * (i % 11 + 1)) for i in range(300))
-    body = body if final_eol else body[:-1]
-    p = tmp_path / "b.mtx"
-    p.write_text("%%MatrixMarket matrix coordinate real general\n7 5 300\n" + body)
-    _FakeIngest.blocks = []
-    with pytest.raises(mmmod._Fallback):
-        mmmod._device_ingest(str(p), 7, 5, 300, 2, None, None, block_bytes=block)
-    blocks = _FakeIngest.blocks
-    assert b"".join(b for b, _ in blocks) == body.encode()
-    assert [last for _, last in blocks] == [False] * (len(blocks) - 1) + [True]
-    assert all(len(b) <= block for b, _ in blocks)
