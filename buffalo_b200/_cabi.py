@@ -118,6 +118,15 @@ PROTOTYPES = {
     "bfl_serve_topk_device": (C.c_int, [_vp, _vp, _i64, C.c_int, _vp, _vp, _vp]),
     "bfl_seen_topk": (C.c_int, [_vp, _vp, _i64, C.c_int, _vp, _vp, _vp, _vp]),
     "bfl_seen_topk_device": (C.c_int, [_vp, _vp, _i64, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp]),
+    # IVF index
+    "bfl_ivf_create": (_vp, []),
+    "bfl_ivf_destroy": (None, [_vp]),
+    "bfl_ivf_attach": (C.c_int, [_vp]),
+    "bfl_ivf_build_device": (C.c_int, [_vp, _vp, _i64, C.c_int, C.c_int, _vp, C.c_int, C.c_int, C.c_uint64]),
+    "bfl_ivf_search_device": (C.c_int, [_vp, _vp, _i64, C.c_int, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp]),
+    "bfl_ivf_set_batch_rows": (C.c_int, [_vp, _i64]),
+    "bfl_ivf_info": (C.c_int, [_vp, _pi64, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "bfl_ivf_read": (C.c_int, [_vp, _vp, _vp, _vp]),
     # validation metrics
     "bfl_eval_unsorted_rows_device": (C.c_int, [_vp, _vp, _i64, _vp, _vp]),
     "bfl_eval_topk_masked_device": (C.c_int, [_vp, _i64, C.c_int, _vp, _i64, C.c_int, _vp, C.c_int, C.c_int, _vp, _vp,

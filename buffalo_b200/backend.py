@@ -923,3 +923,123 @@ def popularity_table_host(keys, n_items, power):
     _cabi.check(_cabi.lib().bfl_popularity_table_host(k.ctypes.data, len(k), int(n_items), int(power), cum.ctypes.data),
                 "bfl_popularity_table_host")
     return cum
+
+IVF_MAX_LISTS = 65536
+IVF_DMAX = 256
+
+
+class IVF(object):
+    """Inverted-file index (csrc/ivf.cu, bfl_ivf_*, DESIGN.md 4.12): the rows clustered by spherical k-means into nlist
+    lists; search scores each query against the rows of its nprobe best lists only, with the scores and ranking of
+    Serve.topk, so nprobe = nlist gives Serve.topk's result bit for bit.  GPU only: build and search raise the
+    library's "no CPU fallback" error without one."""
+
+    def __init__(self):
+        self._lib = _cabi.lib()
+        self._h = self._lib.bfl_ivf_create()
+        if not self._h:
+            raise MemoryError("bfl_ivf_create")
+        self.nlist = 0
+        self.num_rows = 0
+        self.has_bias = False
+
+    def close(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            self._lib.bfl_ivf_destroy(h)
+
+    __del__ = close
+
+    def _attach(self):
+        _cabi.check(self._lib.bfl_ivf_attach(self._h), "bfl_ivf_attach")
+
+    def build(self, rows, bias=None, nlist=1024, iters=10, seed=0):
+        """rows float32 [n, d] host array (C-contiguous), bias float32 [n] or None.  Replaces any earlier index."""
+        _host(rows, np.float32, 2, "rows")
+        n, d = rows.shape
+        nlist, iters = int(nlist), int(iters)
+        if not 1 <= nlist <= min(n, IVF_MAX_LISTS):
+            raise ValueError("nlist must be in [1, min(rows, %d)] = [1, %d]" % (IVF_MAX_LISTS, min(n, IVF_MAX_LISTS)))
+        if iters < 1:
+            raise ValueError("iters must be at least 1")
+        if not 0 < d <= IVF_DMAX:
+            raise ValueError("the index holds rows of 1 to %d floats, got %d" % (IVF_DMAX, d))
+        if bias is not None:
+            bias = np.ascontiguousarray(np.asarray(bias, dtype=np.float32).reshape(-1))
+            if bias.shape[0] != n:
+                raise ValueError("bias must have one value per row")
+        self._attach()
+        import torch
+        dr = torch.from_numpy(rows).cuda()
+        db = None if bias is None else torch.from_numpy(bias).cuda()
+        torch.cuda.synchronize()
+        self.nlist = self.num_rows = 0
+        _cabi.check(self._lib.bfl_ivf_build_device(self._h, dr.data_ptr(), n, d, d, None if db is None else db.data_ptr(),
+                                                   nlist, iters, int(seed) & (2 ** 64 - 1)), "bfl_ivf_build_device")
+        self.nlist, self.num_rows, self.d, self.has_bias = nlist, n, d, bias is not None
+
+    def _check_nprobe(self, nprobe):
+        if isinstance(nprobe, bool) or not isinstance(nprobe, (int, np.integer)):
+            raise ValueError("nprobe must be an integer")
+        nprobe = int(nprobe)
+        if not 1 <= nprobe <= self.nlist:
+            raise ValueError("nprobe must be in [1, nlist=%d]" % self.nlist)
+        if nprobe > SERVE_KMAX and nprobe != self.nlist:
+            raise ValueError("nprobe above %d must be nlist=%d" % (SERVE_KMAX, self.nlist))
+        return nprobe
+
+    def search_device(self, queries, nprobe, k, use_bias=False, stream=None):
+        """queries: torch float32 CUDA tensor [n, >= d] -> (int32 [n, k] row ids, float32 [n, k] scores) CUDA tensors."""
+        import torch
+        nprobe, k = self._check_nprobe(nprobe), Serve._check_k(k)
+        n = queries.shape[0]
+        idx = torch.empty((n, k), dtype=torch.int32, device=queries.device)
+        val = torch.empty((n, k), dtype=torch.float32, device=queries.device)
+        if n:
+            _cabi.check(self._lib.bfl_ivf_search_device(self._h, _dev(queries, "float32", "queries"), n,
+                                                        queries.stride(0), nprobe, k, int(bool(use_bias)),
+                                                        idx.data_ptr(), val.data_ptr(), _stream_ptr(stream)),
+                        "bfl_ivf_search_device")
+        return idx, val
+
+    def search(self, queries, nprobe, k, use_bias=False):
+        """queries float32 [n, >= d] host array -> (int32 [n, k], float32 [n, k]) host arrays: best first, ties to the
+        smaller row id, -1 / 0.0 where the probed lists hold fewer than k rows."""
+        _host(queries, np.float32, 2, "queries")
+        nprobe, k = self._check_nprobe(nprobe), Serve._check_k(k)
+        self._attach()
+        if queries.shape[0] == 0:
+            return np.zeros((0, k), np.int32), np.zeros((0, k), np.float32)
+        import torch
+        idx, val = self.search_device(torch.from_numpy(queries).cuda(), nprobe, k, use_bias)
+        return idx.cpu().numpy(), val.cpu().numpy()
+
+    def _set_batch_rows(self, rows):
+        """Queries per internal batch at most (0: automatic); lets tests cross batch edges at small sizes."""
+        _cabi.check(self._lib.bfl_ivf_set_batch_rows(self._h, int(rows)), "bfl_ivf_set_batch_rows")
+
+    def _read(self, what):
+        n, nl, ld, d = C.c_int64(0), C.c_int(0), C.c_int(0), C.c_int(0)
+        _cabi.check(self._lib.bfl_ivf_info(self._h, C.byref(n), C.byref(nl), C.byref(ld), C.byref(d)), "bfl_ivf_info")
+        out = {"centroids": np.empty((nl.value, ld.value), np.float32), "offsets": np.empty(nl.value, np.int64),
+               "ids": np.empty(n.value, np.int32)}[what]
+        args = [out.ctypes.data if w == what else None for w in ("centroids", "offsets", "ids")]
+        _cabi.check(self._lib.bfl_ivf_read(self._h, *args), "bfl_ivf_read")
+        return out[:, :d.value] if what == "centroids" else out
+
+    def centroids(self):
+        """float32 [nlist, d]: the unit centroids."""
+        return self._read("centroids")
+
+    def offsets(self):
+        """int64 [nlist]: END offsets of the lists into ids()."""
+        return self._read("offsets")
+
+    def ids(self):
+        """int32 [n]: the row ids of every list, list after list, ascending within a list."""
+        return self._read("ids")
+
+    def nbytes(self):
+        """Device bytes of the index: centroids, offsets, ids, list-major rows and bias, chunk counts."""
+        return (self.nlist * self.d * 4 + self.nlist * 8 + self.num_rows * 4 + self.num_rows * self.d * 4
+                + (self.num_rows * 4 if self.has_bias else 0) + self.nlist * 4)

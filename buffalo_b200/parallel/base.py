@@ -127,14 +127,67 @@ class ParALS(Parallel):
                 raise RuntimeError("pool is empty")
         return kept, idx, pool
 
-    def most_similar(self, keys, topk=10, group="item", pool=None, repr=False, ef_search=-1, use_mmap=True):
+    def build_index(self, nlist, group="item", iters=10):
+        """Builds the IVF index (DESIGN.md 4.12) of the current item (algo.Q, with algo.Qb for ParBPRMF with use_bias)
+        or user (algo.P) factors: spherical k-means into nlist lists, iters rounds, seeded with algo.opt.random_seed.
+        topk_recommendation / most_similar with nprobe=... then search it.  It replaces the group's earlier index and
+        goes stale when the factors change (normalize() included): build it again then.  On the GPU only."""
+        if group not in ("item", "user"):
+            raise ValueError(f"Not supported group: {group}")
+        F = self.algo.Q if group == "item" else self.algo.P
+        Fb = self._index_bias(group)
+        if isinstance(nlist, bool) or not isinstance(nlist, (int, np.integer)) or not 1 <= nlist <= min(
+                F.shape[0], backend.IVF_MAX_LISTS):
+            raise ValueError("nlist must be an integer in [1, min(rows, %d)] = [1, %d], got %r"
+                             % (backend.IVF_MAX_LISTS, min(F.shape[0], backend.IVF_MAX_LISTS), nlist))
+        if isinstance(iters, bool) or not isinstance(iters, (int, np.integer)) or iters < 1:
+            raise ValueError("iters must be an integer of at least 1, got %r" % (iters,))
+        F = np.ascontiguousarray(F, dtype=np.float32)
+        ivf = backend.IVF()
+        ivf.build(F, Fb, int(nlist), int(iters), seed=int(self.algo.opt.random_seed))
+        ivf.keys = self._fingerprint(F, Fb)
+        if getattr(self, "_indexes", None) is None:
+            self._indexes = {}
+        self._indexes[group] = ivf
+
+    def _index_bias(self, group):
+        Qb = getattr(self.algo, "Qb", None)
+        if group != "item" or not self._bias or not self.algo.opt.get("use_bias") or Qb is None or not Qb.size:
+            return None
+        return np.ascontiguousarray(Qb, dtype=np.float32).reshape(-1)
+
+    def _search_index(self, group, idx, A, topk, nprobe, with_bias, normalized):
+        """The IVF search of the rows A[idx] in the group's index; every check before any device work."""
+        ivf = (getattr(self, "_indexes", None) or {}).get(group)
+        if ivf is None:
+            raise RuntimeError("no %s index: call build_index(nlist, group=%r) first" % (group, group))
+        nprobe = ivf._check_nprobe(nprobe)
+        topk = backend.Serve._check_k(topk)
+        F = np.ascontiguousarray(self.algo.Q if group == "item" else self.algo.P, dtype=np.float32)
+        now = self._fingerprint(F, self._index_bias(group) if with_bias else None)
+        if now[0] != ivf.keys[0] or (with_bias and now[1] != ivf.keys[1]):
+            raise RuntimeError("the %s index is stale: the factors changed since build_index; call build_index again%s"
+                               % (group, " after algo.normalize(%r)" % group if normalized else ""))
+        return ivf.search(np.ascontiguousarray(A[idx], dtype=np.float32), nprobe, topk,
+                          use_bias=with_bias and ivf.has_bias)
+
+    def most_similar(self, keys, topk=10, group="item", pool=None, repr=False, ef_search=-1, use_mmap=True,
+                     nprobe=None):
+        """nprobe: None ranks every row; an integer in [1, nlist] searches the group's index (build_index, after
+        algo.normalize(group)) and ranks the rows of the nprobe lists nearest each query.  ef_search and use_mmap are
+        accepted and ignored."""
+        if nprobe is not None and pool is not None:
+            raise ValueError("nprobe does not take a pool")
         self.algo.normalize(group=group)
         _, idx, pool = self._resolve(keys, pool, group)
         if group not in ("item", "user"):
             raise ValueError(f"Not supported group: {group}")
         F = self.algo.Q if group == "item" else self.algo.P
         names = self.algo._idmanager.itemids if group == "item" else self.algo._idmanager.userids
-        topks, scores = self._run(idx, F, F, None, topk, pool)
+        if nprobe is not None:
+            topks, scores = self._search_index(group, idx, F, topk, nprobe, False, True)
+        else:
+            topks, scores = self._run(idx, F, F, None, topk, pool)
         if repr:
             topks = [[names[t] for t in tt if t != -1] for tt in topks]
         return topks, scores
@@ -162,15 +215,25 @@ class ParALS(Parallel):
         from buffalo_b200.evaluate.device import _gather_rows
         return _gather_rows(ends, keys, idx)
 
-    def topk_recommendation(self, keys, topk=10, pool=None, repr=False, exclude_seen=False):
+    def topk_recommendation(self, keys, topk=10, pool=None, repr=False, exclude_seen=False, nprobe=None):
         """exclude_seen: False; True to leave out each user's training items (the "rowwise" rows of the algo's data);
         or a scipy sparse (num_users, num_items) matrix whose row u lists the items user u does not get back.  Rows
-        left with fewer than topk candidates are padded with -1 / 0.0."""
+        left with fewer than topk candidates are padded with -1 / 0.0.  nprobe: None ranks every item; an integer in
+        [1, nlist] searches the item index (build_index) and ranks the items of the nprobe lists nearest each user,
+        without pool or exclude_seen."""
+        if nprobe is not None:
+            if pool is not None:
+                raise ValueError("nprobe does not take a pool")
+            if scipy.sparse.issparse(exclude_seen) or exclude_seen:
+                raise ValueError("nprobe does not take exclude_seen")
         if self.algo.opt._nrz_P or self.algo.opt._nrz_Q:
             raise RuntimeError("Cannot make topk recommendation with normalized factors")
         kept, idx, pool = self._resolve(keys, pool, "user")
         Qb = self.algo.Qb if self._bias and self.algo.opt.get("use_bias") else None
-        if scipy.sparse.issparse(exclude_seen) or exclude_seen:
+        if nprobe is not None:
+            topks, scores = self._search_index("item", idx, self.algo.P, topk, nprobe,
+                                               self._index_bias("item") is not None, False)
+        elif scipy.sparse.issparse(exclude_seen) or exclude_seen:
             seen = self._seen_rows(idx, exclude_seen)
             topks, scores = self._run(idx, self.algo.P, self.algo.Q, Qb, topk, pool, seen)
         else:

@@ -392,6 +392,39 @@ int bfl_seen_topk_device(bfl_serve_t* h, const int32_t* d_query_idx, int64_t n, 
                          void* stream);
 
 /* =====================================================================================
+ * Inverted-file (IVF-Flat) index for batch serving (DESIGN.md 4.12).  build_device clusters n DEVICE rows (pitch ld,
+ * first d columns, d <= 256) by spherical k-means into nlist lists (nlist in [1, min(n, 65536)], iters >= 1): nlist
+ * distinct rows drawn with `seed` start it, each row goes to the centroid of the largest dot product (ties to the
+ * smaller list), a centroid becomes the normalised sum of its members' unit rows (an empty list keeps its centroid).
+ * The handle keeps the centroids, the lists (END offsets, row ids ascending) and list-major copies of the rows and of
+ * the bias (d_bias nullable), so the caller's arrays may be freed after the call.  The same arguments and seed give a
+ * bitwise equal index.
+ *  - search_device: DEVICE queries [n x ldq] (ldq >= d) -> d_out_idx / d_out_val [n x k] (row ids best first, -1 /
+ *    0.0f padding): per query the k best of the rows of the nprobe lists whose centroids score best (ties to the
+ *    smaller list), each score bitwise that of bfl_serve_topk on the same rows and bias (use_bias), ties to the smaller
+ *    row id.  nprobe = nlist returns bfl_serve_topk's result.  nprobe in [1, nlist], and at most 4096 unless it is
+ *    nlist; k in [1, 4096].  The call synchronises `stream` first and returns when the results are written.
+ *  - attach: binds the handle to the current device (BFL_ERR_CUDA without a Hopper GPU); build and search attach too.
+ *  - set_batch_rows: queries per internal batch at most (0: chosen from the candidate scratch).
+ *  - info / read: the index's shape; HOST copies of the centroids [nlist x ld], the END offsets [nlist] and the row
+ *    ids [n] (each nullable).
+ *  One call at a time per handle.  The handle owns one stream and a serve handle over the centroids and starts no
+ *  thread; destroy releases all of it.  Argument errors are BFL_ERR_ARG, calls before a build BFL_ERR_STATE.
+ * ===================================================================================== */
+typedef struct bfl_ivf bfl_ivf_t;
+bfl_ivf_t* bfl_ivf_create(void);
+void bfl_ivf_destroy(bfl_ivf_t* h);
+int bfl_ivf_attach(bfl_ivf_t* h);
+int bfl_ivf_build_device(bfl_ivf_t* h, const float* d_rows, int64_t n, int ld, int d,
+                         const float* d_bias /* nullable */, int nlist, int iters, uint64_t seed);
+int bfl_ivf_search_device(bfl_ivf_t* h, const float* d_queries, int64_t n, int ldq, int nprobe, int k, int use_bias,
+                          int32_t* d_out_idx, float* d_out_val, void* stream);
+int bfl_ivf_set_batch_rows(bfl_ivf_t* h, int64_t rows);
+int bfl_ivf_info(bfl_ivf_t* h, int64_t* n, int* nlist, int* ld, int* d);
+int bfl_ivf_read(bfl_ivf_t* h, float* centroids /* nullable */, int64_t* offsets /* nullable */,
+                 int32_t* ids /* nullable */);
+
+/* =====================================================================================
  * Validation metrics on the device (DESIGN.md 4.8): the device path of Evaluable.get_validation_results
  * (buffalo/evaluate/base.py:44-148).  Device pointers, stream-ordered.  A "seen" CSR (END offsets, int32 keys, every
  * row non-decreasing) holds training rows; seen_row[q] names the row of query q.  The held-out CSR is indexed by user.
