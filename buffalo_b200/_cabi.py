@@ -118,6 +118,9 @@ PROTOTYPES = {
     "bfl_serve_topk_device": (C.c_int, [_vp, _vp, _i64, C.c_int, _vp, _vp, _vp]),
     "bfl_seen_topk": (C.c_int, [_vp, _vp, _i64, C.c_int, _vp, _vp, _vp, _vp]),
     "bfl_seen_topk_device": (C.c_int, [_vp, _vp, _i64, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "bfl_cand_topk": (C.c_int, [_vp, _vp, _i64, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "bfl_cand_topk_device": (C.c_int, [_vp, _vp, _i64, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "bfl_cand_set_budget": (C.c_int, [_vp, _i64]),
     # IVF index
     "bfl_ivf_create": (_vp, []),
     "bfl_ivf_destroy": (None, [_vp]),

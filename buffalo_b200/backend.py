@@ -606,24 +606,25 @@ class Serve(_Holder):
                                                 val.data_ptr(), _stream_ptr(stream)), "bfl_serve_topk_device")
         return idx, val
 
-    def _check_seen(self, n, seen_indptr, seen_keys, host):
-        """Argument checks of the seen rows: END offsets int64 [n], non-decreasing from 0, keys int32 in the items."""
+    def _check_seen(self, n, seen_indptr, seen_keys, host, what="seen"):
+        """Argument checks of the seen rows (or, what="cand", of the candidate lists): END offsets int64 [n],
+        non-decreasing from 0, keys int32 in the items."""
         check = _host if host else (lambda a, dt, nd, name: _dev(a, np.dtype(dt).name, name))
-        check(seen_indptr, np.int64, 1, "seen_indptr")
-        check(seen_keys, np.int32, 1, "seen_keys")
+        check(seen_indptr, np.int64, 1, what + "_indptr")
+        check(seen_keys, np.int32, 1, what + "_keys")
         if seen_indptr.shape[0] != n:
-            raise ValueError("seen_indptr must hold one END offset per query (%d), got %d" % (n, seen_indptr.shape[0]))
+            raise ValueError("%s_indptr must hold one END offset per query (%d), got %d" % (what, n, seen_indptr.shape[0]))
         ptr = seen_indptr if host else seen_indptr.cpu().numpy()
         nnz = int(ptr[-1]) if n else 0
         if n and (ptr[0] < 0 or (np.diff(ptr) < 0).any()):
-            raise ValueError("seen_indptr must be non-decreasing END offsets from 0")
+            raise ValueError("%s_indptr must be non-decreasing END offsets from 0" % what)
         if nnz > seen_keys.shape[0]:
-            raise ValueError("seen_indptr ends past the %d seen keys" % seen_keys.shape[0])
+            raise ValueError("%s_indptr ends past the %d %s keys" % (what, seen_keys.shape[0], what))
         if nnz:
             keys = seen_keys[:nnz]
             lo, hi = (int(keys.min()), int(keys.max())) if host else (int(keys.min().item()), int(keys.max().item()))
             if lo < 0 or hi >= self.num_items:
-                raise ValueError("seen key out of range [0, %d)" % self.num_items)
+                raise ValueError("%s key out of range [0, %d)" % (what, self.num_items))
         return nnz
 
     def topk_seen(self, query_idx, k, seen_indptr, seen_keys, want_scores=True):
@@ -675,6 +676,85 @@ class Serve(_Holder):
                 _dev(seen_row, "int32", "seen_row"), idx.data_ptr(), val.data_ptr(), _stream_ptr(stream)),
                 "bfl_seen_topk_device")
         return idx, val
+
+
+    def topk_candidates(self, query_idx, k, cand_indptr, cand_keys, seen=None, want_scores=True):
+        """topk where query i ranks only its own candidate list, row i of the host CSR (cand_indptr int64 END offsets
+        [n], cand_keys int32 item ids in any order, duplicates allowed) instead of the pool: row i is bitwise what topk
+        returns for query i alone with set_pool(its list), ties to the earlier list position.  seen: None or
+        (seen_indptr, seen_keys) as topk_seen takes them.  An empty list, or fewer than k candidates left, pads with
+        -1 / 0.0."""
+        k = self._check_k(k)
+        q = np.ascontiguousarray(query_idx, dtype=np.int32).reshape(-1)
+        if q.size and (q.min() < 0 or q.max() >= self.num_queries):
+            raise ValueError("query index out of range")
+        nc = self._check_seen(q.size, cand_indptr, cand_keys, host=True, what="cand")
+        ckeys = cand_keys if nc else np.zeros(1, np.int32)
+        sptr = skeys = None
+        if seen is not None:
+            sptr, skeys = seen
+            ns = self._check_seen(q.size, sptr, skeys, host=True)
+            skeys = skeys if ns else np.zeros(1, np.int32)
+        idx = np.empty((q.size, k), dtype=np.int32)
+        val = np.empty((q.size, k), dtype=np.float32) if want_scores else None
+        if q.size:
+            _cabi.check(self._lib.bfl_cand_topk(self._h, q.ctypes.data, q.size, k, cand_indptr.ctypes.data,
+                                                ckeys.ctypes.data, None if sptr is None else sptr.ctypes.data,
+                                                None if skeys is None else skeys.ctypes.data, idx.ctypes.data,
+                                                None if val is None else val.ctypes.data), "bfl_cand_topk")
+        return idx, val
+
+    def topk_candidates_device(self, query_idx, k, cand_indptr, cand_keys, cand_row=None, seen=None, stream=None):
+        """topk_candidates on torch CUDA tensors, stream-ordered: query q ranks row cand_row[q] (default q) of the
+        candidate CSR (int64 END offsets, int32 keys); seen: None or (seen_indptr, seen_keys[, seen_row]) as
+        topk_seen_device takes them (rows not in ascending order are sorted first).  Synchronises once per internal
+        batch."""
+        import torch
+        k = self._check_k(k)
+        n = query_idx.shape[0]
+        dev = query_idx.device
+        nc = self._check_seen(cand_indptr.shape[0], cand_indptr, cand_keys, host=False, what="cand")
+        ckeys = cand_keys[:nc] if nc else torch.zeros(1, dtype=torch.int32, device=dev)
+        cand_row = self._check_rows(cand_row, n, cand_indptr.shape[0], "cand")
+        sptr = skeys = srow = None
+        if seen is not None:
+            sptr, skeys = seen[0], seen[1]
+            srow = seen[2] if len(seen) > 2 else None
+            ns = self._check_seen(sptr.shape[0], sptr, skeys, host=False)
+            skeys = skeys[:ns] if ns else torch.zeros(1, dtype=torch.int32, device=dev)
+            if ns and eval_unsorted_rows(sptr, skeys, stream):
+                lens = torch.diff(sptr, prepend=sptr.new_zeros(1))
+                major = torch.repeat_interleave(torch.arange(sptr.shape[0], dtype=torch.int32, device=dev), lens)
+                sptr, skeys, _ = csr_from_triples_device(major, skeys, torch.ones(ns, dtype=torch.float32, device=dev),
+                                                         sptr.shape[0], self.num_items, stream=stream)
+            srow = self._check_rows(srow, n, sptr.shape[0], "seen")
+        idx = torch.empty((n, k), dtype=torch.int32, device=dev)
+        val = torch.empty((n, k), dtype=torch.float32, device=dev)
+        if n:
+            _cabi.check(self._lib.bfl_cand_topk_device(
+                self._h, _dev(query_idx, "int32", "query_idx"), n, k, cand_indptr.data_ptr(), ckeys.data_ptr(),
+                None if cand_row is None else cand_row.data_ptr(), None if sptr is None else sptr.data_ptr(),
+                None if skeys is None else skeys.data_ptr(), None if srow is None else srow.data_ptr(),
+                idx.data_ptr(), val.data_ptr(), _stream_ptr(stream)), "bfl_cand_topk_device")
+        return idx, val
+
+    @staticmethod
+    def _check_rows(row, n, rows, what):
+        """row: None (query q reads row q: the CSR needs n rows) or int32 CUDA [n] row numbers inside the CSR."""
+        if row is None:
+            if rows != n:
+                raise ValueError("without %s_row the %s CSR needs one row per query" % (what, what))
+            return None
+        _dev(row, "int32", what + "_row")
+        if row.shape[0] != n:
+            raise ValueError("%s_row must name one row per query" % what)
+        if n and (int(row.min().item()) < 0 or int(row.max().item()) >= rows):
+            raise ValueError("%s_row names a row outside the %s CSR" % (what, what))
+        return row
+
+    def _set_cand_budget(self, entries):
+        """Test hook: list entries per internal batch of topk_candidates (0: the default)."""
+        _cabi.check(self._lib.bfl_cand_set_budget(self._h, int(entries)), "bfl_cand_set_budget")
 
 
 def csr_from_triples_device(major, minor, vals, num_major, num_minor, sort_minor=True, stream=None):

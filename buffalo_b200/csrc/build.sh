@@ -9,6 +9,7 @@ SRCS="$HERE/bfl_common.cu $HERE/als.cu"
 [ -f "$HERE/topk.cu" ] && SRCS="$SRCS $HERE/topk.cu"
 [ -f "$HERE/serve.cu" ] && SRCS="$SRCS $HERE/serve.cu"
 [ -f "$HERE/ivf.cu" ] && SRCS="$SRCS $HERE/ivf.cu"
+[ -f "$HERE/candidates.cu" ] && SRCS="$SRCS $HERE/candidates.cu"
 [ -f "$HERE/evaluate.cu" ] && SRCS="$SRCS $HERE/evaluate.cu"
 [ -f "$HERE/ingest.cu" ] && SRCS="$SRCS $HERE/ingest.cu"
 [ -f "$HERE/plsi.cu" ] && SRCS="$SRCS $HERE/plsi.cu"

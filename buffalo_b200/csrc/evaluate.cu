@@ -20,65 +20,6 @@ constexpr unsigned long long EV_EMPTY = SEEN_EMPTY;
 constexpr int EV_SUM_BLOCKS = 128;
 constexpr int EV_SUM_WIDTH = 8;
 
-struct KeySel {
-    unsigned int hist[256];
-    unsigned long long prefix;
-    unsigned int kk, cnt;
-    int stop;
-};
-
-// The k smallest of the keys get(0..n) that are not EV_EMPTY (n_valid of them, all distinct) -> out[0..min(k, n_valid))
-// in no particular order; returns that count.  MSB-first radix select over 8-bit digits, stopping as soon as the
-// remaining bin is taken whole.  All threads of the CTA (TK_THREADS) call it.
-template <class Get>
-__device__ int select_smallest(Get get, int64_t n, int64_t n_valid, int k, unsigned long long* out, KeySel& sc) {
-    const int tid = threadIdx.x, lane = tid & 31;
-    unsigned long long prefix = 0, mask = 0;
-    if (n_valid > k) {
-        if (tid == 0) sc.kk = (unsigned)k;
-        for (int shift = 56; shift >= 0; shift -= 8) {
-            sc.hist[tid] = 0;
-            __syncthreads();
-            for (int64_t i = tid; i < n; i += TK_THREADS) {
-                const unsigned long long key = get(i);
-                if (key != EV_EMPTY && (key & mask) == prefix) atomicAdd(&sc.hist[(unsigned)(key >> shift) & 255u], 1u);
-            }
-            __syncthreads();
-            if (tid == 0) {
-                const unsigned kk = sc.kk;
-                unsigned cum = 0;
-                int b = 0;
-                for (; b < 255; ++b) {
-                    if (cum + sc.hist[b] >= kk) break;
-                    cum += sc.hist[b];
-                }
-                sc.kk = kk - cum;
-                sc.stop = sc.hist[b] == kk - cum;
-                sc.prefix = prefix | ((unsigned long long)b << shift);
-            }
-            __syncthreads();
-            prefix = sc.prefix;
-            mask |= 255ull << shift;
-            if (sc.stop) break;
-        }
-    }
-    // every key whose digits so far are at most the selected ones: exactly min(k, n_valid) keys
-    if (tid == 0) sc.cnt = 0;
-    __syncthreads();
-    for (int64_t i0 = 0; i0 < n; i0 += TK_THREADS) {
-        const int64_t i = i0 + tid;
-        const unsigned long long key = i < n ? get(i) : EV_EMPTY;
-        const bool take = key != EV_EMPTY && (key & mask) <= prefix;
-        const unsigned bal = __ballot_sync(FULL, take);
-        unsigned base = 0;
-        if (lane == 0 && bal) base = atomicAdd(&sc.cnt, (unsigned)__popc(bal));
-        base = __shfl_sync(FULL, base, 0);
-        if (take) out[base + __popc(bal & ((1u << lane) - 1u))] = key;
-    }
-    __syncthreads();
-    return n_valid > k ? k : (int)n_valid;
-}
-
 __global__ void __launch_bounds__(TK_THREADS) eval_slice_kernel(
     const float* __restrict__ Qr, int64_t nq, int ldq, const float* __restrict__ It, int64_t n_items, int ldi,
     const float* __restrict__ bias, int d, int k, int nslices, const int64_t* __restrict__ seen_indptr,

@@ -26,6 +26,7 @@ using namespace bfl;
 namespace {
 
 constexpr int64_t SV_SEEN_KEYS = (int64_t)1 << 24;  // seen keys per internal batch aimed at (a longer row is a batch)
+constexpr int64_t SV_CAND_LIST = (int64_t)1 << 24;  // list entries per internal batch of bfl_cand_topk (likewise)
 
 // A seen CSR on the device (END offsets, every row non-decreasing); query q of a batch reads row row[q], or row q.
 struct SeenRows {
@@ -247,6 +248,16 @@ struct bfl_serve {
     int64_t* pin_sp[2] = {nullptr, nullptr};
     int32_t* pin_sk[2] = {nullptr, nullptr};
     size_t pin_sp_cap = 0, pin_sk_cap = 0;
+    // candidate-list calls (candidates.cu): the batch's lists as uploaded (cp / ck, staged through their own two pinned
+    // slots), the work list (unit_end / key_end); the rank keys and counts go to cand_k / cand_cnt
+    DevBuf<int64_t> cp;
+    DevBuf<int32_t> ck;
+    DevBuf<long long> unit_end, key_end;
+    cudaEvent_t cstaged[2] = {nullptr, nullptr};
+    int64_t* pin_cp[2] = {nullptr, nullptr};
+    int32_t* pin_ck[2] = {nullptr, nullptr};
+    size_t pin_cp_cap = 0, pin_ck_cap = 0;
+    int64_t cand_budget = 0;                        // list entries per batch; 0: SV_CAND_LIST
 
     int attach() {
         if (compute) return BFL_OK;
@@ -260,6 +271,7 @@ struct bfl_serve {
             BFL_CUDA(cudaEventCreateWithFlags(&scored[s], cudaEventDisableTiming));
             BFL_CUDA(cudaEventCreateWithFlags(&copied[s], cudaEventDisableTiming));
             BFL_CUDA(cudaEventCreateWithFlags(&staged[s], cudaEventDisableTiming));
+            BFL_CUDA(cudaEventCreateWithFlags(&cstaged[s], cudaEventDisableTiming));
         }
         return BFL_OK;
     }
@@ -284,34 +296,40 @@ struct bfl_serve {
     }
     // the two pinned slots the seen rows of a batch are staged in: rows END offsets and n_keys keys each
     int reserve_seen_pinned(size_t rows, size_t n_keys) {
-        if (rows <= pin_sp_cap && n_keys <= pin_sk_cap) return BFL_OK;
-        release_seen_pinned();
+        return reserve_rows_pinned(rows, n_keys, pin_sp, pin_sk, pin_sp_cap, pin_sk_cap);
+    }
+    void release_seen_pinned() { release_rows_pinned(pin_sp, pin_sk, pin_sp_cap, pin_sk_cap); }
+    static int reserve_rows_pinned(size_t rows, size_t n_keys, int64_t** pp, int32_t** pk, size_t& cap_p, size_t& cap_k) {
+        if (rows <= cap_p && n_keys <= cap_k) return BFL_OK;
+        release_rows_pinned(pp, pk, cap_p, cap_k);
         for (int s = 0; s < 2; ++s) {
-            BFL_CUDA(cudaMallocHost(&pin_sp[s], rows * sizeof(int64_t)));
-            BFL_CUDA(cudaMallocHost(&pin_sk[s], n_keys * sizeof(int32_t)));
+            BFL_CUDA(cudaMallocHost(&pp[s], rows * sizeof(int64_t)));
+            BFL_CUDA(cudaMallocHost(&pk[s], n_keys * sizeof(int32_t)));
         }
-        pin_sp_cap = rows;
-        pin_sk_cap = n_keys;
+        cap_p = rows;
+        cap_k = n_keys;
         return BFL_OK;
     }
-    void release_seen_pinned() {
+    static void release_rows_pinned(int64_t** pp, int32_t** pk, size_t& cap_p, size_t& cap_k) {
         for (int s = 0; s < 2; ++s) {
-            if (pin_sp[s]) cudaFreeHost(pin_sp[s]);
-            if (pin_sk[s]) cudaFreeHost(pin_sk[s]);
-            pin_sp[s] = nullptr;
-            pin_sk[s] = nullptr;
+            if (pp[s]) cudaFreeHost(pp[s]);
+            if (pk[s]) cudaFreeHost(pk[s]);
+            pp[s] = nullptr;
+            pk[s] = nullptr;
         }
-        pin_sp_cap = pin_sk_cap = 0;
+        cap_p = cap_k = 0;
     }
     ~bfl_serve() {
         if (compute) cudaStreamSynchronize(compute);
         if (copy) cudaStreamSynchronize(copy);
         release_pinned();
         release_seen_pinned();
+        release_rows_pinned(pin_cp, pin_ck, pin_cp_cap, pin_ck_cap);
         for (int s = 0; s < 2; ++s) {
             if (scored[s]) cudaEventDestroy(scored[s]);
             if (copied[s]) cudaEventDestroy(copied[s]);
             if (staged[s]) cudaEventDestroy(staged[s]);
+            if (cstaged[s]) cudaEventDestroy(cstaged[s]);
         }
         if (compute) cudaStreamDestroy(compute);
         if (copy) cudaStreamDestroy(copy);
@@ -354,9 +372,19 @@ struct bfl_serve {
     // leaves out the items of its row
     int run_batch(const int32_t* d_qidx, int64_t nb, int k, int32_t* d_out_i, float* d_out_v, cudaStream_t st,
                   const SeenRows* seen = nullptr);
-    // the host-array call of bfl_serve_topk and bfl_seen_topk (seen_indptr == nullptr: no seen rows)
+    // one batch of candidate-list queries, stream-ordered: query q of the batch ranks its list (row q of `cand`) ->
+    // d_out_i / d_out_v [nb x k]; n_units / n_keys: the batch's work-list totals, or -1 to read them back (synchronises)
+    int run_cand_batch(const int32_t* d_qidx, int64_t nb, int k, const CandRows& cand, const CandRows* seen,
+                       long long n_units, long long n_keys, int32_t* d_out_i, float* d_out_v, cudaStream_t st);
+    // the host-array call of bfl_serve_topk, bfl_seen_topk (seen_indptr == nullptr: no seen rows) and bfl_cand_topk
+    // (cand_indptr != nullptr: row i of the host CSR is query i's candidate list)
     int topk_host(const int32_t* query_idx, int64_t n, int k, int32_t* out_idx, float* out_val,
-                  const int64_t* seen_indptr, const int32_t* seen_keys);
+                  const int64_t* seen_indptr, const int32_t* seen_keys, const int64_t* cand_indptr = nullptr,
+                  const int32_t* cand_keys = nullptr);
+    // uploads the rows [r0, r0 + nb) of a host CSR through pinned slot s (pin_p / pin_k, released by event ev) into
+    // dp / dk, offsets from 0, on `compute`
+    int upload_rows(const int64_t* indptr, const int32_t* keys, int64_t r0, int64_t nb, int64_t* pin_p, int32_t* pin_k,
+                    cudaEvent_t ev, DevBuf<int64_t>& dp, DevBuf<int32_t>& dk);
     // uploads the seen rows [r0, r0 + nb) of a host CSR through pinned slot s; sorts them on the device when unsorted
     int stage_seen(const int64_t* indptr, const int32_t* keys, int64_t r0, int64_t nb, bool unsorted, int s,
                    SeenRows* out);
@@ -430,17 +458,40 @@ int bfl_serve::run_batch(const int32_t* d_qidx, int64_t nb, int k, int32_t* d_ou
     return BFL_OK;
 }
 
+int bfl_serve::run_cand_batch(const int32_t* d_qidx, int64_t nb, int k, const CandRows& cand, const CandRows* seen,
+                              long long n_units, long long n_keys, int32_t* d_out_i, float* d_out_v, cudaStream_t st) {
+    if (BFL_OK != unit_end.reserve((size_t)nb) || BFL_OK != key_end.reserve((size_t)nb)) return BFL_ERR_CUDA;
+    if (int rc = cand_plan(cand, nb, k, unit_end.p, key_end.p, st)) return rc;
+    if (n_units < 0) {
+        BFL_CUDA(cudaMemcpyAsync(&n_units, unit_end.p + nb - 1, sizeof(long long), cudaMemcpyDeviceToHost, st));
+        BFL_CUDA(cudaMemcpyAsync(&n_keys, key_end.p + nb - 1, sizeof(long long), cudaMemcpyDeviceToHost, st));
+        BFL_CUDA(cudaStreamSynchronize(st));
+    }
+    if (BFL_OK != cand_k.reserve((size_t)std::max(n_keys, 1ll)) || BFL_OK != cand_cnt.reserve((size_t)std::max(n_units, 1ll)))
+        return BFL_ERR_CUDA;
+    return cand_batch(queries, n_q, ldq, d_qidx, nb, items, ldi, bias, d, k, cand,
+                      seen ? *seen : CandRows{nullptr, nullptr, nullptr, 0}, unit_end.p, key_end.p, n_units, cand_k.p,
+                      cand_cnt.p, d_out_i, d_out_v, st);
+}
+
+int bfl_serve::upload_rows(const int64_t* indptr, const int32_t* keys, int64_t r0, int64_t nb, int64_t* pin_p,
+                           int32_t* pin_k, cudaEvent_t ev, DevBuf<int64_t>& dp, DevBuf<int32_t>& dk) {
+    const int64_t kb = r0 > 0 ? indptr[r0 - 1] : 0, nk = indptr[r0 + nb - 1] - kb;
+    // the slot was last read by the upload of the batch before the previous one
+    BFL_CUDA(cudaEventSynchronize(ev));
+    memcpy(pin_k, keys + kb, sizeof(int32_t) * (size_t)nk);
+    for (int64_t i = 0; i < nb; ++i) pin_p[i] = indptr[r0 + i] - kb;
+    if (BFL_OK != dp.reserve((size_t)nb) || BFL_OK != dk.reserve((size_t)(nk > 0 ? nk : 1))) return BFL_ERR_CUDA;
+    BFL_CUDA(cudaMemcpyAsync(dp.p, pin_p, sizeof(int64_t) * (size_t)nb, cudaMemcpyHostToDevice, compute));
+    BFL_CUDA(cudaMemcpyAsync(dk.p, pin_k, sizeof(int32_t) * (size_t)nk, cudaMemcpyHostToDevice, compute));
+    BFL_CUDA(cudaEventRecord(ev, compute));
+    return BFL_OK;
+}
+
 int bfl_serve::stage_seen(const int64_t* indptr, const int32_t* keys, int64_t r0, int64_t nb, bool unsorted, int s,
                           SeenRows* out) {
-    const int64_t kb = r0 > 0 ? indptr[r0 - 1] : 0, nk = indptr[r0 + nb - 1] - kb;
-    // slot s was last read by the upload of the batch before the previous one
-    BFL_CUDA(cudaEventSynchronize(staged[s]));
-    memcpy(pin_sk[s], keys + kb, sizeof(int32_t) * (size_t)nk);
-    for (int64_t i = 0; i < nb; ++i) pin_sp[s][i] = indptr[r0 + i] - kb;
-    if (BFL_OK != sp.reserve((size_t)nb) || BFL_OK != sk.reserve((size_t)(nk > 0 ? nk : 1))) return BFL_ERR_CUDA;
-    BFL_CUDA(cudaMemcpyAsync(sp.p, pin_sp[s], sizeof(int64_t) * (size_t)nb, cudaMemcpyHostToDevice, compute));
-    BFL_CUDA(cudaMemcpyAsync(sk.p, pin_sk[s], sizeof(int32_t) * (size_t)nk, cudaMemcpyHostToDevice, compute));
-    BFL_CUDA(cudaEventRecord(staged[s], compute));
+    if (int rc = upload_rows(indptr, keys, r0, nb, pin_sp[s], pin_sk[s], staged[s], sp, sk)) return rc;
+    const int64_t nk = indptr[r0 + nb - 1] - (r0 > 0 ? indptr[r0 - 1] : 0);
     *out = SeenRows{sp.p, sk.p, nullptr};
     if (!unsorted) return BFL_OK;
     // rows in session order (or with duplicates out of place): the device radix sort of the ingest path, by (row, key)
@@ -459,13 +510,15 @@ int bfl_serve::stage_seen(const int64_t* indptr, const int32_t* keys, int64_t r0
 }
 
 int bfl_serve::topk_host(const int32_t* query_idx, int64_t n, int k, int32_t* out_idx, float* out_val,
-                         const int64_t* seen_indptr, const int32_t* seen_keys) {
+                         const int64_t* seen_indptr, const int32_t* seen_keys, const int64_t* cand_indptr,
+                         const int32_t* cand_keys) {
     int rc = BFL_OK;
-    // batches of at most batch_rows(k) queries; with seen rows also of at most SV_SEEN_KEYS seen keys, unless a single
-    // row holds more (it is then a batch of its own)
+    // batches of at most batch_rows(k) queries; with seen rows also of at most SV_SEEN_KEYS seen keys, with candidate
+    // lists of at most cand_budget list entries, unless a single row holds more (it is then a batch of its own)
     const int64_t B = batch_rows(k) < n ? batch_rows(k) : n;
+    const int64_t list_budget = cand_budget > 0 ? cand_budget : SV_CAND_LIST;
     std::vector<int64_t> start{0};
-    int64_t max_keys = 1;
+    int64_t max_keys = 1, max_list = 1;
     while (start.back() < n) {
         const int64_t b0 = start.back();
         int64_t e = n - b0 < B ? n : b0 + B;
@@ -474,9 +527,27 @@ int bfl_serve::topk_host(const int32_t* query_idx, int64_t n, int k, int32_t* ou
             e = std::max<int64_t>(b0 + 1, std::upper_bound(seen_indptr + b0, seen_indptr + e, kb + SV_SEEN_KEYS) - seen_indptr);
             max_keys = std::max<int64_t>(max_keys, seen_indptr[e - 1] - kb);
         }
+        if (cand_indptr) {
+            const int64_t cb = b0 > 0 ? cand_indptr[b0 - 1] : 0;
+            e = std::max<int64_t>(b0 + 1, std::upper_bound(cand_indptr + b0, cand_indptr + e, cb + list_budget) - cand_indptr);
+            max_list = std::max<int64_t>(max_list, cand_indptr[e - 1] - cb);
+        }
         start.push_back(e);
     }
     const int64_t nbatch = (int64_t)start.size() - 1;
+    // the work-list totals of each batch of candidate lists (as cand_units_kernel counts them)
+    std::vector<long long> n_units(cand_indptr ? nbatch : 0, 0), n_keys(cand_indptr ? nbatch : 0, 0);
+    long long max_units = 1, max_rank_keys = 1;
+    for (int64_t b = 0; b < (int64_t)n_units.size(); ++b) {
+        for (int64_t r = start[b]; r < start[b + 1]; ++r) {
+            const int64_t len = cand_indptr[r] - (r > 0 ? cand_indptr[r - 1] : 0);
+            const int64_t full = len / SV_SLICE, rest = len - full * SV_SLICE;
+            n_units[b] += full + (rest > 0);
+            n_keys[b] += full * std::min(k, SV_SLICE) + std::min<int64_t>(k, rest);
+        }
+        max_units = std::max(max_units, n_units[b]);
+        max_rank_keys = std::max(max_rank_keys, n_keys[b]);
+    }
     // batches holding a row that is not non-decreasing are sorted on the device
     std::vector<char> unsorted(seen_indptr ? nbatch : 0, 0);
     bool any_unsorted = false;
@@ -500,6 +571,11 @@ int bfl_serve::topk_host(const int32_t* query_idx, int64_t n, int k, int32_t* ou
     if (any_unsorted && (BFL_OK != sorted_sp.reserve((size_t)B) || BFL_OK != sorted_sk.reserve((size_t)max_keys) ||
                          BFL_OK != sort_major.reserve((size_t)max_keys) || BFL_OK != sort_vals.reserve((size_t)max_keys)))
         return BFL_ERR_CUDA;
+    if (cand_indptr && (BFL_OK != reserve_rows_pinned((size_t)B, (size_t)max_list, pin_cp, pin_ck, pin_cp_cap, pin_ck_cap) ||
+                        BFL_OK != cp.reserve((size_t)B) || BFL_OK != ck.reserve((size_t)max_list) ||
+                        BFL_OK != unit_end.reserve((size_t)B) || BFL_OK != key_end.reserve((size_t)B) ||
+                        BFL_OK != cand_k.reserve((size_t)max_rank_keys) || BFL_OK != cand_cnt.reserve((size_t)max_units)))
+        return BFL_ERR_CUDA;
     BFL_CUDA(cudaMemcpyAsync(qidx.p, query_idx, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, compute));
     // batch b is scored on `compute` into slot b & 1 and copied to that slot's pinned buffers on `copy`; the host
     // drains batch b - 1 into the caller's arrays (and stages the seen rows of batch b + 1) while batch b runs
@@ -516,7 +592,15 @@ int bfl_serve::topk_host(const int32_t* query_idx, int64_t n, int k, int32_t* ou
         const int64_t b0 = start[b], nb = start[b + 1] - b0;
         SeenRows seen{};
         if (seen_indptr) rc = stage_seen(seen_indptr, seen_keys, b0, nb, unsorted[b] != 0, s, &seen);
-        if (rc == BFL_OK) rc = run_batch(qidx.p + b0, nb, k, out_i[s].p, out_v[s].p, compute, seen_indptr ? &seen : nullptr);
+        if (rc == BFL_OK && cand_indptr) {
+            rc = upload_rows(cand_indptr, cand_keys, b0, nb, pin_cp[s], pin_ck[s], cstaged[s], cp, ck);
+            const CandRows cand{cp.p, ck.p, nullptr, 0}, cseen{seen.indptr, seen.keys, nullptr, 0};
+            if (rc == BFL_OK)
+                rc = run_cand_batch(qidx.p + b0, nb, k, cand, seen_indptr ? &cseen : nullptr, n_units[b], n_keys[b],
+                                    out_i[s].p, out_v[s].p, compute);
+        } else if (rc == BFL_OK) {
+            rc = run_batch(qidx.p + b0, nb, k, out_i[s].p, out_v[s].p, compute, seen_indptr ? &seen : nullptr);
+        }
         if (rc == BFL_OK) {
             BFL_CUDA(cudaEventRecord(scored[s], compute));
             BFL_CUDA(cudaStreamWaitEvent(copy, scored[s], 0));
@@ -661,22 +745,35 @@ int bfl_serve_topk(bfl_serve_t* h, const int32_t* query_idx, int64_t n, int k, i
     return h->topk_host(query_idx, n, k, out_idx, out_val, nullptr, nullptr);
 }
 
+// n rows of a host CSR of item ids ("seen" or "candidate" rows): END offsets non-decreasing from 0, keys in the items
+static int check_rows(const bfl_serve_t* h, const int64_t* indptr, const int32_t* keys, int64_t n, const char* what) {
+    const std::string w(what);
+    if (!indptr) BFL_FAIL(BFL_ERR_ARG, "serve: the " + w + " rows need their END offsets");
+    int64_t prev = 0;
+    for (int64_t i = 0; i < n; ++i) {
+        if (indptr[i] < prev) BFL_FAIL(BFL_ERR_ARG, "serve: " + w + " END offsets must be non-decreasing from 0");
+        prev = indptr[i];
+    }
+    if (prev > 0 && !keys) BFL_FAIL(BFL_ERR_ARG, "serve: " + w + " keys missing");
+    for (int64_t e = 0; e < prev; ++e)
+        if (keys[e] < 0 || keys[e] >= h->n_items) BFL_FAIL(BFL_ERR_ARG, "serve: " + w + " key out of range");
+    return BFL_OK;
+}
+
+static int check_query_idx(const bfl_serve_t* h, const int32_t* query_idx, int64_t n) {
+    for (int64_t i = 0; i < n; ++i)
+        if (query_idx[i] < 0 || query_idx[i] >= h->n_q) BFL_FAIL(BFL_ERR_ARG, "serve: query index out of range");
+    return BFL_OK;
+}
+
 int bfl_seen_topk(bfl_serve_t* h, const int32_t* query_idx, int64_t n, int k, const int64_t* seen_indptr,
                   const int32_t* seen_keys, int32_t* out_idx, float* out_val) {
     if (!h) BFL_FAIL(BFL_ERR_ARG, "serve: null handle");
     int rc = h->check_ready(n, k, query_idx, out_idx);
     if (rc != BFL_OK) return rc;
     if (!seen_indptr) BFL_FAIL(BFL_ERR_ARG, "serve: the seen rows need their END offsets");
-    for (int64_t i = 0; i < n; ++i)
-        if (query_idx[i] < 0 || query_idx[i] >= h->n_q) BFL_FAIL(BFL_ERR_ARG, "serve: query index out of range");
-    int64_t prev = 0;
-    for (int64_t i = 0; i < n; ++i) {
-        if (seen_indptr[i] < prev) BFL_FAIL(BFL_ERR_ARG, "serve: seen END offsets must be non-decreasing from 0");
-        prev = seen_indptr[i];
-    }
-    if (prev > 0 && !seen_keys) BFL_FAIL(BFL_ERR_ARG, "serve: seen keys missing");
-    for (int64_t e = 0; e < prev; ++e)
-        if (seen_keys[e] < 0 || seen_keys[e] >= h->n_items) BFL_FAIL(BFL_ERR_ARG, "serve: seen key out of range");
+    if (BFL_OK != check_query_idx(h, query_idx, n) || BFL_OK != check_rows(h, seen_indptr, seen_keys, n, "seen"))
+        return BFL_ERR_ARG;
     return h->topk_host(query_idx, n, k, out_idx, out_val, seen_indptr, seen_keys);
 }
 
@@ -695,6 +792,45 @@ int bfl_seen_topk_device(bfl_serve_t* h, const int32_t* d_query_idx, int64_t n, 
         rc = h->run_batch(d_query_idx + b0, nb, k, d_out_idx + b0 * k, d_out_val + b0 * k, (cudaStream_t)stream, &seen);
         if (rc != BFL_OK) return rc;
     }
+    return BFL_OK;
+}
+
+int bfl_cand_topk(bfl_serve_t* h, const int32_t* query_idx, int64_t n, int k, const int64_t* cand_indptr,
+                  const int32_t* cand_keys, const int64_t* seen_indptr, const int32_t* seen_keys, int32_t* out_idx,
+                  float* out_val) {
+    if (!h) BFL_FAIL(BFL_ERR_ARG, "serve: null handle");
+    int rc = h->check_ready(n, k, query_idx, out_idx);
+    if (rc != BFL_OK) return rc;
+    if (BFL_OK != check_query_idx(h, query_idx, n) || BFL_OK != check_rows(h, cand_indptr, cand_keys, n, "candidate") ||
+        (seen_indptr && BFL_OK != check_rows(h, seen_indptr, seen_keys, n, "seen")))
+        return BFL_ERR_ARG;
+    return h->topk_host(query_idx, n, k, out_idx, out_val, seen_indptr, seen_keys, cand_indptr, cand_keys);
+}
+
+int bfl_cand_topk_device(bfl_serve_t* h, const int32_t* d_query_idx, int64_t n, int k, const int64_t* d_cand_indptr,
+                         const int32_t* d_cand_keys, const int32_t* d_cand_row, const int64_t* d_seen_indptr,
+                         const int32_t* d_seen_keys, const int32_t* d_seen_row, int32_t* d_out_idx, float* d_out_val,
+                         void* stream) {
+    if (!h) BFL_FAIL(BFL_ERR_ARG, "serve: null handle");
+    int rc = h->check_ready(n, k, d_query_idx, d_out_idx);
+    if (rc != BFL_OK) return rc;
+    if (!d_cand_indptr || !d_cand_keys) BFL_FAIL(BFL_ERR_ARG, "serve: bad candidate rows");
+    if (d_seen_indptr && !d_seen_keys) BFL_FAIL(BFL_ERR_ARG, "serve: bad seen rows");
+    const int64_t B = h->batch_rows(k);
+    for (int64_t b0 = 0; b0 < n; b0 += B) {
+        const int64_t nb = n - b0 < B ? n - b0 : B;
+        const CandRows cand{d_cand_indptr, d_cand_keys, d_cand_row ? d_cand_row + b0 : nullptr, b0};
+        const CandRows seen{d_seen_indptr, d_seen_keys, d_seen_row ? d_seen_row + b0 : nullptr, b0};
+        rc = h->run_cand_batch(d_query_idx + b0, nb, k, cand, d_seen_indptr ? &seen : nullptr, -1, -1,
+                               d_out_idx + b0 * k, d_out_val ? d_out_val + b0 * k : nullptr, (cudaStream_t)stream);
+        if (rc != BFL_OK) return rc;
+    }
+    return BFL_OK;
+}
+
+int bfl_cand_set_budget(bfl_serve_t* h, int64_t list_entries) {
+    if (!h || list_entries < 0) BFL_FAIL(BFL_ERR_ARG, "serve: bad candidate budget");
+    h->cand_budget = list_entries;
     return BFL_OK;
 }
 

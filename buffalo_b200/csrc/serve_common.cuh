@@ -210,4 +210,22 @@ namespace bfl {
 // [0, n_src) gives a zero row), stream-ordered; serve.cu
 int serve_gather_rows(const float* src, int64_t n_src, int ld, const int32_t* idx, int64_t n, int d, float* dst,
                       cudaStream_t st);
+
+// A device CSR of END offsets read per query: query q of a batch reads row row[q], or row base + q without `row`.
+struct CandRows {
+    const int64_t* indptr;
+    const int32_t* keys;
+    const int32_t* row;
+    int64_t base;
+};
+// candidates.cu, stream-ordered.  cand_plan: the work list of a batch of nb queries with candidate lists `cand`:
+// unit_end / key_end [nb] become the inclusive sums of each query's units (slices of up to 1024 list positions) and of
+// its rank-key slots.  cand_batch: per query q, the k best of its list (scores and ties of bfl_serve_topk with the list
+// as the pool), without the items of its sorted seen row when seen.indptr is set -> out_idx (item ids, -1 pads) /
+// out_val (nullable; 0.0f pads) [nb x k].  cand_key / cand_cnt hold key_end[nb - 1] keys and n_units counts.
+int cand_plan(CandRows cand, int64_t nb, int k, long long* unit_end, long long* key_end, cudaStream_t st);
+int cand_batch(const float* queries, int64_t n_q, int ldq, const int32_t* qidx, int64_t nb, const float* items, int ldi,
+               const float* bias, int d, int k, CandRows cand, CandRows seen, const long long* unit_end,
+               const long long* key_end, long long n_units, unsigned long long* cand_key, int32_t* cand_cnt,
+               int32_t* out_idx, float* out_val, cudaStream_t st);
 }  // namespace bfl

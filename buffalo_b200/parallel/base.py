@@ -55,6 +55,31 @@ def _topn_unseen(scores, num_items, pool, topk, seen_indptr, seen_keys, out_keys
     out_scores[:, :k] = np.where(valid, np.take_along_axis(scores, order, axis=1), 0)
 
 
+def cand_topn(indexes, P, Q, Qb, topk, cand_indptr, cand_keys, seen_indptr=None, seen_keys=None):
+    """dot_topn over a candidate list per query: row i ranks only the items of row i of the CSR (END offsets), in list
+    order, ties to the earlier position; with seen rows (a CSR of END offsets, row i per query) those items are left
+    out.  (keys int32, scores float32) [n, topk], -1 / 0 padded; an empty list gives a padded row."""
+    n = len(indexes)
+    keys = np.full((n, topk), -1, dtype=np.int32)
+    scores = np.zeros((n, topk), dtype=np.float32)
+    cand_indptr = np.asarray(cand_indptr, dtype=np.int64)
+    for i, u in enumerate(indexes):
+        pool = np.asarray(cand_keys[(cand_indptr[i - 1] if i else 0):cand_indptr[i]], dtype=np.int64)
+        if not pool.size:
+            continue
+        s = P[[u]].dot(Q[pool].T)[0]
+        if Qb is not None and Qb.size:
+            s = s + Qb.reshape(-1)[pool]
+        order = np.argsort(-s, kind="stable")
+        if seen_indptr is not None:
+            row = seen_keys[(seen_indptr[i - 1] if i else 0):seen_indptr[i]]
+            order = order[~np.isin(pool[order], row)]
+        order = order[:topk]
+        keys[i, :len(order)] = pool[order]
+        scores[i, :len(order)] = s[order]
+    return keys, scores
+
+
 class Parallel(object):
     def __init__(self, algo, *argv, **kwargs):
         self.algo = algo
@@ -88,16 +113,19 @@ class Parallel(object):
             self._serve_key = key
         return self._serve
 
+    @staticmethod
+    def _on_device(indexes, A, B, topk):
+        # On the device when one is present and the call is within the kernels' limits.  The items must fit in device
+        # memory next to the gathered query rows: an allocation failure is an error, not a silent switch to NumPy.
+        return (backend.device_available() and len(indexes) and 0 < topk <= backend.SERVE_KMAX
+                and B.shape[0] < 2 ** 31
+                and all(x.dtype == np.float32 and x.flags["C_CONTIGUOUS"] for x in (A, B)))
+
     def _run(self, indexes, A, B, Bb, topk, pool, seen=None):
         """seen: None, or (END offsets int64, keys int32) whose row i holds the items query indexes[i] must not get."""
         if Bb is not None and not Bb.size:
             Bb = None
-        # On the device when one is present and the call is within the kernels' limits.  The items must fit in device
-        # memory next to the gathered query rows: an allocation failure is an error, not a silent switch to NumPy.
-        on_device = (backend.device_available() and len(indexes) and 0 < topk <= backend.SERVE_KMAX
-                     and B.shape[0] < 2 ** 31
-                     and all(x.dtype == np.float32 and x.flags["C_CONTIGUOUS"] for x in (A, B)))
-        if on_device:
+        if self._on_device(indexes, A, B, topk):
             h = self._serve_handle(B, None if Bb is None else np.ascontiguousarray(Bb, dtype=np.float32))
             # only the rows asked for go to the device, read from the live array at every call
             h.set_queries(np.ascontiguousarray(A[indexes]))
@@ -112,6 +140,17 @@ class Parallel(object):
         else:
             dot_topn(indexes, A, B, Bb, keys, scores, pool, topk, self.num_workers)
         return keys, scores
+
+    def _run_cands(self, indexes, A, B, Bb, topk, cands, seen=None):
+        """_run with a candidate list per query instead of one pool: cands (END offsets int64, keys int32) whose row i
+        lists the items query indexes[i] ranks."""
+        if Bb is not None and not Bb.size:
+            Bb = None
+        if self._on_device(indexes, A, B, topk):
+            h = self._serve_handle(B, None if Bb is None else np.ascontiguousarray(Bb, dtype=np.float32))
+            h.set_queries(np.ascontiguousarray(A[indexes]))
+            return h.topk_candidates(np.arange(len(indexes), dtype=np.int32), topk, *cands, seen=seen)
+        return cand_topn(indexes, A, B, Bb, topk, *cands, *(seen or ()))
 
 
 class ParALS(Parallel):
@@ -192,6 +231,19 @@ class ParALS(Parallel):
             topks = [[names[t] for t in tt if t != -1] for tt in topks]
         return topks, scores
 
+    @staticmethod
+    def _pool_matrix(pool, rows, num_items):
+        """(END offsets int64, keys int32) of a scipy sparse (rows, num_items) candidate matrix as tocsr() stores it:
+        every row's columns in stored order, duplicates kept, values ignored.  Checks the shape and the columns."""
+        m = pool.tocsr()
+        if m.shape != (rows, num_items):
+            raise ValueError("pool must be a (%d, %d) matrix, got %s" % (rows, num_items, m.shape))
+        nnz = int(m.indptr[-1])
+        keys = np.asarray(m.indices[:nnz])
+        if keys.size and (int(keys.min()) < 0 or int(keys.max()) >= num_items):
+            raise ValueError("pool holds a column outside [0, %d)" % num_items)
+        return np.asarray(m.indptr[1:], dtype=np.int64), np.ascontiguousarray(keys, dtype=np.int32)
+
     def _seen_rows(self, idx, exclude_seen):
         """(END offsets int64, keys int32) of the seen rows of users idx: rows of the algo's training data ("rowwise"
         group) for exclude_seen=True, of a scipy sparse (num_users, num_items) matrix otherwise."""
@@ -216,10 +268,14 @@ class ParALS(Parallel):
         return _gather_rows(ends, keys, idx)
 
     def topk_recommendation(self, keys, topk=10, pool=None, repr=False, exclude_seen=False, nprobe=None):
-        """exclude_seen: False; True to leave out each user's training items (the "rowwise" rows of the algo's data);
-        or a scipy sparse (num_users, num_items) matrix whose row u lists the items user u does not get back.  Rows
-        left with fewer than topk candidates are padded with -1 / 0.0.  nprobe: None ranks every item; an integer in
-        [1, nlist] searches the item index (build_index) and ranks the items of the nprobe lists nearest each user,
+        """pool: None ranks every item; a list of item ids (or an index array) is one candidate pool for every user; a
+        scipy sparse (num_users, num_items) matrix gives each user its own candidates, row u (as tocsr() stores it,
+        values ignored, duplicates kept, ties to the earlier entry): a user's row of the result is then what a call
+        with that user alone and that row as the pool returns.  An empty row gives a row of -1 / 0.0; topk must be in
+        [1, 4096].  exclude_seen: False; True to leave out each user's training items (the "rowwise" rows of the algo's
+        data); or a scipy sparse (num_users, num_items) matrix whose row u lists the items user u does not get back.
+        Rows left with fewer than topk candidates are padded with -1 / 0.0.  nprobe: None ranks every item; an integer
+        in [1, nlist] searches the item index (build_index) and ranks the items of the nprobe lists nearest each user,
         without pool or exclude_seen."""
         if nprobe is not None:
             if pool is not None:
@@ -228,8 +284,18 @@ class ParALS(Parallel):
                 raise ValueError("nprobe does not take exclude_seen")
         if self.algo.opt._nrz_P or self.algo.opt._nrz_Q:
             raise RuntimeError("Cannot make topk recommendation with normalized factors")
-        kept, idx, pool = self._resolve(keys, pool, "user")
         Qb = self.algo.Qb if self._bias and self.algo.opt.get("use_bias") else None
+        if scipy.sparse.issparse(pool):
+            kept, idx, _ = self._resolve(keys, None, "user")
+            topk = backend.Serve._check_k(topk)
+            from buffalo_b200.evaluate.device import _gather_rows
+            cands = _gather_rows(*self._pool_matrix(pool, self.algo.P.shape[0], self.algo.Q.shape[0]), idx)
+            seen = self._seen_rows(idx, exclude_seen) if scipy.sparse.issparse(exclude_seen) or exclude_seen else None
+            topks, scores = self._run_cands(idx, self.algo.P, self.algo.Q, Qb, topk, cands, seen)
+            if repr:
+                topks = [[self.algo._idmanager.itemids[t] for t in tt if t != -1] for tt in topks]
+            return kept, topks, scores
+        kept, idx, pool = self._resolve(keys, pool, "user")
         if nprobe is not None:
             topks, scores = self._search_index("item", idx, self.algo.P, topk, nprobe,
                                                self._index_bias("item") is not None, False)
@@ -245,13 +311,22 @@ class ParALS(Parallel):
     def fold_in_recommendation(self, histories, topk=10, pool=None, exclude_seen=True, repr=False):
         """(topks, scores), one row per history row, for users folded into the model (DESIGN.md 4.10): the rows of
         algo.fold_in(histories) with its defaults, ranked against the items as topk_recommendation ranks (pools, -1 / 0.0
-        padding).  exclude_seen: leave each row's history items out.  All on the device: the folded rows are bound as the
+        padding).  pool may also be a scipy sparse (n, num_items) matrix: row i lists history row i's own candidates,
+        as topk_recommendation takes a per-user pool.  exclude_seen: leave each row's history items out.  All on the device: the folded rows are bound as the
         serve handle's queries and never reach the host.  Models with fold_in: ALS and PLSI."""
         if not callable(getattr(self.algo, "_fold_in_device", None)):
             raise NotImplementedError("fold_in_recommendation needs a model with fold_in (ALS, PLSI), not %s"
                                       % type(self.algo).__name__)
         topk = backend.Serve._check_k(topk)
-        if pool is not None:
+        cands = None
+        if scipy.sparse.issparse(pool):
+            if not (scipy.sparse.issparse(histories) or isinstance(histories, (list, tuple))):
+                raise ValueError("histories must be a scipy sparse matrix or a list of lists of item ids, got %s"
+                                 % type(histories).__name__)
+            n_hist = histories.shape[0] if scipy.sparse.issparse(histories) else len(histories)
+            cands = self._pool_matrix(pool, n_hist, self.algo.Q.shape[0])
+            pool = None
+        elif pool is not None:
             pool = self.algo.get_index_pool(pool, group="item")
             if len(pool) == 0:
                 raise RuntimeError("pool is empty")
@@ -265,7 +340,10 @@ class ParALS(Parallel):
             h.bind_queries(tX)
             h.set_pool(pool)
             qidx = torch.arange(n, dtype=torch.int32, device=tX.device)
-            if exclude_seen:
+            if cands is not None:
+                cptr, ckeys = (torch.from_numpy(x).to(tX.device) for x in (cands[0], _nonempty(cands[1])))
+                idx, val = h.topk_candidates_device(qidx, topk, cptr, ckeys, seen=(indptr, keys) if exclude_seen else None)
+            elif exclude_seen:
                 idx, val = h.topk_seen_device(qidx, topk, indptr, keys)
             else:
                 idx, val = h.topk_device(qidx, topk)
@@ -317,6 +395,11 @@ class ParALS(Parallel):
 
 class ParBPRMF(ParALS):
     _bias = True
+
+
+def _nonempty(a):
+    """a, or one zero when a is empty (a device array handed to the library holds at least one element)."""
+    return a if a.size else np.zeros(1, a.dtype)
 
 
 def _unsupported(name):

@@ -392,6 +392,34 @@ int bfl_seen_topk_device(bfl_serve_t* h, const int32_t* d_query_idx, int64_t n, 
                          void* stream);
 
 /* =====================================================================================
+ * Batch serving top-k over a candidate list per query (DESIGN.md 4.13), on a serve handle: query i ranks only the
+ * items of its own list (item ids in any order, duplicates allowed), and row i of the result is bitwise what
+ * bfl_serve_topk (with seen rows: bfl_seen_topk) returns for that query alone with its list set as the pool: the same
+ * scores, item ids best first, ties to the earlier list position.  A query whose list is empty, or holds fewer than k
+ * candidates once its seen items are left out, gets -1 / 0.0f padding; that is not an error.  The handle's pool is not
+ * used.  k in [1, 4096].  Lists and seen rows are arguments of the call, so nothing of them stays on the handle.
+ *  - cand_topk: HOST arrays.  cand_indptr[n] END offsets (row i holds the list of query i: cand_keys[cand_indptr[i - 1]
+ *    .. cand_indptr[i]), from 0), keys in [0, n_items); seen rows (nullable) as bfl_seen_topk takes them.  Batches hold
+ *    at most 2^24 list entries (bfl_cand_set_budget changes that; a longer row is a batch of its own) and the rows
+ *    bfl_serve_topk would batch; each batch's lists are staged through two pinned buffers and uploaded while the
+ *    previous batch runs.  Non-monotone offsets or a key out of range is BFL_ERR_ARG before any device work.
+ *  - cand_topk_device: DEVICE arrays, stream-ordered on `stream`; query q reads row d_cand_row[q] of the candidate CSR
+ *    (d_cand_row nullable: row q) and row d_seen_row[q] of the seen CSR (d_seen_indptr nullable: no seen rows;
+ *    d_seen_row nullable: row q; rows non-decreasing).  Keys must be in [0, n_items).  The call synchronises `stream`
+ *    once per internal batch to size its scratch.  d_out_val nullable.
+ *  - cand_set_budget: list entries per batch of cand_topk (0: the default).
+ * ===================================================================================== */
+int bfl_cand_topk(bfl_serve_t* h, const int32_t* query_idx, int64_t n, int k, const int64_t* cand_indptr,
+                  const int32_t* cand_keys, const int64_t* seen_indptr /* nullable */, const int32_t* seen_keys,
+                  int32_t* out_idx, float* out_val /* nullable */);
+int bfl_cand_topk_device(bfl_serve_t* h, const int32_t* d_query_idx, int64_t n, int k, const int64_t* d_cand_indptr,
+                         const int32_t* d_cand_keys, const int32_t* d_cand_row /* nullable */,
+                         const int64_t* d_seen_indptr /* nullable */, const int32_t* d_seen_keys,
+                         const int32_t* d_seen_row /* nullable */, int32_t* d_out_idx,
+                         float* d_out_val /* nullable */, void* stream);
+int bfl_cand_set_budget(bfl_serve_t* h, int64_t list_entries);
+
+/* =====================================================================================
  * Inverted-file (IVF-Flat) index for batch serving (DESIGN.md 4.12).  build_device clusters n DEVICE rows (pitch ld,
  * first d columns, d <= 256) by spherical k-means into nlist lists (nlist in [1, min(n, 65536)], iters >= 1): nlist
  * distinct rows drawn with `seed` start it, each row goes to the centroid of the largest dot product (ties to the
