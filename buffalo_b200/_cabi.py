@@ -25,6 +25,7 @@ PROTOTYPES = {
     "bfl_last_error": (_cs, []),
     "bfl_abi_version": (C.c_int, []),
     "bfl_compiled_sm": (C.c_int, []),
+    "bfl_require_device": (C.c_int, []),
     "bfl_kernel_launch_count": (_i64, []),
     "bfl_ipc_open": (_vp, [_vp]),
     "bfl_ipc_close": (C.c_int, [_vp]),
@@ -137,6 +138,12 @@ PROTOTYPES = {
     "bfl_eval_ranking_terms_device": (C.c_int, [_vp, _i64, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp]),
     "bfl_eval_score_terms_device": (C.c_int, [_vp, _vp, _vp, C.c_int, C.c_int, _vp, _vp, _vp, _i64, _vp, _vp]),
     "bfl_eval_sum_device": (C.c_int, [_vp, _i64, C.c_int, _vp, _vp]),
+    # offline evaluation
+    "bfl_eval_cutoff_terms_device": (C.c_int, [_vp, _i64, C.c_int, _vp, _vp, _vp, _vp, C.c_int, _vp, _vp, _vp, _i64,
+                                               _vp]),
+    "bfl_eval_ild_device": (C.c_int, [_vp, _i64, C.c_int, C.c_int, _vp, C.c_int, C.c_int, _vp, C.c_int, _vp, _i64, _vp]),
+    "bfl_eval_coverage_mark_device": (C.c_int, [_vp, _i64, C.c_int, _vp, C.c_int, _vp, _vp]),
+    "bfl_eval_coverage_count_device": (C.c_int, [_vp, _i64, C.c_int, _vp, _vp]),
     # ingest helpers
     "bfl_csr_from_triples_device": (C.c_int, [_vp, _vp, _vp, _i64, _i32, _i32, C.c_int, _vp, _vp, _vp, _vp]),
     "bfl_csr_from_triples_host": (C.c_int, [_vp, _vp, _vp, _i64, _i32, _i32, C.c_int, _vp, _vp, _vp]),

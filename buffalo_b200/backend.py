@@ -455,6 +455,11 @@ def device_available():
         return False
 
 
+def require_device():
+    """Raises the library's BackendError ("... no CPU fallback") unless an sm_90 GPU is current."""
+    _cabi.check(_cabi.lib().bfl_require_device(), "bfl_require_device")
+
+
 def topk_host(queries, items, item_bias, k):
     """k best item indices per query row for scores = queries @ items.T (+ item_bias), best first, computed on the
     device (bfl_topk_host).  queries [nq, d], items [I, d] float32 host arrays; returns int32 [nq, k]."""
@@ -836,6 +841,58 @@ def eval_sum(terms, stream=None):
                                                 terms.shape[0], terms.shape[1], out.data_ptr(), _stream_ptr(stream)),
                 "bfl_eval_sum_device")
     return out.cpu().numpy()
+
+
+EVAL_ILD_KMAX = 256
+
+
+def eval_cutoff_terms(ranked, truth_indptr, truth_keys, truth_row, cutoffs, gains, ideal, terms, stream=None):
+    """Writes rows of the float64 [n_cut, rows, 8] device tensor `terms` (its row q for ranked row q; pass a view such as
+    terms[:, s:s + n]) with bfl_eval_cutoff_terms_device's columns 0-7 for the int32 [n, k] ranked lists.  cutoffs: int32
+    device tensor, ascending and distinct, each in [1, k]; truth_row: int32 device tensor or None (row q)."""
+    n, k = ranked.shape
+    if terms.dim() != 3 or terms.shape[0] != cutoffs.shape[0] or terms.shape[1] != n or terms.shape[2] != 8 \
+            or terms.stride(1) != 8 or terms.stride(2) != 1:
+        raise ValueError("terms must be a [%d, %d, 8] view with contiguous rows, got %s"
+                         % (cutoffs.shape[0], n, tuple(terms.shape)))
+    _cabi.check(_cabi.lib().bfl_eval_cutoff_terms_device(
+        _dev(ranked, "int32", "ranked"), n, k, _dev(truth_indptr, "int64", "truth_indptr"),
+        _dev(truth_keys, "int32", "truth_keys"), None if truth_row is None else _dev(truth_row, "int32", "truth_row"),
+        _dev(cutoffs, "int32", "cutoffs"), cutoffs.shape[0], _dev(gains, "float64", "gains"),
+        _dev(ideal, "float64", "ideal"), terms.data_ptr(), terms.stride(0), _stream_ptr(stream)),
+        "bfl_eval_cutoff_terms_device")
+
+
+def eval_ild(ranked, kmax, items, cutoffs, terms, stream=None):
+    """Columns 6-7 of eval_cutoff_terms' `terms` view: intra-list diversity over the rows of the contiguous float32
+    [n_items, d] device tensor `items`; kmax = the largest cutoff (<= EVAL_ILD_KMAX)."""
+    n, k = ranked.shape
+    if terms.dim() != 3 or terms.shape[:2] != (cutoffs.shape[0], n) or terms.stride(1) != 8 or terms.stride(2) != 1:
+        raise ValueError("terms must be a [%d, %d, 8] view with contiguous rows" % (cutoffs.shape[0], n))
+    if items.dim() != 2:
+        raise ValueError("items must be a [n_items, d] tensor")
+    _cabi.check(_cabi.lib().bfl_eval_ild_device(
+        _dev(ranked, "int32", "ranked"), n, k, int(kmax), _dev(items, "float32", "items"), items.shape[1],
+        items.shape[1], _dev(cutoffs, "int32", "cutoffs"), cutoffs.shape[0], terms.data_ptr(), terms.stride(0),
+        _stream_ptr(stream)), "bfl_eval_ild_device")
+
+
+def eval_coverage_mark(ranked, bucket, first, stream=None):
+    """first[item] = min(first[item], bucket[p]) over the entries at positions p < len(bucket) of the int32 [n, k] lists."""
+    n, k = ranked.shape
+    _cabi.check(_cabi.lib().bfl_eval_coverage_mark_device(
+        _dev(ranked, "int32", "ranked"), n, k, _dev(bucket, "int32", "bucket"), bucket.shape[0],
+        _dev(first, "int32", "first"), _stream_ptr(stream)), "bfl_eval_coverage_mark_device")
+
+
+def eval_coverage_count(first, n_cut, stream=None):
+    """int64 numpy [n_cut]: the number of items whose `first` entry is c, for each c < n_cut."""
+    import torch
+    count = torch.empty(int(n_cut), dtype=torch.int64, device=first.device)
+    _cabi.check(_cabi.lib().bfl_eval_coverage_count_device(_dev(first, "int32", "first"), first.shape[0], int(n_cut),
+                                                           count.data_ptr(), _stream_ptr(stream)),
+                "bfl_eval_coverage_count_device")
+    return count.cpu().numpy()
 
 
 def csr_from_triples_host(major, minor, vals, num_major, num_minor, sort_minor=True):

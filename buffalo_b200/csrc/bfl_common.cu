@@ -279,6 +279,7 @@ extern "C" {
 const char* bfl_last_error(void) { return bfl::t_last_error.c_str(); }
 int bfl_abi_version(void) { return 1; }
 int bfl_compiled_sm(void) { return 90; }
+int bfl_require_device(void) { return bfl::require_device(); }
 int64_t bfl_kernel_launch_count(void) { return (int64_t)bfl::g_launches.load(); }
 void* bfl_ipc_open(const void* handle64) {
     if (!handle64) {

@@ -49,6 +49,21 @@ class Evaluable(object):
         res.update(ev.scores())
         return res
 
+    def evaluate(self, test, cutoffs=(10,), exclude_seen=True, diversity=False, per_user=False):
+        """Ranking metrics of this model on held-out interactions, on the GPU (DESIGN.md 4.14).
+
+        test: a scipy sparse (num_users, num_items) matrix in the model's index space; row u's ground truth is its
+        distinct columns with a nonzero value after duplicates are summed, and only users with at least one are
+        evaluated.  Each is ranked once at the largest cutoff by the masked top-k of the validation path, leaving out
+        exclude_seen's items as ParALS.topk_recommendation does: True the rows of the attached training data, False
+        nothing, a scipy sparse (num_users, num_items) matrix its rows.  cutoffs: integers in [1, 4096] (<= 256 with
+        diversity).  diversity=True adds ild@K over the rows of the item factors Q.  The result is evaluate_lists'
+        for those lists.  Unlike get_validation_results(), users without training items are evaluated too.  Not for
+        WARP with score_func="l2", which has no device ranking.  GPU only: without one the
+        backend's "no CPU fallback" error is raised after the argument checks."""
+        from buffalo_b200.evaluate.offline import evaluate_model
+        return evaluate_model(self, test, cutoffs, exclude_seen, diversity, per_user)
+
     def _device_eval_route(self):
         """The EvalModel of the device path (evaluate/device.py), or None for the host path: the device path needs a
         trainer that provides _device_eval_model, 0 < topk <= 4096, a GPU, and the private option _b200_device_eval

@@ -35,6 +35,51 @@ def _gather_rows(indptr, keys, rows):
     return out_ptr, np.ascontiguousarray(keys[pos], dtype=np.int32)
 
 
+def to_device(a, dtype, dev):
+    import torch
+    return torch.from_numpy(np.ascontiguousarray(a, dtype=dtype)).to(dev)
+
+
+class SortedRows(object):
+    """Rows `rows` (in that order) of a host CSR of END offsets, handed to device calls that need every row in ascending
+    order: the validation users' training rows here, the truth and exclusion rows of evaluate/offline.py.  With
+    resident=True the rows stay on the device when they fit in MEM_FRACTION of the free device memory; otherwise each
+    batch gathers, uploads and sorts its own."""
+
+    def __init__(self, indptr, keys, rows, dev, num_items, resident=True):
+        self.dev, self.num_items = dev, num_items
+        nnz = int(indptr[-1]) if len(indptr) else 0
+        self.indptr, self.keys = _gather_rows(np.asarray(indptr, dtype=np.int64), np.asarray(keys[:nnz]), rows)
+        nbytes = self.keys.nbytes + self.indptr.nbytes
+        self.resident = resident and nbytes < MEM_FRACTION * backend.device_free_bytes()
+        if self.resident:
+            self.d_rows = self._sorted(to_device(self.indptr, np.int64, dev), to_device(_nonempty(self.keys), np.int32, dev))
+
+    def mean_len(self):
+        return int(np.ceil(len(self.keys) / max(len(self.indptr), 1)))
+
+    def _sorted(self, indptr, keys):
+        """The CSR with every row sorted: unchanged when the device check finds all rows sorted (the rows of a
+        "matrix" database), else rebuilt by the device radix sort (a "stream" database keeps session order)."""
+        import torch
+        if backend.eval_unsorted_rows(indptr, keys) == 0:
+            return indptr, keys
+        lens = torch.diff(indptr, prepend=indptr.new_zeros(1))
+        major = torch.repeat_interleave(torch.arange(indptr.shape[0], dtype=torch.int32, device=self.dev), lens)
+        ones = torch.ones(keys.shape[0], dtype=torch.float32, device=self.dev)
+        sorted_indptr, sorted_keys, _ = backend.csr_from_triples_device(major, keys, ones, indptr.shape[0],
+                                                                        self.num_items)
+        return sorted_indptr, sorted_keys
+
+    def rows_for(self, local):
+        """(indptr, keys, row) device tensors: query q of a batch reads CSR row row[q], which holds rows[local[q]]."""
+        if self.resident:
+            return self.d_rows + (to_device(local, np.int32, self.dev),)
+        ptr, keys = _gather_rows(self.indptr, self.keys, local)
+        indptr, keys = self._sorted(to_device(ptr, np.int64, self.dev), to_device(_nonempty(keys), np.int32, self.dev))
+        return indptr, keys, to_device(np.arange(len(local)), np.int32, self.dev)
+
+
 class ValidationState(object):
     def __init__(self, data, dev, max_users=None):
         import torch
@@ -51,40 +96,19 @@ class ValidationState(object):
         self.gt_indptr, self.gt_keys, _ = backend.csr_from_triples_device(t(row, np.int32), self.cols, self.vals,
                                                                           self.num_users, self.num_items)
         grp = data.get_group("rowwise")
-        indptr = np.asarray(grp["indptr"][:], dtype=np.int64)
-        nnz = int(indptr[-1]) if len(indptr) else 0
-        self.seen_indptr, self.seen_keys = _gather_rows(indptr, np.asarray(grp["key"][:nnz]), self.vali_rows)
         self.max_users = max_users
-        seen_bytes = self.seen_keys.nbytes + self.seen_indptr.nbytes
-        self.resident = max_users is None and seen_bytes < MEM_FRACTION * backend.device_free_bytes()
-        if self.resident:   # every validation user's training row on the device for the life of the Data
-            self.d_seen = self._sorted(t(self.seen_indptr, np.int64), t(_nonempty(self.seen_keys), np.int32))
+        # every validation user's training row on the device for the life of the Data, when it fits
+        self.seen = SortedRows(grp["indptr"][:], grp["key"], self.vali_rows, dev, self.num_items,
+                               resident=max_users is None)
+        self.seen_indptr, self.seen_keys, self.resident = self.seen.indptr, self.seen.keys, self.seen.resident
         torch.cuda.current_stream(dev).synchronize()
 
     def _to_dev(self, a, dtype):
-        import torch
-        return torch.from_numpy(np.ascontiguousarray(a, dtype=dtype)).to(self.dev)
-
-    def _sorted(self, indptr, keys):
-        """The CSR with every row sorted: unchanged when the device check finds all rows sorted (the rows of a
-        "matrix" database), else rebuilt by the device radix sort (a "stream" database keeps session order)."""
-        import torch
-        if backend.eval_unsorted_rows(indptr, keys) == 0:
-            return indptr, keys
-        lens = torch.diff(indptr, prepend=indptr.new_zeros(1))
-        major = torch.repeat_interleave(torch.arange(indptr.shape[0], dtype=torch.int32, device=self.dev), lens)
-        ones = torch.ones(keys.shape[0], dtype=torch.float32, device=self.dev)
-        sorted_indptr, sorted_keys, _ = backend.csr_from_triples_device(major, keys, ones, indptr.shape[0],
-                                                                        self.num_items)
-        return sorted_indptr, sorted_keys
+        return to_device(a, dtype, self.dev)
 
     def seen_for(self, local):
         """(seen_indptr, seen_keys, seen_row) device tensors covering the validation users vali_rows[local]."""
-        if self.resident:
-            return self.d_seen + (self._to_dev(local, np.int32),)
-        ptr, keys = _gather_rows(self.seen_indptr, self.seen_keys, local)
-        indptr, keys = self._sorted(self._to_dev(ptr, np.int64), self._to_dev(_nonempty(keys), np.int32))
-        return indptr, keys, self._to_dev(np.arange(len(local)), np.int32)
+        return self.seen.rows_for(local)
 
 
 def state_of(data, dev, max_users=None):

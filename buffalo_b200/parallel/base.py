@@ -80,6 +80,28 @@ def cand_topn(indexes, P, Q, Qb, topk, cand_indptr, cand_keys, seen_indptr=None,
     return keys, scores
 
 
+def seen_csr(algo, exclude_seen):
+    """(END offsets int64, keys) of every user's seen row, as exclude_seen=... names them: the rows of the algo's
+    training data ("rowwise" group) for exclude_seen=True, of a scipy sparse (num_users, num_items) matrix otherwise."""
+    num_users, num_items = algo.P.shape[0], algo.Q.shape[0]
+    if scipy.sparse.issparse(exclude_seen):
+        m = exclude_seen.tocsr()
+        if m.shape != (num_users, num_items):
+            raise ValueError("exclude_seen must be a (%d, %d) matrix, got %s" % (num_users, num_items, m.shape))
+        ends = np.asarray(m.indptr[1:], dtype=np.int64)
+        keys = np.asarray(m.indices[:int(m.indptr[-1])])
+        if keys.size and (keys.min() < 0 or keys.max() >= num_items):
+            raise ValueError("exclude_seen holds a column outside [0, %d)" % num_items)
+        return ends, keys
+    data = getattr(algo, "data", None)
+    if data is None:
+        raise ValueError("exclude_seen=True needs the training data attached to the model; pass a scipy "
+                         "sparse (num_users, num_items) matrix of the seen items instead")
+    grp = data.get_group("rowwise")
+    ends = np.asarray(grp["indptr"][:], dtype=np.int64)
+    return ends, np.asarray(grp["key"][:int(ends[-1]) if len(ends) else 0])
+
+
 class Parallel(object):
     def __init__(self, algo, *argv, **kwargs):
         self.algo = algo
@@ -245,27 +267,9 @@ class ParALS(Parallel):
         return np.asarray(m.indptr[1:], dtype=np.int64), np.ascontiguousarray(keys, dtype=np.int32)
 
     def _seen_rows(self, idx, exclude_seen):
-        """(END offsets int64, keys int32) of the seen rows of users idx: rows of the algo's training data ("rowwise"
-        group) for exclude_seen=True, of a scipy sparse (num_users, num_items) matrix otherwise."""
-        num_users, num_items = self.algo.P.shape[0], self.algo.Q.shape[0]
-        if scipy.sparse.issparse(exclude_seen):
-            m = exclude_seen.tocsr()
-            if m.shape != (num_users, num_items):
-                raise ValueError("exclude_seen must be a (%d, %d) matrix, got %s" % (num_users, num_items, m.shape))
-            ends = np.asarray(m.indptr[1:], dtype=np.int64)
-            keys = np.asarray(m.indices[:int(m.indptr[-1])])
-            if keys.size and (keys.min() < 0 or keys.max() >= num_items):
-                raise ValueError("exclude_seen holds a column outside [0, %d)" % num_items)
-        else:
-            data = getattr(self.algo, "data", None)
-            if data is None:
-                raise ValueError("exclude_seen=True needs the training data attached to the model; pass a scipy "
-                                 "sparse (num_users, num_items) matrix of the seen items instead")
-            grp = data.get_group("rowwise")
-            ends = np.asarray(grp["indptr"][:], dtype=np.int64)
-            keys = np.asarray(grp["key"][:int(ends[-1]) if len(ends) else 0])
+        """(END offsets int64, keys int32) of the seen rows of users idx (seen_csr)."""
         from buffalo_b200.evaluate.device import _gather_rows
-        return _gather_rows(ends, keys, idx)
+        return _gather_rows(*seen_csr(self.algo, exclude_seen), idx)
 
     def topk_recommendation(self, keys, topk=10, pool=None, repr=False, exclude_seen=False, nprobe=None):
         """pool: None ranks every item; a list of item ids (or an index array) is one candidate pool for every user; a

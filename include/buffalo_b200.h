@@ -45,6 +45,9 @@ const char* bfl_last_error(void);
 /* library/ABI version and the SM architecture the kernels were compiled for (90) */
 int bfl_abi_version(void);
 int bfl_compiled_sm(void);
+/* BFL_OK when a CUDA device of compute capability 9.0 is current, else BFL_ERR_CUDA with the "no CPU fallback" error:
+ * the check every device call makes first, for callers that want it before their own device work */
+int bfl_require_device(void);
 /* number of kernels this library launched since load (bench.py's gpu_launches claim) */
 int64_t bfl_kernel_launch_count(void);
 /* Map another process's device allocation into this process with the CURRENT device as accessor
@@ -481,6 +484,33 @@ int bfl_eval_score_terms_device(const float* d_P, const float* d_Q, const float*
                                 const int32_t* d_rows, const int32_t* d_cols, const float* d_vals, int64_t n,
                                 double* d_terms, void* stream);
 int bfl_eval_sum_device(const double* d_terms, int64_t n, int width, double* d_out, void* stream);
+
+/* =====================================================================================
+ * Offline evaluation on held-out interactions (DESIGN.md 4.14): the device path of Evaluable.evaluate and
+ * buffalo_b200.evaluate.evaluate_lists.  Device pointers, stream-ordered.  d_ranked [n x k] holds ranked item lists,
+ * -1 for padding.  d_cutoffs [n_cut] holds the cutoffs ascending and distinct, each in [1, k].  d_terms holds one
+ * [rows x 8] fp64 slab per cutoff, slab_stride doubles apart (>= 8 n); row q of a call writes row q of every slab.  Slab
+ * columns: hit, recall, precision, ndcg, ap / min(|T|, K), reciprocal rank, ild, 1 if the ild counts.
+ *  - cutoff_terms: per row q, its truth row d_truth_row[q] (d_truth_row nullable: row q) of the truth CSR (END
+ *    offsets, every row ascending without duplicates); writes columns 0-5 and zeros in 6-7.  d_gains[i] = 1 / log2(i + 2)
+ *    and d_ideal its prefix sums, at least as long as the largest cutoff.  A row with an empty truth row gets zeros.
+ *  - ild: columns 6-7: over the valid entries among the first K, the mean of 1 - cos over all pairs of their rows of
+ *    d_items [n_items x ld] (first d columns; cos = 0 when a row has zero norm), counted when there are at least two.
+ *    kmax = the largest cutoff, at most 256 and at most k.
+ *  - coverage_mark: d_first[item] = min(d_first[item], d_bucket[p]) for every entry at position p < kmax, where
+ *    d_bucket[p] is the index of the smallest cutoff > p.  Start d_first at n_cut; calls on several batches accumulate.
+ *  - coverage_count: d_count[c] (u64) = the number of items whose d_first is c, for c < n_cut (<= 4096).
+ * ===================================================================================== */
+int bfl_eval_cutoff_terms_device(const int32_t* d_ranked, int64_t n, int k, const int64_t* d_truth_indptr,
+                                 const int32_t* d_truth_keys, const int32_t* d_truth_row /* nullable */,
+                                 const int32_t* d_cutoffs, int n_cut, const double* d_gains, const double* d_ideal,
+                                 double* d_terms, int64_t slab_stride, void* stream);
+int bfl_eval_ild_device(const int32_t* d_ranked, int64_t n, int k, int kmax, const float* d_items, int ld, int d,
+                        const int32_t* d_cutoffs, int n_cut, double* d_terms, int64_t slab_stride, void* stream);
+int bfl_eval_coverage_mark_device(const int32_t* d_ranked, int64_t n, int k, const int32_t* d_bucket, int kmax,
+                                  int32_t* d_first, void* stream);
+int bfl_eval_coverage_count_device(const int32_t* d_first, int64_t n_items, int n_cut, unsigned long long* d_count,
+                                   void* stream);
 
 /* =====================================================================================
  * Ingest helpers (SURVEY.md 8(f-1), 8(f-4)).
