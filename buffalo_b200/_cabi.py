@@ -122,6 +122,7 @@ PROTOTYPES = {
     "bfl_cand_topk": (C.c_int, [_vp, _vp, _i64, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bfl_cand_topk_device": (C.c_int, [_vp, _vp, _i64, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bfl_cand_set_budget": (C.c_int, [_vp, _i64]),
+    "bfl_mmr_rerank_device": (C.c_int, [_vp, _vp, _vp, _i64, C.c_int, C.c_int, C.c_float, _vp, _vp, _vp]),
     # IVF index
     "bfl_ivf_create": (_vp, []),
     "bfl_ivf_destroy": (None, [_vp]),

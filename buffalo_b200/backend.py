@@ -493,6 +493,7 @@ def topk_device(queries, items, item_bias, k, stream=None):
 
 
 SERVE_KMAX = 4096
+MMR_MMAX = 256        # candidates per row of the MMR re-ranking (its Gram triangle lives in shared memory)
 
 
 class Serve(_Holder):
@@ -741,6 +742,34 @@ class Serve(_Holder):
                 None if cand_row is None else cand_row.data_ptr(), None if sptr is None else sptr.data_ptr(),
                 None if skeys is None else skeys.data_ptr(), None if srow is None else srow.data_ptr(),
                 idx.data_ptr(), val.data_ptr(), _stream_ptr(stream)), "bfl_cand_topk_device")
+        return idx, val
+
+    def rerank_mmr_device(self, cand_idx, cand_val, k, diversify, stream=None):
+        """MMR re-ranking (bfl_mmr_rerank_device) of torch CUDA candidate lists against the handle's items: cand_idx
+        int32 [n, m] item ids (-1 pads), cand_val float32 [n, m] their scores, 1 <= k <= m <= MMR_MMAX, diversify in
+        [0, 1] -> (int32 [n, k], float32 [n, k]) CUDA tensors, stream-ordered.  The id range check synchronises."""
+        import torch
+        _dev(cand_idx, "int32", "cand_idx")
+        _dev(cand_val, "float32", "cand_val")
+        if cand_idx.dim() != 2 or cand_val.shape != cand_idx.shape:
+            raise ValueError("cand_idx and cand_val must be [n, m] tensors of one shape")
+        n, m = cand_idx.shape
+        k = int(k)
+        if not 1 <= k <= m <= MMR_MMAX:
+            raise ValueError("need 1 <= k <= m <= %d, got k=%d, m=%d" % (MMR_MMAX, k, m))
+        if not 0.0 <= float(diversify) <= 1.0:
+            raise ValueError("diversify must be in [0, 1], got %r" % (diversify,))
+        if self._d is None:
+            raise ValueError("set the items before reranking")
+        if n and cand_idx.numel():
+            lo, hi = torch.aminmax(cand_idx)
+            if int(lo.item()) < -1 or int(hi.item()) >= self.num_items:
+                raise ValueError("cand_idx holds an id outside [-1, %d)" % self.num_items)
+        idx = torch.empty((n, k), dtype=torch.int32, device=cand_idx.device)
+        val = torch.empty((n, k), dtype=torch.float32, device=cand_idx.device)
+        _cabi.check(self._lib.bfl_mmr_rerank_device(self._h, cand_idx.data_ptr(), cand_val.data_ptr(), n, m, k,
+                                                    float(diversify), idx.data_ptr(), val.data_ptr(),
+                                                    _stream_ptr(stream)), "bfl_mmr_rerank_device")
         return idx, val
 
     @staticmethod

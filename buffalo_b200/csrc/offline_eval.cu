@@ -6,11 +6,12 @@
 //                             ballot and a warp scan give the hit count, the DCG and the AP sum up to each entry, and the
 //                             values at every cutoff inside the chunk are written to that cutoff's [n x 8] slab;
 //   oe_ild_kernel           : one CTA per row; the Gram matrix of the row's first kmax item rows (kmax <= 256) is built
-//                             in shared memory, d in tiles of OE_TD columns, then 1 - cos per pair summed per cutoff;
+//                             in shared memory (gram_common.cuh), then 1 - cos per pair summed per cutoff;
 //   oe_coverage_mark_kernel : first[item] = min over every list entry of the cutoff index the entry's position falls in;
 //   oe_coverage_count_kernel: the number of items per first cutoff index (integers, so any order gives the same count).
 #include <algorithm>
 
+#include "gram_common.cuh"
 #include "seen_common.cuh"
 
 using namespace bfl;
@@ -20,9 +21,6 @@ namespace {
 constexpr int OE_WIDTH = 8;          // hit, recall, precision, ndcg, ap, rr, ild, ild counted
 constexpr int OE_TERMS_THREADS = 256;
 constexpr int OE_ILD_KMAX = 256;
-constexpr int OE_TD = 32;            // Gram tile: columns of d per pass
-constexpr int OE_TDS = OE_TD + 4;    // its row stride in floats: rows stay 16-byte aligned, thread b's reads of row b
-                                     // spread over 8 banks
 constexpr int OE_COUNT_THREADS = 256;
 
 // terms[c * slab + r * OE_WIDTH + j]: slab c is the [n x 8] block of cutoff c.
@@ -86,55 +84,25 @@ __global__ void __launch_bounds__(OE_TERMS_THREADS) oe_cutoff_terms_kernel(
     }
 }
 
-// Shared memory: one tile [kmax][OE_TDS] of item rows, per position b the fp64 sum over valid a < b of 1 - cos(a, b),
-// the row's items, and the Gram triangle G[b * (b + 1) / 2 + a] (a <= b < kmax) in fp32.  Thread b owns column b of the
-// triangle: every tile adds its OE_TD products to G[a, b] for a = 0..b in that order, so each dot product has one fixed
-// order.
+// Shared memory: one tile [kmax][GRAM_TDS] of item rows, per position b the fp64 sum over valid a < b of 1 - cos(a, b),
+// the row's items, and the Gram triangle of gram_triangle (gram_common.cuh).
 __global__ void __launch_bounds__(OE_ILD_KMAX) oe_ild_kernel(const int32_t* __restrict__ ranked, int k, int kmax,
                                                              const float* __restrict__ items, int ld, int d,
                                                              const int32_t* __restrict__ cutoffs, int n_cut,
                                                              double* __restrict__ terms, int64_t slab) {
     extern __shared__ __align__(16) unsigned char oe_smem[];
     // tile first: its rows are read as float4, so it must start on 16 bytes (its size, 144 kmax, keeps pair_sum on 8)
-    float* tile = reinterpret_cast<float*>(oe_smem);                        // [kmax][OE_TDS]
-    double* pair_sum = reinterpret_cast<double*>(tile + (size_t)kmax * OE_TDS);   // [kmax]
+    float* tile = reinterpret_cast<float*>(oe_smem);                        // [kmax][GRAM_TDS]
+    double* pair_sum = reinterpret_cast<double*>(tile + gram_tile_floats(kmax));   // [kmax]
     int32_t* item = reinterpret_cast<int32_t*>(pair_sum + kmax);            // [kmax]
     float* G = reinterpret_cast<float*>(item + kmax);                       // [kmax * (kmax + 1) / 2]
     const int tid = threadIdx.x, nt = blockDim.x;
     const int64_t r = blockIdx.x;
     const int32_t* rk = ranked + r * (int64_t)k;
     for (int b = tid; b < kmax; b += nt) item[b] = rk[b];
-    for (int p = tid; p < kmax * (kmax + 1) / 2; p += nt) G[p] = 0.f;
-    __syncthreads();
+    gram_triangle(item, kmax, items, ld, d, tile, G);
     const int b = tid;
     const size_t gb = (size_t)b * (b + 1) / 2;
-    for (int d0 = 0; d0 < d; d0 += OE_TD) {
-        for (int e = tid; e < kmax * OE_TD; e += nt) {
-            const int a = e / OE_TD, t = e - a * OE_TD;
-            const int32_t it = item[a];
-            tile[a * OE_TDS + t] = it >= 0 && d0 + t < d ? items[(int64_t)it * ld + d0 + t] : 0.f;
-        }
-        __syncthreads();
-        if (b < kmax) {
-            float xb[OE_TD];
-#pragma unroll
-            for (int t = 0; t < OE_TD; ++t) xb[t] = tile[b * OE_TDS + t];
-            for (int a = 0; a <= b; ++a) {
-                const float4* xa = reinterpret_cast<const float4*>(tile + a * OE_TDS);
-                float acc = 0.f;
-#pragma unroll
-                for (int t = 0; t < OE_TD / 4; ++t) {
-                    const float4 v = xa[t];
-                    acc = fmaf(v.x, xb[4 * t], acc);
-                    acc = fmaf(v.y, xb[4 * t + 1], acc);
-                    acc = fmaf(v.z, xb[4 * t + 2], acc);
-                    acc = fmaf(v.w, xb[4 * t + 3], acc);
-                }
-                G[gb + a] += acc;
-            }
-        }
-        __syncthreads();
-    }
     if (b < kmax) {
         double s = 0.0;
         if (item[b] >= 0) {
@@ -190,9 +158,9 @@ __global__ void __launch_bounds__(OE_COUNT_THREADS) oe_coverage_count_kernel(con
 }
 
 size_t ild_smem_bytes(int kmax) {
-    static_assert((sizeof(float) * OE_TDS) % 16 == 0, "tile rows must keep float4 alignment");
-    return sizeof(float) * (size_t)kmax * OE_TDS + sizeof(double) * kmax + sizeof(int32_t) * kmax +
-           sizeof(float) * (size_t)kmax * (kmax + 1) / 2;
+    static_assert((sizeof(float) * GRAM_TDS) % 16 == 0, "tile rows must keep float4 alignment");
+    return sizeof(float) * gram_tile_floats(kmax) + sizeof(double) * kmax + sizeof(int32_t) * kmax +
+           sizeof(float) * gram_triangle_floats(kmax);
 }
 
 }  // namespace

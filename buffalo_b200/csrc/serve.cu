@@ -828,6 +828,19 @@ int bfl_cand_topk_device(bfl_serve_t* h, const int32_t* d_query_idx, int64_t n, 
     return BFL_OK;
 }
 
+int bfl_mmr_rerank_device(bfl_serve_t* h, const int32_t* d_cand_idx, const float* d_cand_val, int64_t n, int m,
+                          int k, float diversify, int32_t* d_out_idx, float* d_out_val, void* stream) {
+    if (!h) BFL_FAIL(BFL_ERR_ARG, "serve: null handle");
+    if (!d_cand_idx || !d_cand_val || !d_out_idx || !d_out_val || n < 0)
+        BFL_FAIL(BFL_ERR_ARG, "mmr: bad arguments");
+    if (m < 1 || m > 256 || k < 1 || k > m) BFL_FAIL(BFL_ERR_ARG, "mmr: need 1 <= k <= m <= 256");
+    if (!(diversify >= 0.f && diversify <= 1.f)) BFL_FAIL(BFL_ERR_ARG, "mmr: diversify must be in [0, 1]");
+    if (n > INT_MAX) BFL_FAIL(BFL_ERR_ARG, "mmr: too many rows in one call");
+    if (!h->items) BFL_FAIL(BFL_ERR_STATE, "mmr: set the items first");
+    return mmr_rerank(h->items, h->ldi, h->d, d_cand_idx, d_cand_val, n, m, k, diversify, d_out_idx, d_out_val,
+                      (cudaStream_t)stream);
+}
+
 int bfl_cand_set_budget(bfl_serve_t* h, int64_t list_entries) {
     if (!h || list_entries < 0) BFL_FAIL(BFL_ERR_ARG, "serve: bad candidate budget");
     h->cand_budget = list_entries;

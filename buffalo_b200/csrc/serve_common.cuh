@@ -228,4 +228,8 @@ int cand_batch(const float* queries, int64_t n_q, int ldq, const int32_t* qidx, 
                const float* bias, int d, int k, CandRows cand, CandRows seen, const long long* unit_end,
                const long long* key_end, long long n_units, unsigned long long* cand_key, int32_t* cand_cnt,
                int32_t* out_idx, float* out_val, cudaStream_t st);
+// rerank.cu, stream-ordered: the MMR re-ranking of n rows of m candidates (item ids, -1 pads; scores) against the item
+// rows (pitch ld, first d columns) -> out_idx / out_val [n x k].  1 <= k <= m <= 256, 0 <= diversify <= 1.
+int mmr_rerank(const float* items, int ld, int d, const int32_t* cand_idx, const float* cand_val, int64_t n, int m,
+               int k, float diversify, int32_t* out_idx, float* out_val, cudaStream_t st);
 }  // namespace bfl

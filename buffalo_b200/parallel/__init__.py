@@ -1,1 +1,1 @@
-from buffalo_b200.parallel.base import ParALS, ParBPRMF, ParCFR, ParW2V, dot_topn, quickselect
+from buffalo_b200.parallel.base import ParALS, ParBPRMF, ParCFR, ParW2V, dot_topn, quickselect, rerank_mmr

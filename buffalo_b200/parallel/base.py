@@ -102,6 +102,137 @@ def seen_csr(algo, exclude_seen):
     return ends, np.asarray(grp["key"][:int(ends[-1]) if len(ends) else 0])
 
 
+RERANK_BATCH_BYTES = 256 << 20   # device candidate lists (ids + scores) per batch of a diversified call
+
+
+def _check_diversify(diversify, candidates, topk):
+    """(w, M) of topk_recommendation's diversify / diversify_candidates, or None when diversify is None; w is rounded to
+    float32 as the device takes it, so both paths use the same weight.  ValueError on anything else."""
+    if diversify is None:
+        if candidates is not None:
+            raise ValueError("diversify_candidates needs diversify")
+        return None
+    if isinstance(diversify, bool) or not isinstance(diversify, (int, float, np.integer, np.floating)) \
+            or not 0 <= diversify <= 1:
+        raise ValueError("diversify must be None or a real number in [0, 1], got %r" % (diversify,))
+    if isinstance(topk, bool) or not isinstance(topk, (int, np.integer)) or not 1 <= topk <= backend.MMR_MMAX:
+        raise ValueError("topk must be an integer in [1, %d] with diversify, got %r" % (backend.MMR_MMAX, topk))
+    if candidates is None:
+        candidates = min(4 * int(topk), backend.MMR_MMAX)
+    if isinstance(candidates, bool) or not isinstance(candidates, (int, np.integer)) \
+            or not topk <= candidates <= backend.MMR_MMAX:
+        raise ValueError("diversify_candidates must be an integer in [topk, %d] = [%d, %d], got %r"
+                         % (backend.MMR_MMAX, topk, backend.MMR_MMAX, candidates))
+    return float(np.float32(diversify)), int(candidates)
+
+
+def mmr_numpy(cand_idx, cand_val, F, topk, w):
+    """The MMR re-ranking of bfl_mmr_rerank_device (DESIGN.md 4.15) in NumPy: rows of candidate ids (-1 pads) and
+    their scores, item rows F (float32, bias excluded) -> (keys int32, scores float32) [n, topk], -1 / 0.0 padded.  The
+    cosines are taken in fp64 from the fp32 rows, so they can differ from the device's fp32 dot products in the last
+    bits."""
+    cand_idx, cand_val = np.asarray(cand_idx), np.asarray(cand_val, dtype=np.float32)
+    n = cand_idx.shape[0]
+    keys = np.full((n, topk), -1, dtype=np.int32)
+    scores = np.zeros((n, topk), dtype=np.float32)
+    for r in range(n):
+        pos = np.flatnonzero(cand_idx[r] >= 0)
+        if not pos.size:
+            continue
+        ids, s = cand_idx[r, pos], cand_val[r, pos]
+        s64 = s.astype(np.float64)
+        lo, hi = s64.min(), s64.max()
+        rel = (s64 - lo) / (hi - lo) if hi > lo else np.ones(len(pos))
+        X = np.asarray(F[ids], dtype=np.float32).astype(np.float64)
+        G = X @ X.T
+        nrm = np.diag(G)
+        ok = (nrm[:, None] > 0) & (nrm[None, :] > 0)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            cos = np.where(ok, G / np.sqrt(nrm[:, None] * nrm[None, :]), 0.0)
+        picked = np.zeros(len(pos), dtype=bool)
+        maxsim = np.full(len(pos), -np.inf)
+        for t in range(min(topk, len(pos))):
+            obj = (1.0 - w) * rel if t == 0 else (1.0 - w) * rel - w * maxsim
+            p = int(np.argmax(np.where(picked, -np.inf, obj)))   # the first of equal maxima: the smaller position
+            keys[r, t], scores[r, t] = ids[p], s[p]
+            picked[p] = True
+            maxsim = np.maximum(maxsim, cos[p])
+    return keys, scores
+
+
+def _on_torch(x, dev):
+    """x as a CUDA tensor on dev: a torch tensor as it is, a host array copied (an empty one as one zero)."""
+    import torch
+    return x if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(_nonempty(x))).to(dev)
+
+
+def _device_stage(h, M, dev, seen=None, cands=None):
+    """stage(q) -> (ids, scores) CUDA [len(q), M]: the candidate call of a serve handle whose queries are set, for the
+    query rows q (int32 CUDA), which are also the rows of the seen / candidate CSRs (END offsets, keys; host arrays or
+    CUDA tensors).  The pool is the handle's."""
+    sv = None if seen is None else (_on_torch(seen[0], dev), _on_torch(seen[1], dev))
+    if cands is not None:
+        cptr, ckeys = _on_torch(cands[0], dev), _on_torch(cands[1], dev)
+        return lambda q: h.topk_candidates_device(q, M, cptr, ckeys, cand_row=q,
+                                                  seen=None if sv is None else (sv[0], sv[1], q))
+    if sv is not None:
+        return lambda q: h.topk_seen_device(q, M, sv[0], sv[1], seen_row=q)
+    return lambda q: h.topk_device(q, M)
+
+
+def _rerank_batches(h, n, topk, w, M, dev, stage):
+    """(keys int32, scores float32) host [n, topk]: stage's M candidates of every query row reranked on the device,
+    RERANK_BATCH_BYTES of candidate lists at a time (rows are independent, so the split changes nothing)."""
+    import torch
+    keys = np.empty((n, topk), dtype=np.int32)
+    scores = np.empty((n, topk), dtype=np.float32)
+    rows = max(1, RERANK_BATCH_BYTES // (8 * M))
+    for b0 in range(0, n, rows):
+        nb = min(rows, n - b0)
+        q = torch.arange(b0, b0 + nb, dtype=torch.int32, device=dev)
+        ci, cv = stage(q)
+        ri, rv = h.rerank_mmr_device(ci, cv, topk, w)
+        keys[b0:b0 + nb], scores[b0:b0 + nb] = ri.cpu().numpy(), rv.cpu().numpy()
+    return keys, scores
+
+
+def rerank_mmr(cand_idx, cand_val, item_factors, topk, diversify):
+    """MMR re-ranking (DESIGN.md 4.15) of candidate lists made elsewhere, such as IVF results or another retriever:
+    cand_idx an (n, m) integer array of item indexes (-1 pads, duplicates are ordinary candidates, m <= 256), cand_val
+    their (n, m) scores, item_factors the (num_items, d) rows whose cosines measure similarity.  Per row, topk of the
+    candidates picked greedily: at each step the largest (1 - diversify) rel - diversify max-cos-to-the-picked, rel the
+    score scaled to [0, 1] over the row, ties to the earlier position.  Returns (keys int32, scores float32) [n, topk]
+    in pick order, the scores as given, -1 / 0.0 once the valid candidates run out.  diversify = 0 keeps the first
+    topk candidates of a best-first list.  On the GPU when one is present, in NumPy otherwise."""
+    ci, cv = np.asarray(cand_idx), np.asarray(cand_val)
+    if ci.ndim != 2 or not np.issubdtype(ci.dtype, np.integer) or ci.shape[1] < 1 or cv.shape != ci.shape:
+        raise ValueError("cand_idx must be an (n, m) integer array with m >= 1 and cand_val of the same shape, got %s "
+                         "and %s" % (ci.shape, cv.shape))
+    F = np.ascontiguousarray(item_factors, dtype=np.float32)
+    if F.ndim != 2 or F.shape[0] < 1 or F.shape[1] < 1:
+        raise ValueError("item_factors must be a (num_items, d) array, got shape %s" % (F.shape,))
+    n, m = ci.shape
+    if m > backend.MMR_MMAX:
+        raise ValueError("at most %d candidates per row, got %d" % (backend.MMR_MMAX, m))
+    if isinstance(topk, bool) or not isinstance(topk, (int, np.integer)) or not 1 <= topk <= m:
+        raise ValueError("topk must be an integer in [1, %d], got %r" % (m, topk))
+    w, _ = _check_diversify(diversify, m, topk)
+    if ci.size and (int(ci.min()) < -1 or int(ci.max()) >= F.shape[0]):
+        raise ValueError("cand_idx holds an index outside [-1, %d)" % F.shape[0])
+    ci, cv = np.ascontiguousarray(ci, dtype=np.int32), np.ascontiguousarray(cv, dtype=np.float32)
+    if not (backend.device_available() and n and F.shape[0] < 2 ** 31):
+        return mmr_numpy(ci, cv, F, int(topk), w)
+    import torch
+    dev = torch.device("cuda", torch.cuda.current_device())
+    h = backend.Serve()
+    try:
+        h.set_items(F)
+        tci, tcv = torch.from_numpy(ci).to(dev), torch.from_numpy(cv).to(dev)
+        return _rerank_batches(h, n, int(topk), w, m, dev, lambda q: (tci[q.long()], tcv[q.long()]))
+    finally:
+        h.close()
+
+
 class Parallel(object):
     def __init__(self, algo, *argv, **kwargs):
         self.algo = algo
@@ -173,6 +304,26 @@ class Parallel(object):
             h.set_queries(np.ascontiguousarray(A[indexes]))
             return h.topk_candidates(np.arange(len(indexes), dtype=np.int32), topk, *cands, seen=seen)
         return cand_topn(indexes, A, B, Bb, topk, *cands, *(seen or ()))
+
+    def _run_diverse(self, indexes, A, B, Bb, topk, div, pool=None, seen=None, cands=None):
+        """_run (or _run_cands with cands) at k = M, then the MMR re-ranking of those M candidates down to topk against
+        the item rows B; div = (w, M) of _check_diversify.  On the device the candidates never leave it."""
+        w, M = div
+        if Bb is not None and not Bb.size:
+            Bb = None
+        if self._on_device(indexes, A, B, M):
+            import torch
+            h = self._serve_handle(B, None if Bb is None else np.ascontiguousarray(Bb, dtype=np.float32))
+            h.set_queries(np.ascontiguousarray(A[indexes]))
+            if cands is None:
+                h.set_pool(None if pool is None or len(pool) == 0 else pool)
+            dev = torch.device("cuda", torch.cuda.current_device())
+            return _rerank_batches(h, len(indexes), topk, w, M, dev, _device_stage(h, M, dev, seen, cands))
+        if cands is not None:
+            keys, scores = self._run_cands(indexes, A, B, Bb, M, cands, seen)
+        else:
+            keys, scores = self._run(indexes, A, B, Bb, M, pool, seen)
+        return mmr_numpy(keys, scores, B, topk, w)
 
 
 class ParALS(Parallel):
@@ -271,7 +422,8 @@ class ParALS(Parallel):
         from buffalo_b200.evaluate.device import _gather_rows
         return _gather_rows(*seen_csr(self.algo, exclude_seen), idx)
 
-    def topk_recommendation(self, keys, topk=10, pool=None, repr=False, exclude_seen=False, nprobe=None):
+    def topk_recommendation(self, keys, topk=10, pool=None, repr=False, exclude_seen=False, nprobe=None,
+                            diversify=None, diversify_candidates=None):
         """pool: None ranks every item; a list of item ids (or an index array) is one candidate pool for every user; a
         scipy sparse (num_users, num_items) matrix gives each user its own candidates, row u (as tocsr() stores it,
         values ignored, duplicates kept, ties to the earlier entry): a user's row of the result is then what a call
@@ -280,8 +432,15 @@ class ParALS(Parallel):
         data); or a scipy sparse (num_users, num_items) matrix whose row u lists the items user u does not get back.
         Rows left with fewer than topk candidates are padded with -1 / 0.0.  nprobe: None ranks every item; an integer
         in [1, nlist] searches the item index (build_index) and ranks the items of the nprobe lists nearest each user,
-        without pool or exclude_seen."""
+        without pool or exclude_seen.  diversify: None ranks by score; a real number w in [0, 1] reranks each user's
+        diversify_candidates best candidates (M, default min(4 topk, 256), in [topk, 256]) by Maximal Marginal
+        Relevance (DESIGN.md 4.15): topk picks, each the candidate of the largest (1 - w) relevance - w largest cosine
+        of its item factors to the picks before it, with the candidates' scores (not sorted).  Every candidate stage
+        above takes it, nprobe does not (rerank_mmr reranks IVF results); w = 0 gives the plain result."""
+        div = _check_diversify(diversify, diversify_candidates, topk)
         if nprobe is not None:
+            if div is not None:
+                raise ValueError("nprobe does not take diversify")
             if pool is not None:
                 raise ValueError("nprobe does not take a pool")
             if scipy.sparse.issparse(exclude_seen) or exclude_seen:
@@ -295,7 +454,10 @@ class ParALS(Parallel):
             from buffalo_b200.evaluate.device import _gather_rows
             cands = _gather_rows(*self._pool_matrix(pool, self.algo.P.shape[0], self.algo.Q.shape[0]), idx)
             seen = self._seen_rows(idx, exclude_seen) if scipy.sparse.issparse(exclude_seen) or exclude_seen else None
-            topks, scores = self._run_cands(idx, self.algo.P, self.algo.Q, Qb, topk, cands, seen)
+            if div is not None:
+                topks, scores = self._run_diverse(idx, self.algo.P, self.algo.Q, Qb, topk, div, seen=seen, cands=cands)
+            else:
+                topks, scores = self._run_cands(idx, self.algo.P, self.algo.Q, Qb, topk, cands, seen)
             if repr:
                 topks = [[self.algo._idmanager.itemids[t] for t in tt if t != -1] for tt in topks]
             return kept, topks, scores
@@ -305,22 +467,30 @@ class ParALS(Parallel):
                                                self._index_bias("item") is not None, False)
         elif scipy.sparse.issparse(exclude_seen) or exclude_seen:
             seen = self._seen_rows(idx, exclude_seen)
-            topks, scores = self._run(idx, self.algo.P, self.algo.Q, Qb, topk, pool, seen)
+            if div is not None:
+                topks, scores = self._run_diverse(idx, self.algo.P, self.algo.Q, Qb, topk, div, pool, seen)
+            else:
+                topks, scores = self._run(idx, self.algo.P, self.algo.Q, Qb, topk, pool, seen)
+        elif div is not None:
+            topks, scores = self._run_diverse(idx, self.algo.P, self.algo.Q, Qb, topk, div, pool)
         else:
             topks, scores = self._run(idx, self.algo.P, self.algo.Q, Qb, topk, pool)
         if repr:
             topks = [[self.algo._idmanager.itemids[t] for t in tt if t != -1] for tt in topks]
         return kept, topks, scores
 
-    def fold_in_recommendation(self, histories, topk=10, pool=None, exclude_seen=True, repr=False):
+    def fold_in_recommendation(self, histories, topk=10, pool=None, exclude_seen=True, repr=False, diversify=None,
+                               diversify_candidates=None):
         """(topks, scores), one row per history row, for users folded into the model (DESIGN.md 4.10): the rows of
         algo.fold_in(histories) with its defaults, ranked against the items as topk_recommendation ranks (pools, -1 / 0.0
         padding).  pool may also be a scipy sparse (n, num_items) matrix: row i lists history row i's own candidates,
         as topk_recommendation takes a per-user pool.  exclude_seen: leave each row's history items out.  All on the device: the folded rows are bound as the
-        serve handle's queries and never reach the host.  Models with fold_in: ALS and PLSI."""
+        serve handle's queries and never reach the host.  diversify / diversify_candidates as topk_recommendation takes
+        them: the folded rows' candidates are reranked on the device too.  Models with fold_in: ALS and PLSI."""
         if not callable(getattr(self.algo, "_fold_in_device", None)):
             raise NotImplementedError("fold_in_recommendation needs a model with fold_in (ALS, PLSI), not %s"
                                       % type(self.algo).__name__)
+        div = _check_diversify(diversify, diversify_candidates, topk)
         topk = backend.Serve._check_k(topk)
         cands = None
         if scipy.sparse.issparse(pool):
@@ -344,14 +514,18 @@ class ParALS(Parallel):
             h.bind_queries(tX)
             h.set_pool(pool)
             qidx = torch.arange(n, dtype=torch.int32, device=tX.device)
-            if cands is not None:
+            if div is not None:
+                topks, scores = _rerank_batches(h, n, topk, div[0], div[1], tX.device, _device_stage(
+                    h, div[1], tX.device, (indptr, keys) if exclude_seen else None, cands))
+            elif cands is not None:
                 cptr, ckeys = (torch.from_numpy(x).to(tX.device) for x in (cands[0], _nonempty(cands[1])))
                 idx, val = h.topk_candidates_device(qidx, topk, cptr, ckeys, seen=(indptr, keys) if exclude_seen else None)
             elif exclude_seen:
                 idx, val = h.topk_seen_device(qidx, topk, indptr, keys)
             else:
                 idx, val = h.topk_device(qidx, topk)
-            topks, scores = idx.cpu().numpy(), val.cpu().numpy()
+            if div is None:
+                topks, scores = idx.cpu().numpy(), val.cpu().numpy()
         finally:
             # the folded rows are freed with this call; every query on the handle sets its own queries first
             h._bound.pop("queries", None)

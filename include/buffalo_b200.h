@@ -423,6 +423,26 @@ int bfl_cand_topk_device(bfl_serve_t* h, const int32_t* d_query_idx, int64_t n, 
 int bfl_cand_set_budget(bfl_serve_t* h, int64_t list_entries);
 
 /* =====================================================================================
+ * Maximal Marginal Relevance re-ranking (DESIGN.md 4.15), on a serve handle: per row, k of its m candidates picked
+ * greedily for relevance against similarity to the items already picked, the diversify option of ParALS / ParBPRMF
+ * topk_recommendation.  Row i's candidates are d_cand_idx[i * m .. i * m + m) (item ids in [0, n_items), -1 pads;
+ * duplicates are ordinary candidates) with their scores d_cand_val (what bfl_serve_topk_device, bfl_seen_topk_device
+ * or bfl_cand_topk_device return at k = m).  Over the row's valid candidates:
+ *  - rel_j = (s_j - s_min) / (s_max - s_min) in fp64, 1 when all scores are equal;
+ *  - cos(a, b) of the item rows the handle holds (its ld and d, no bias): fp32 dot products in the fixed tiled order of
+ *    bfl_eval_ild_device, the cosine in fp64, 0 when either row has zero norm;
+ *  - step t = 0 .. k - 1 picks the unpicked candidate of the largest (1 - w) rel_j - w max_{p picked} cos(p, j) (the
+ *    max term left out at t = 0), ties to the smaller position.
+ * d_out_idx / d_out_val [n x k]: the picks in pick order with their scores bitwise as given (not sorted), -1 / 0.0f
+ * once the valid candidates run out.  diversify = 0 returns the first k candidates of a best-first list.  A row's
+ * output depends on that row alone.  1 <= k <= m <= 256, 0 <= diversify <= 1, n < 2^31; a bad argument is
+ * BFL_ERR_ARG before any launch, a handle without items BFL_ERR_STATE.  DEVICE arrays, stream-ordered on `stream`;
+ * nothing is uploaded and no scratch is allocated.
+ * ===================================================================================== */
+int bfl_mmr_rerank_device(bfl_serve_t* h, const int32_t* d_cand_idx, const float* d_cand_val, int64_t n, int m,
+                          int k, float diversify, int32_t* d_out_idx, float* d_out_val, void* stream);
+
+/* =====================================================================================
  * Inverted-file (IVF-Flat) index for batch serving (DESIGN.md 4.12).  build_device clusters n DEVICE rows (pitch ld,
  * first d columns, d <= 256) by spherical k-means into nlist lists (nlist in [1, min(n, 65536)], iters >= 1): nlist
  * distinct rows drawn with `seed` start it, each row goes to the centroid of the largest dot product (ties to the
