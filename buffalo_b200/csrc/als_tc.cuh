@@ -23,11 +23,11 @@
 //                     is issued whole rows ahead of its use; per tile of 32 entries it writes the gather plan (keys,
 //                     2^e sqrt|w|, w, count / flags) into a 16-slot ring -- it runs up to 8 groups ahead;
 //   4 convert warps  : (a) gathers: one hand-off ahead of its use, warp cw copies the rows cw, cw + 4, ... of a planned
-//                     tile with one coalesced 16-byte-per-lane cp.async per 512 bytes (SASS LDGSTS) into a ring of raw
-//                     fp32 tiles (commit / wait groups + one mbarrier arrival per warp);
+//                     tile with one coalesced 16-byte-per-lane cp.async per 512 bytes (SASS LDGSTS) into a three-stage
+//                     ring (commit / wait groups + one mbarrier arrival per warp);
 //                     (b) convert: thread = feature m: reads column m of the raw tile (conflict-free), scales, splits,
 //                     and writes 16-byte groups of 8 consecutive k into the K-major un-swizzled operand slabs (8 x 16 B
-//                     core matrices, conflict-free); accumulates b_m = sum w q_m (exact fp32) and the loss pieces in
+//                     core matrices, conflict-free) over the group's rows in the same stage; accumulates b_m = sum w q_m (exact fp32) and the loss pieces in
 //                     registers; groups of two full tiles take a branch-free straight-line path;
 //   MMA warpgroup    : executes the generic -> async proxy fence for the group it has acquired, then issues wgmma
 //                     (SASS HGMMA) for the two 64-row halves of the row's matrix, accumulating in registers: rows 64..127
@@ -35,7 +35,8 @@
 //                     symmetric -- split-row chunks accumulate full blocks); entries with negative weight travel in
 //                     their own tiles and are subtracted with the negate-A immediate.  At a row's end it waits for the
 //                     MMAs, stores 2^-2e x accumulator (and the transpose of rows 64..127 x columns 0..63) into the
-//                     shared-memory matrix of the epilogue and reloads 2^2e (G + reg I) for the next row;
+//                     shared-memory matrix of the epilogue and starts the next row from the CTA's shared-memory copy of
+//                     2^2e (G + reg I);
 //   4 epilogue warps : a systolic pipeline over the row's blocks.  Thread j owns matrix row j, warp q column block q:
 //                     h = M x - b from the shared matrix; then warp q folds the deltas of blocks 0..q-1 into its h as
 //                     they are published, runs the 3-step CG of its own 32 x 32 block and publishes its delta.  Nothing in
@@ -68,9 +69,10 @@ constexpr int NXS = 8;     // x buffers of the epilogue pipeline (a fast warp pu
 // Hand-offs are per GROUP of PT consecutive tiles of the CTA's tile stream (a group may span rows: every tile carries its own
 // flags): the barrier round trips of a one-tile hand-off cost as much as the math of a tile.
 constexpr int PT = 2;      // tiles per hand-off group
-constexpr int NR = 2;      // raw stages (groups); the shared-memory matrix of the epilogue leaves no room for a third
-constexpr int NO = 2;      // operand stages (groups)
-constexpr int GATHER_AHEAD = 1;   // groups between a convert warp's gather issue and its use of the group (< NR)
+// Ring of stages (groups): a group's gathered fp32 rows and its operand slabs are both 32 KB and share one stage, which
+// holds the rows of group g + 1 (being gathered), then group g (converted in place), then group g - 1 (read by wgmma)
+constexpr int NS = 3;
+constexpr int GATHER_AHEAD = 1;   // groups between a convert warp's gather issue and its use of the group (< NS - 1)
 constexpr int NPG = 8, NP = NPG * PT;   // gather-plan ring (small slots): the planner runs up to NPG groups ahead
 constexpr int NBV = 8;     // ring of per-row vectors handed from the convert warps to the epilogue
 // d = 128: 32 gathered rows per stage; d = 256 (split-row mode only): 16 rows per stage, and the chunk matrix is
@@ -89,13 +91,26 @@ constexpr uint32_t F_FIRST = 1u << 8, F_LAST = 1u << 9, F_NEG = 1u << 10, F_STOP
 // and the epilogue's reads (thread j reads row j of one column) are both free of bank conflicts
 __device__ __forceinline__ int msw(int c) { return ((c >> 1) & 3) << 3; }
 
+// 2^2e (G + reg I) of a fused launch, packed: the 8 x 8 blocks (R, C) with R >= C, block (R, C) at float
+// 64 (R (R + 1) / 2 + C), element (r, c) at 8 (r % 8) + c % 8 in it (the diagonal blocks are stored whole)
+constexpr int G_FLOATS = 16 * 17 / 2 * 64;
+__device__ __forceinline__ int g_block(int R, int C) { return (R * (R + 1) / 2 + C) * 64; }
+
+template <int D>
+union Stage {
+    // operand slab: element (feature m, entry k) at byte (k/8)*LBO + (m/8)*128 + (m%8)*16 + (k%8)*2
+    unsigned char op[PT][2][Cfg<D>::OP_BYTES];        // [tile of the group][head|tail]
+    float raw[PT][Cfg<D>::TILE * D];                   // gathered rows, pitch D
+};
+static_assert(sizeof(Stage<128>::op) == sizeof(Stage<128>::raw) && sizeof(Stage<256>::op) == sizeof(Stage<256>::raw),
+              "a group's rows and its slabs fill the same stage");
+
 template <int D>
 struct Smem {
     static constexpr int TILE = Cfg<D>::TILE;
-    // operand slab: element (feature m, entry k) at byte (k/8)*LBO + (m/8)*128 + (m%8)*16 + (k%8)*2
-    alignas(1024) unsigned char op[NO][PT][2][Cfg<D>::OP_BYTES];   // [stage][tile of the group][head|tail]
-    alignas(128) float raw[NR][PT][TILE * D];          // gathered rows, pitch D
+    alignas(1024) Stage<D> st[NS];
     alignas(128) float mat[128 * 128];                 // fused mode: M of the row being solved (column-major, msw)
+    alignas(16) float g[G_FLOATS];                     // fused mode: 2^2e (G + reg I), loaded once per CTA
     alignas(16) float bvec[NBV][KH][D];                // b = sum w q
     alignas(16) float sumq[NBV][KH][D];                // sum q (loss only)
     alignas(16) float xs[NXS][D];                      // 128-bit reads: every vector below is 16-byte aligned
@@ -106,9 +121,10 @@ struct Smem {
     alignas(16) int32_t keys[NP][TILE];                //              gathered row per slot
     float wsum[NBV][KH];                               // sum w (loss only)
     uint32_t meta_raw[NP];                             //              count | flags
-    uint32_t meta_op[NO][PT];
+    uint32_t meta_op[NS][PT];
     int badrow[NXS];
-    alignas(8) uint64_t plan_full[NPG], plan_empty[NPG], raw_full[NR], raw_empty[NR], op_full[NO], op_empty[NO];
+    // per stage: raw_full (the group's rows have landed), op_full (converted), st_empty (the MMAs are done with it)
+    alignas(8) uint64_t plan_full[NPG], plan_empty[NPG], raw_full[NS], op_full[NS], st_empty[NS];
     alignas(8) uint64_t acc_full, acc_empty, x_full[NXS], d_full[4];
 };
 // deterministic loss of the fused mode: the epilogue warps' terms of a row, handed to the last block's warp
@@ -116,6 +132,8 @@ template <int D>
 struct SmemDet : Smem<D> {
     double lossp[NXS][4][2];
 };
+// one CTA per SM: 227 KB of shared memory per block on sm_90
+static_assert(sizeof(SmemDet<128>) <= 232448 && sizeof(SmemDet<256>) <= 232448, "shared memory of als_tc_kernel");
 
 // PARTIAL = false: rows of a.row_list[row_begin..row_end) are solved in place.
 // PARTIAL = true : the list holds chunk items of long rows (pairs: row, chunk index); the chunk's matrix and vectors are
@@ -139,7 +157,8 @@ struct TcArgs {
     float* scratch;         // PARTIAL: per slot D*D matrix + D (b) + D (sum q) + 4 (sum w, ...) floats
     int64_t split;          // PARTIAL: chunk length in nnz
     int pass;               // PARTIAL, d = 256: which 128 x 128 block of the chunk matrix this launch accumulates (0..2)
-    int debug;              // BFL_TC_DEBUG (timing experiments only; results are wrong): 1 no gathers, 2 no MMAs, 4 no convert math, 8 no epilogue math, 16 planner only
+    int debug;              // BFL_TC_DEBUG (timing experiments only; results are wrong): 1 no gathers, 2 no MMAs, 4 no convert math, 8 no epilogue math, 16 planner only,
+                            // 32 fused rows start from a zero accumulator instead of 2^2e (G + reg I) (values only: the start is read from shared memory either way)
 };
 
 template <int D>
@@ -192,18 +211,15 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
     const int warp = __shfl_sync(FULL, tid >> 5, 0);
 
     if (tid == 0) {
-        for (int i = 0; i < NR; ++i) {
+        for (int i = 0; i < NS; ++i) {
             // every barrier counts WARPS, not threads: an arrive executed by 32 lanes is 32 serial barrier updates
             mbar_init(&S.raw_full[i], N_CONV);
-            mbar_init(&S.raw_empty[i], N_CONV);
+            mbar_init(&S.op_full[i], N_CONV);
+            mbar_init(&S.st_empty[i], 4);
         }
         for (int i = 0; i < NPG; ++i) {
             mbar_init(&S.plan_full[i], 1);
             mbar_init(&S.plan_empty[i], N_CONV);
-        }
-        for (int i = 0; i < NO; ++i) {
-            mbar_init(&S.op_full[i], N_CONV);
-            mbar_init(&S.op_empty[i], 4);
         }
         mbar_init(&S.acc_full, 4);
         mbar_init(&S.acc_empty, 4);
@@ -214,8 +230,23 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
         }
         mbar_init_fence();
     }
-    __syncthreads();
     const float scale = __ldg(a.tc_scales), inv2 = __ldg(a.tc_scales + 1);
+    if (!PARTIAL) {
+        // the fused rows' accumulator start, the same fp32 values for every row of the launch.  Only the lower block
+        // triangle is kept: G from the Gram kernel is symmetric bit for bit ((i, j) and (j, i) are the same FMAs in the
+        // same order)
+        const float s2 = scale * scale;
+        const bool zero = ta.debug & 32;
+        for (int e = tid; e < 128 * 128; e += THREADS) {
+            const int r = e >> 7, c = e & 127;
+            if ((r >> 3) >= (c >> 3)) {
+                float g = zero ? 0.f : __ldg(a.G + e);
+                g += r == c && !zero ? a.reg : 0.f;
+                S.g[g_block(r >> 3, c >> 3) + 8 * (r & 7) + (c & 7)] = g * s2;
+            }
+        }
+    }
+    __syncthreads();
 
     const int64_t nitems = a.row_end - a.row_begin;
     const int64_t my_first = (int64_t)blockIdx.x;
@@ -424,26 +455,35 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
             if constexpr (PARTIAL) wgmma_m64n128k16_f16<NEG>(d0, adesc, bdesc);
             else wgmma_m64n64k16_f16<NEG>(d0, adesc, bdesc);
         };
-        // a new row's accumulator: 2^2e (G + reg I) in fused mode (so that the epilogue reads one matrix), 0 for chunks
+        // A new row's accumulator: 2^2e (G + reg I) in fused mode (so that the epilogue reads one matrix), 0 for chunks.
+        // acc_init_nh sets the registers of (n, h): elements (fr + 8 h, 8 n + fc + i) of d0 and (fr + 8 h + 64, ...) of d1,
+        // from S.g; an element above the block diagonal is read from its mirror.  The block row of fr is warp-uniform.
+        const int rb = 2 * wq;
+        const int g_lo = 8 * (lane >> 2) + fc, g_up = 8 * fc + (lane >> 2);   // offsets in a block below / above
+        auto g_pair = [&](int R, int C) -> float2 {   // elements (8 R + lane / 4, 8 C + fc + {0, 1})
+            const bool low = R >= C;
+            const float* p = S.g + (low ? g_block(R, C) + g_lo : g_block(C, R) + g_up);
+            return make_float2(p[0], p[low ? 1 : 8]);
+        };
+        auto acc_init_nh = [&](const int n, const int h) {
+            if constexpr (PARTIAL) {
+                d0[4 * n + 2 * h] = 0.f; d0[4 * n + 2 * h + 1] = 0.f;
+                d1[4 * n + 2 * h] = 0.f; d1[4 * n + 2 * h + 1] = 0.f;
+            } else {
+                if (8 * n < N0) {
+                    const float2 g0 = g_pair(rb + h, n);
+                    d0[4 * n + 2 * h] = g0.x; d0[4 * n + 2 * h + 1] = g0.y;
+                }
+                const float2 g1 = n < 8 ? *reinterpret_cast<const float2*>(S.g + g_block(8 + rb + h, n) + g_lo)
+                                        : g_pair(8 + rb + h, n);
+                d1[4 * n + 2 * h] = g1.x; d1[4 * n + 2 * h + 1] = g1.y;
+            }
+        };
         auto acc_init = [&]() {
-            const float s2 = scale * scale;
 #pragma unroll
             for (int n = 0; n < 16; ++n)
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int r = fr + 8 * h, c = 8 * n + fc;
-                    float2 g0 = make_float2(0.f, 0.f), g1 = make_float2(0.f, 0.f);
-                    if (!PARTIAL) {
-                        if (8 * n < N0) g0 = __ldg(reinterpret_cast<const float2*>(a.G + (size_t)r * D + c));
-                        g1 = __ldg(reinterpret_cast<const float2*>(a.G + (size_t)(r + 64) * D + c));
-                        g0.x += r == c ? a.reg : 0.f;
-                        g0.y += r == c + 1 ? a.reg : 0.f;
-                        g1.x += r + 64 == c ? a.reg : 0.f;
-                        g1.y += r + 64 == c + 1 ? a.reg : 0.f;
-                    }
-                    if (8 * n < N0) { d0[4 * n + 2 * h] = g0.x * s2; d0[4 * n + 2 * h + 1] = g0.y * s2; }
-                    d1[4 * n + 2 * h] = g1.x * s2; d1[4 * n + 2 * h + 1] = g1.y * s2;
-                }
+                for (int h = 0; h < 2; ++h) acc_init_nh(n, h);
         };
         uint32_t os = 0, oph = 0, aph = 0;
         int64_t seq = 0;   // rows (items) finished so far
@@ -460,7 +500,7 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                     break;
                 }
                 const int ksteps = (ta.debug & 2) ? 0 : (int)(meta & 0xffu);
-                const uint32_t hi = s32(&S.op[os][e][0][0]), lo = s32(&S.op[os][e][1][0]);
+                const uint32_t hi = s32(&S.st[os].op[e][0][0]), lo = s32(&S.st[os].op[e][1][0]);
                 wgmma_fence();
 #pragma unroll 1
                 for (int ks = 0; ks < ksteps; ++ks) {
@@ -522,11 +562,14 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                                         }
                                     }
                                 }
+                        acc_init();
                     } else {
+                        // the next row's start is loaded into each register pair right after its last store, so that the
+                        // shared-memory loads overlap the stores
 #pragma unroll
                         for (int n = 0; n < 16; ++n)
 #pragma unroll
-                            for (int h = 0; h < 2; ++h)
+                            for (int h = 0; h < 2; ++h) {
 #pragma unroll
                                 for (int i = 0; i < 2; ++i) {
                                     const int r = fr + 8 * h, c = 8 * n + fc + i;
@@ -537,20 +580,21 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                                         S.mat[(r + 64) * 128 + (c ^ msw(r + 64))] = v1;
                                     }
                                 }
+                                acc_init_nh(n, h);
+                            }
                     }
                     __syncwarp();
                     if (lane == 0) mbar_arrive(&S.acc_full);
                     aph ^= 1u;
                     ++seq;
-                    acc_init();
                 }
             }
             wgmma_wait<0>();   // the group's operand reads are done
 #pragma unroll
             for (int i = 0; i < 64; ++i) { if (i < N0 / 2) acc_fence(d0[i]); acc_fence(d1[i]); }
             __syncwarp();
-            if (lane == 0) mbar_arrive(&S.op_empty[os]);   // (after a stop nobody waits for it any more)
-            if (++os == NO) { os = 0; oph ^= 1u; }
+            if (lane == 0) mbar_arrive(&S.st_empty[os]);   // (after a stop nobody waits for it any more)
+            if (++os == NS) { os = 0; oph ^= 1u; }
         }
     } else if (warp >= W_CONV && warp < W_CONV + N_CONV) {
         // ================= convert: raw fp32 -> scaled fp16 head/tail operand slabs =================
@@ -560,7 +604,7 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
         const int ct = cta & 127;          // feature(s) of this thread
         const int kh = cta >> 7;           // which part of a tile's entries this convert set takes
         constexpr int CHS = TILE / 8 / KH; // 8-entry chunks per tile and set
-        uint32_t rs = 0, rph = 0, os = 0, oph = 0, bslot = 0;
+        uint32_t rs = 0, rph = 0, bslot = 0;   // stage of the group being converted
         float2 bacc[NF], qacc[NF];
         float wacc = 0.f;
 #pragma unroll
@@ -572,7 +616,7 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
         // commit group per group; before converting a group a warp waits for its own copies (cp.async.wait_group) and
         // posts one arrival on the stage's mbarrier.
         const int cw = cta >> 5;
-        uint32_t gs = 0, gph = 0, grs = 0, grph = 0;   // plan group slot / raw stage of the next group to gather
+        uint32_t gs = 0, gph = 0, grs = 0, grph = 0;   // plan group slot / stage of the next group to gather
         bool plan_end = false;
         auto gather = [&]() {
             if (plan_end) {
@@ -580,7 +624,7 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                 return;
             }
             mbar_wait(&S.plan_full[gs], gph);
-            mbar_wait(&S.raw_empty[grs], grph ^ 1u);   // every convert warp is done with the group that used this stage
+            mbar_wait(&S.st_empty[grs], grph ^ 1u);   // the MMAs are done with the group that used this stage
             const uint32_t gm0 = S.meta_raw[gs * PT], gm1 = S.meta_raw[gs * PT + 1];
             if (PT == 2 && !(ta.debug & 1) && ((gm0 | gm1) & F_STOP) == 0 && (gm0 & 0xffu) == TILE && (gm1 & 0xffu) == TILE) {
                 // two full tiles (the common case): straight-line copies, no per-row predicates
@@ -594,7 +638,7 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
 #pragma unroll
                     for (int i = 0; i < TILE / N_CONV; ++i) {
                         const float* src = a.Y + (int64_t)kk[e][i] * a.ld + lane * 4;
-                        float* dst = &S.raw[grs][e][(cw + N_CONV * i) * D + lane * 4];
+                        float* dst = &S.st[grs].raw[e][(cw + N_CONV * i) * D + lane * 4];
 #pragma unroll
                         for (int c = 0; c < D / 128; ++c) cp_async16_cg(dst + c * 128, src + c * 128);
                     }
@@ -611,7 +655,7 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                         const int slot = cw + N_CONV * i;
                         if (slot < gcnt) {
                             const float* src = a.Y + (int64_t)S.keys[gs * PT + e][slot] * a.ld + lane * 4;
-                            float* dst = &S.raw[grs][e][slot * D + lane * 4];
+                            float* dst = &S.st[grs].raw[e][slot * D + lane * 4];
 #pragma unroll
                             for (int c = 0; c < D / 128; ++c) cp_async16_cg(dst + c * 128, src + c * 128);
                         }
@@ -620,7 +664,7 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
             }
             cp_async_commit();
             if (++gs == NPG) { gs = 0; gph ^= 1u; }
-            if (++grs == NR) { grs = 0; grph ^= 1u; }
+            if (++grs == NS) { grs = 0; grph ^= 1u; }
         };
         uint32_t cs = 0;   // plan group slot of the group being converted
         bool done = false;
@@ -658,8 +702,9 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                     for (int i = 0; i < 8; ++i)
 #pragma unroll
                         for (int f = 0; f < NF; ++f)
-                            qv[e][(c * 8 + i) * NF + f] = S.raw[rs][e][((kh * CHS + c) * 8 + i) * D + ct + 128 * f];
-            mbar_wait(&S.op_empty[os], oph ^ 1u);
+                            qv[e][(c * 8 + i) * NF + f] = S.st[rs].raw[e][((kh * CHS + c) * 8 + i) * D + ct + 128 * f];
+            // the slabs overwrite the rows in place: every convert thread has read its rows of the group first
+            named_bar_sync(1, N_CONV * 32);
             const uint32_t cm0 = S.meta_raw[cs * PT], cm1 = S.meta_raw[cs * PT + 1];
             const bool fast2 = PT == 2 && !(ta.debug & 4) && ((cm0 | cm1) & F_STOP) == 0 && (cm0 & 0xffu) == TILE &&
                                (cm1 & 0xffu) == TILE;
@@ -678,8 +723,8 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                         qacc[f].x = first ? 0.f : qacc[f].x; qacc[f].y = first ? 0.f : qacc[f].y;
                     }
                     wacc = first ? 0.f : wacc;
-                    unsigned char* hi = &S.op[os][e][0][0];
-                    unsigned char* lo = &S.op[os][e][1][0];
+                    unsigned char* hi = &S.st[rs].op[e][0][0];
+                    unsigned char* lo = &S.st[rs].op[e][1][0];
 #pragma unroll
                     for (int c = 0; c < CHS; ++c) {
                         const int kc = kh * CHS + c, k0 = kc * 8;
@@ -721,7 +766,7 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                     }
                     if (LOSS1 && ct == 0) S.wsum[bslot][kh] = wacc;
                     bslot = (bslot + ((meta & F_LAST) ? 1u : 0u)) & (NBV - 1);
-                    if (cta == 0) S.meta_op[os][e] = (uint32_t)(TILE / 16) | (meta & (F_FIRST | F_LAST | F_NEG));
+                    if (cta == 0) S.meta_op[rs][e] = (uint32_t)(TILE / 16) | (meta & (F_FIRST | F_LAST | F_NEG));
                 }
             } else
 #pragma unroll
@@ -730,7 +775,7 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                 const uint32_t psl = cs * PT + e;   // the tile's plan slot
                 const uint32_t meta = S.meta_raw[psl];
                 if (meta & F_STOP) {
-                    if (cta == 0) S.meta_op[os][e] = F_STOP;
+                    if (cta == 0) S.meta_op[rs][e] = F_STOP;
                     done = true;
                     continue;
                 }
@@ -740,8 +785,8 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                     for (int f = 0; f < NF; ++f) { bacc[f] = make_float2(0.f, 0.f); qacc[f] = make_float2(0.f, 0.f); }
                     wacc = 0.f;
                 }
-                unsigned char* hi = &S.op[os][e][0][0];
-                unsigned char* lo = &S.op[os][e][1][0];
+                unsigned char* hi = &S.st[rs].op[e][0][0];
+                unsigned char* lo = &S.st[rs].op[e][1][0];
                 // one chunk = 8 consecutive entries k of this thread's feature(s): a 16-byte group of the head and of the
                 // tail slab.  GUARD: the tile is not full -- slots >= cnt hold stale rows (scale and weight 0 from the
                 // planner; the value is zeroed as well so that a stale Inf/NaN cannot leak into an unrelated row).
@@ -801,20 +846,18 @@ __global__ void __launch_bounds__(THREADS, 1) als_tc_kernel(TcArgs ta) {
                     if (LOSS1 && ct == 0) S.wsum[bslot][kh] = wacc;
                     bslot = (bslot + 1) & (NBV - 1);
                 }
-                if (cta == 0) S.meta_op[os][e] = (uint32_t)ksteps | (meta & (F_FIRST | F_LAST | F_NEG));
+                if (cta == 0) S.meta_op[rs][e] = (uint32_t)ksteps | (meta & (F_FIRST | F_LAST | F_NEG));
             }
             // (no proxy fence here: FENCE.VIEW.ASYNC in a thread with cp.async / global loads in flight waits for them -- the
             // next groups' gathers -- so the generic->async proxy fence is executed by the MMA-issuing warp after it has
             // acquired the group through op_full)
             __syncwarp();
-            if (lane == 0) {   // one arrival per warp on each of the three hand-offs of a group
-                mbar_arrive(&S.raw_empty[rs]);
+            if (lane == 0) {   // one arrival per warp on each of the two hand-offs of a group
                 mbar_arrive(&S.plan_empty[cs]);
-                mbar_arrive(&S.op_full[os]);
+                mbar_arrive(&S.op_full[rs]);
             }
             cs = (cs + 1) & (NPG - 1);
-            if (++rs == NR) { rs = 0; rph ^= 1u; }
-            if (++os == NO) { os = 0; oph ^= 1u; }
+            if (++rs == NS) { rs = 0; rph ^= 1u; }
         }
     } else {
         // ================= epilogue: explicit-matrix block Gauss-Seidel / CG, systolic over the blocks of a row =================

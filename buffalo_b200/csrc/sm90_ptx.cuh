@@ -52,6 +52,11 @@ __device__ __forceinline__ void cp_async_bulk_g2s(void* smem_dst, const void* gs
                  : "memory");
 }
 
+// barrier `id` (1..15; 0 is __syncthreads) of the first `nthreads` threads that reach it, a multiple of 32
+__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+
 // generic-proxy writes to shared memory -> visible to the async proxy (tensor-core operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
