@@ -95,7 +95,7 @@ def plsi_kernel_seconds(m, H, iters, repeats):
     vdim = st.holder.get_vdim()
     X0 = fold_in.start_rows(None, len(indptr), m.opt.d, 1.0 / m.opt.d)
     ind_t, keys_t, vals_t, tX = fold_in.to_device(indptr, keys, vals, X0, vdim)
-    run = lambda: st.holder.fold_in_device(st.Q, ind_t, keys_t, vals_t, tX, iters, m.opt.alpha1)
+    run = lambda: st.holder.fold_in_device(st.F, ind_t, keys_t, vals_t, tX, iters, m.opt.alpha1)
     run()
     best = []
     for _ in range(repeats):

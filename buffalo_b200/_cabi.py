@@ -81,6 +81,8 @@ PROTOTYPES = {
     "bfl_sgd_read_stats": (C.c_int, [_vp, _pd, _pi64]),
     "bfl_sgd_reduce_items_device": (C.c_int, [_vp, _vp]),
     "bfl_sgd_segment_len": (C.c_int, []),
+    "bfl_sgd_fold_in_items_device": (C.c_int, [_vp, _vp, _i64, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _i64,
+                                               _vp, _vp, C.c_int, _vp, _vp, _vp]),
     # PLSI
     "bfl_plsi_create": (_vp, []),
     "bfl_plsi_destroy": (None, [_vp]),

@@ -117,18 +117,50 @@ class ALS(Algo, ALSOption, Evaluable, Serializable):
                     h.update_device(0, 0, n, loss)
             finally:
                 # the rows and the CSR belong to this call and are freed with its results (every call binds its own
-                # before it solves); the holder keeps only its scratch, the resident Q is st.Q
+                # before it solves); the holder keeps only its scratch, the resident Q is st.F
                 h._keep = []
         return tX, (ind_t, keys_t, vals_t)
 
     @staticmethod
     def _bind_fold_items(st, h, X):
         """Binds rows X and the state's resident Q to the fold-in holder h, with the Gram of this Q computed once."""
-        h.bind_factors(X, st.Q)
+        h.bind_factors(X, st.F)
+        ALS._fold_gram(st, h, 0)
+
+    @staticmethod
+    def _fold_gram(st, h, axis):
+        """The Gram of the state's resident factors, computed on the holder once per upload of them."""
         if st.derived_key != st.key:
             st.derived_key = None
-            h.precompute_device(0)
+            h.precompute_device(axis)
             st.derived_key = st.key
+
+    def fold_in_items(self, histories, init=None, sweeps=1):
+        """float32 [n, d] item rows for n new items, with the user factors fixed: `sweeps` applications of the row
+        solve that train()'s item half-epoch applies (the model's optimizer and options -- reg_i, adaptive_reg with the
+        item's entry count, the split-row path for long rows -- against the Gram of the current P).  histories: a scipy
+        sparse (n, num_users) matrix in the units of the training data, or a list of n lists of user ids (unknown ids
+        dropped, value 1.0).  init: None (zero rows) or an (n, d) array of start rows.  Rows without history keep their
+        start row.  P, Q and the training holder are not written; serve the rows with add_items().  The padded P and its
+        Gram stay on the device between calls until P or the options change (rows * vdim * 4 bytes: 5 GB at 10M users
+        and d = 128).  On the GPU only: without one the backend's "no CPU fallback" error is raised."""
+        if self.opt._nrz_P:
+            raise RuntimeError("Cannot fold in items with normalized user factors")
+        sweeps = fold_in.positive_int(sweeps, "sweeps")
+        st, h, (ind_t, keys_t, vals_t, tX) = fold_in.begin(self, CuALS, histories, init, 0.0, side="P")
+        n = tX.shape[0]
+        if n:
+            import torch
+            try:
+                h.bind_factors(st.F, tX)
+                h.bind_csr(1, ind_t, keys_t, vals_t)
+                self._fold_gram(st, h, 1)
+                loss = torch.zeros(2, dtype=torch.float64, device=tX.device)
+                for _ in range(sweeps):
+                    h.update_device(1, 0, n, loss)
+            finally:
+                h._keep = []
+        return tX[:, :self.opt.d].cpu().numpy()
 
     # ---- explanations (DESIGN.md 4.11) --------------------------------------------------------
     EXPLAIN_DMAX, EXPLAIN_KMAX, EXPLAIN_TOPM_MAX = 256, 4096, 64
@@ -157,7 +189,7 @@ class ALS(Algo, ALSOption, Evaluable, Serializable):
         num_items = self.Q.shape[0]
         indptr, keys, vals = fold_in.history_csr(self, histories, num_items)
         targets = fold_in.target_matrix(self, items, len(indptr), num_items, self.EXPLAIN_KMAX)
-        st, h = fold_in.item_state(self, CuALS)
+        st, h = fold_in.resident_state(self, CuALS)
         n, k = targets.shape
         if n == 0 or k == 0:
             return (np.zeros((n, k), np.float32), np.full((n, k, topm), -1, np.int32),
@@ -243,6 +275,7 @@ class ALS(Algo, ALSOption, Evaluable, Serializable):
         return rmse
 
     def train(self, training_callback=None):
+        self._check_catalogue()
         if self.P.shape[1] != self.vdim:      # factors replaced by the user at width d: re-pad
             for name in ("P", "Q"):
                 F = getattr(self, name)

@@ -166,6 +166,56 @@ class Algo(abc.ABC):
             idx = []
         return np.array(idx) if many else idx[0]
 
+    # ---- new items (DESIGN.md 4.16) ------------------------------------------------------------
+    def add_items(self, ids, rows, bias=None):
+        """Serves new items: appends `rows` (n, d) to Q and their names `ids` to the item-id map (built from the data
+        first if it has not been), and for models with item biases (BPRMF, WARP) `bias` (n,) to Qb, 0 when None.  The
+        rows are what fold_in_items returns; under normalize("item") they are normalized too, so cosines stay
+        consistent.  Every query path then sees the new items; an item index built before the call reports itself
+        stale.  Raises ValueError, changing nothing, on duplicate or already-known ids, a wrong shape, non-finite values
+        or a bias for a model without item biases.  A later train() needs data with the grown catalogue."""
+        if not isinstance(ids, (list, tuple, np.ndarray)):
+            raise ValueError("ids must be a list of item ids, got %s" % type(ids).__name__)
+        ids = list(ids)
+        if len(set(ids)) != len(ids):
+            raise ValueError("ids hold duplicates")
+        if not self._idmanager.itemid_mapped:
+            self.build_itemid_map()
+        known = [i for i in ids if i in self._idmanager.itemid_map]
+        if known:
+            raise ValueError("ids already known: %s" % known[:10])
+        n, d = len(ids), self.opt.d
+        X = np.asarray(rows, dtype=np.float32)
+        if X.shape != (n, d):
+            raise ValueError("rows must be (%d, %d), got %s" % (n, d, X.shape))
+        if not np.isfinite(X).all():
+            raise ValueError("rows hold non-finite values")
+        has_bias = getattr(self, "Qb", None) is not None
+        if bias is not None and not has_bias:
+            raise ValueError("this model has no item biases")
+        b = np.zeros(n, np.float32) if bias is None else np.asarray(bias, dtype=np.float32)
+        if b.shape != (n,):
+            raise ValueError("bias must be (%d,), got %s" % (n, b.shape))
+        if not np.isfinite(b).all():
+            raise ValueError("bias holds non-finite values")
+        if self.opt._nrz_Q:
+            X = self._normalize(X).astype(np.float32)
+        G = np.zeros((n, self.Q.shape[1]), np.float32)
+        G[:, :d] = X
+        self.Q = np.ascontiguousarray(np.vstack([self.Q, G]), dtype=np.float32)
+        if has_bias:
+            self.Qb = np.ascontiguousarray(np.vstack([np.asarray(self.Qb, np.float32).reshape(-1, 1), b[:, None]]))
+        start = len(self._idmanager.itemids)
+        self._idmanager.itemids = list(self._idmanager.itemids) + ids
+        self._idmanager.itemid_map.update({v: start + i for i, v in enumerate(ids)})
+
+    def _check_catalogue(self):
+        """train() on data whose item count no longer matches Q (after add_items) would index past the factors."""
+        num_items = self.data.get_header()["num_items"]
+        if getattr(self, "Q", None) is not None and self.Q.shape[0] != num_items:
+            raise ValueError("Q has %d rows but the data has %d items: items were added with add_items; train on data "
+                             "that includes them, or call initialize() to start again" % (self.Q.shape[0], num_items))
+
     def get_index_pool(self, pool, group="item"):
         if isinstance(pool, list):
             pool = np.array([p for p in self.get_index(pool, group) if p is not None])

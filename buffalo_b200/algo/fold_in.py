@@ -1,21 +1,24 @@
-"""Folding-in (DESIGN.md 4.10): the host side that ALS.fold_in, PLSI.fold_in and ALS.explain (4.11) share.
+"""Folding-in (DESIGN.md 4.10, 4.16): the host side that ALS.fold_in, PLSI.fold_in, ALS.explain (4.11) and the item
+fold-ins (ALS / BPRMF / WARP .fold_in_items) share.
 
-A fold-in computes user rows from their histories with the model's item factors held fixed.  This module turns the
-caller's histories and start rows into checked host arrays (before any device work), keeps the model's item factors on
+A user fold-in computes user rows from their histories with the model's item factors held fixed; an item fold-in
+computes item rows from the users who interacted with them, with the user factors held fixed.  This module turns the
+caller's histories and start rows into checked host arrays (before any device work), keeps the fixed side's factors on
 the device, padded to the holder's row pitch and uploaded again only when their bits change, and moves one call's
-histories to the device as one CSR.  The solves themselves are the models' (als.py, plsi.py)."""
+histories to the device as one CSR.  The solves themselves are the models' (als.py, plsi.py, bpr.py)."""
 import json
 
 import numpy as np
 import scipy.sparse
 
 
-def history_csr(algo, histories, num_items):
-    """(END offsets int64 [n], keys int32, vals float32) host arrays of the histories:
+def history_csr(algo, histories, num_items, group="item"):
+    """(END offsets int64 [n], keys int32, vals float32) host arrays of the histories; `group` is what the columns are
+    ("item" for user fold-in, "user" for item fold-in, where num_items is the number of users):
       * a scipy sparse (n, num_items) matrix, read after tocsr() / sort_indices() (on a copy: the caller's matrix is not
-        changed), so each row's entries are in ascending item order; values in the units of the training data;
-      * or a list of n lists of item ids, mapped through the model's item-id map; unknown ids are dropped, every entry
-        has the value 1.0 and each row is put in ascending item order.
+        changed), so each row's entries are in ascending column order; values in the units of the training data;
+      * or a list of n lists of ids, mapped through the model's id map of `group`; unknown ids are dropped, every entry
+        has the value 1.0 and each row is put in ascending column order.
     Raises ValueError on a wrong column count, a key outside [0, num_items) or another input type."""
     if scipy.sparse.issparse(histories):
         if histories.ndim != 2 or histories.shape[1] != num_items:
@@ -25,17 +28,17 @@ def history_csr(algo, histories, num_items):
         nnz = int(m.indptr[-1])
         keys = np.asarray(m.indices[:nnz])
         if keys.size and (int(keys.min()) < 0 or int(keys.max()) >= num_items):
-            raise ValueError("histories hold an item outside [0, %d)" % num_items)
+            raise ValueError("histories hold a%s %s outside [0, %d)" % ("n" if group == "item" else "", group, num_items))
         return (np.ascontiguousarray(m.indptr[1:], dtype=np.int64), np.ascontiguousarray(keys, dtype=np.int32),
                 np.ascontiguousarray(m.data[:nnz], dtype=np.float32))
     if not isinstance(histories, (list, tuple)):
-        raise ValueError("histories must be a scipy sparse matrix or a list of lists of item ids, got %s"
-                         % type(histories).__name__)
+        raise ValueError("histories must be a scipy sparse matrix or a list of lists of %s ids, got %s"
+                         % (group, type(histories).__name__))
     rows = []
     for h in histories:
         if not isinstance(h, (list, tuple, np.ndarray)):
-            raise ValueError("every history must be a list of item ids, got %s" % type(h).__name__)
-        idx = algo.get_index(list(h), group="item") if len(h) else []
+            raise ValueError("every history must be a list of %s ids, got %s" % (group, type(h).__name__))
+        idx = algo.get_index(list(h), group=group) if len(h) else []
         rows.append(np.sort(np.array([i for i in idx if i is not None], dtype=np.int64), kind="stable"))
     lens = np.array([len(r) for r in rows], dtype=np.int64)
     keys = np.concatenate(rows).astype(np.int32) if rows else np.zeros(0, np.int32)
@@ -91,14 +94,17 @@ def positive_int(value, name):
 
 
 class ItemState(object):
-    """A model's fold-in state on the device: a backend holder of its own, made from the model's options, and the item
-    factors Q padded to the holder's row pitch (padding columns zero).  `key` is the checksum of Q's bits (the rule of
-    Parallel._fingerprint) and the options; refresh() uploads Q again, and marks derived data such as the ALS Gram
-    stale, when either changed: normalize(), a second train() or an in-place edit."""
+    """A model's fold-in state on the device for one fixed side: a backend holder of its own, made from the model's
+    options, and that side's factors F padded to the holder's row pitch (padding columns zero) -- Q for user fold-in, P
+    for item fold-in (resident_state).  `key` is the checksum of F's bits (the rule of Parallel._fingerprint) and the
+    options; refresh() uploads F again, and marks derived data such as the ALS Gram stale, when either changed:
+    normalize(), a second train() or an in-place edit.  F costs rows * vdim * 4 bytes of device memory for as long as
+    the model lives (P at 10M users and d = 128: 5 GB)."""
 
     def __init__(self):
-        self.key = self.okey = self.holder = self.Q = None
-        self.derived_key = None          # key the holder's derived item data (the ALS Gram) was computed for
+        self.key = self.okey = self.holder = self.F = None
+        self.derived_key = None          # key the holder's derived data (the ALS Gram) was computed for
+        self.extra = {}                  # name -> (key, device arrays) kept between calls: cached()
 
     @staticmethod
     def make_holder(make, opt):
@@ -107,40 +113,71 @@ class ItemState(object):
             raise ValueError("fold_in: the model's options were refused: %s" % getattr(holder, "last_error", ""))
         return holder
 
-    def refresh(self, make, opt, Q):
+    def refresh(self, make, opt, F):
         """make: the holder class; returns the holder.  Without a GPU, creating the holder raises the backend's
         "no CPU fallback" error."""
-        from buffalo_b200.parallel.base import Parallel
         okey = json.dumps(opt, sort_keys=True, default=str)
         if self.holder is None or self.okey != okey:
-            self.holder, self.okey, self.key, self.derived_key, self.Q = self.make_holder(make, opt), okey, None, None, None
-        key = Parallel._fingerprint(np.ascontiguousarray(Q, dtype=np.float32))
+            self.holder, self.okey, self.key, self.derived_key, self.F = self.make_holder(make, opt), okey, None, None, None
+            self.extra = {}
+        key = fingerprint(F)
         if self.key != key:
-            import torch
-            vdim, d = self.holder.get_vdim(), int(opt["d"])
-            self.Q, self.key = None, None
-            T = torch.zeros((Q.shape[0], vdim), dtype=torch.float32, device=device())
-            T[:, :d] = torch.from_numpy(np.ascontiguousarray(Q[:, :d], dtype=np.float32)).to(T.device)
-            self.Q, self.key = T, key
+            self.F, self.key = None, None
+            self.F, self.key = padded(F, self.holder.get_vdim(), int(opt["d"])), key
         return self.holder
 
+    def cached(self, name, key, build):
+        """The device arrays build() returns, kept under `name` until a call brings another `key` (or the options
+        change)."""
+        old = self.extra.pop(name, None)
+        if old is not None and old[0] == key:
+            self.extra[name] = old
+            return old[1]
+        value = build()
+        self.extra[name] = (key, value)
+        return value
 
-def begin(model, make, histories, init, fill):
+
+def fingerprint(A):
+    """Checksum of the bits of A as float32 / its own dtype (the rule of Parallel._fingerprint)."""
+    from buffalo_b200.parallel.base import Parallel
+    A = np.asarray(A)
+    A = np.ascontiguousarray(A, dtype=np.float32) if A.dtype.kind == "f" else np.ascontiguousarray(A)
+    return Parallel._fingerprint(A.reshape(A.shape[0], -1) if A.ndim else A.reshape(1, 1))
+
+
+def padded(F, vdim, d):
+    """torch CUDA float32 [rows, vdim]: F's first d columns, zero padding."""
+    import torch
+    T = torch.zeros((F.shape[0], vdim), dtype=torch.float32, device=device())
+    T[:, :d] = torch.from_numpy(np.ascontiguousarray(F[:, :d], dtype=np.float32)).to(T.device)
+    return T
+
+
+def begin(model, make, histories, init, fill, side="Q"):
     """The common start of a model's fold-in: the checked host input (histories, start rows filled with `fill` when
-    init is None), then the model's ItemState refreshed for its current Q with a holder from `make`, and the call's
-    device arrays.  Returns (state, holder, (indptr, keys, vals, X) as to_device gives them)."""
-    indptr, keys, vals = history_csr(model, histories, model.Q.shape[0])
+    init is None), then the model's state for the fixed `side` ("Q": user fold-in, "P": item fold-in) refreshed with a
+    holder from `make`, and the call's device arrays.  Returns (state, holder, (indptr, keys, vals, X) as to_device
+    gives them)."""
+    indptr, keys, vals = history_csr(model, histories, *columns(model, side))
     X0 = start_rows(init, len(indptr), model.opt.d, fill)
-    st, h = item_state(model, make)
+    st, h = resident_state(model, make, side)
     return st, h, to_device(indptr, keys, vals, X0, h.get_vdim())
 
 
-def item_state(model, make):
-    """(the model's ItemState, its holder), refreshed for the model's current Q and options."""
-    if getattr(model, "_fold_state", None) is None:
-        model._fold_state = ItemState()
-    st = model._fold_state
-    return st, st.refresh(make, model.opt, model.Q)
+def columns(model, side):
+    """(column count, id group) of the histories of a fold-in against the fixed `side`."""
+    return (model.Q.shape[0], "item") if side == "Q" else (model.P.shape[0], "user")
+
+
+def resident_state(model, make, side="Q"):
+    """(the model's ItemState for the fixed `side`, its holder), refreshed for the model's current factors of that side
+    and its options.  The two sides keep separate states: their holders hold different Grams."""
+    attr = "_fold_state" if side == "Q" else "_fold_state_items"
+    if getattr(model, attr, None) is None:
+        setattr(model, attr, ItemState())
+    st = getattr(model, attr)
+    return st, st.refresh(make, model.opt, model.Q if side == "Q" else model.P)
 
 
 def device():

@@ -138,7 +138,7 @@ class PLSI(Algo, PLSIOption, Evaluable, Serializable):
         """fold_in's rows as a torch CUDA tensor [n, vdim] (padding zero), and the histories' device CSR."""
         iters = fold_in.positive_int(self.opt.num_iters if iters is None else iters, "iters")
         st, h, (ind_t, keys_t, vals_t, tX) = fold_in.begin(self, CuPLSI, histories, init, 1.0 / self.opt.d)
-        h.fold_in_device(st.Q, ind_t, keys_t, vals_t, tX, iters, self.opt.alpha1)
+        h.fold_in_device(st.F, ind_t, keys_t, vals_t, tX, iters, self.opt.alpha1)
         return tX, (ind_t, keys_t, vals_t)
 
     # ---- training -----------------------------------------------------------------------------

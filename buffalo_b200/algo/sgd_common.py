@@ -75,6 +75,7 @@ class SGDTrainerMixin(object):
         return loss
 
     def train(self, training_callback=None):
+        self._check_catalogue()
         self.validation_result = {}
         self.sampling_loss_samples()
         self._prepare_train()

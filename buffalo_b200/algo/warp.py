@@ -21,8 +21,8 @@ class WARP(BPRMF):
     def new(path, data_fields=[]):
         return WARP.instantiate(WARPOption, path, data_fields)
 
-    def _draw(self, rows, cols):
-        return np.random.normal(scale=1.0 / (self.opt.d ** 2), size=(rows, cols)).astype("float32")   # warp.py:83-88 (signed)
+    def _draw(self, rows, cols, rng=np.random):
+        return rng.normal(scale=1.0 / (self.opt.d ** 2), size=(rows, cols)).astype("float32")   # warp.py:83-88 (signed)
 
     def prepare_sampling(self):
         pass  # warp.py:72-77: uniform negatives only

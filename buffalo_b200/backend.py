@@ -327,6 +327,30 @@ class CuSGD(_Holder):
         """Samples / item entries per segment of the deterministic user and item sums."""
         return _cabi.lib().bfl_sgd_segment_len()
 
+    def fold_in_items_device(self, P, Q, Qb, train_indptr, train_keys, cum, indptr, users, X, Xb, epochs, trace=None,
+                             stream=None):
+        """Item fold-in (bfl_sgd_fold_in_items_device): `epochs` epochs of training's item side on the rows X [n, vdim]
+        and biases Xb [n] (start values in, results out) with P, Q [rows, vdim] and Qb [Q rows] frozen.  train_indptr /
+        train_keys: the training data's rowwise CSR (int64 END offsets, int32 items); cum: the int64 popularity table or
+        None for uniform negatives; indptr / users: the new rows' END offsets and int32 user ids.  trace: None or
+        (negs, trials) int32 tensors [epochs, nnz * samples per positive] / [epochs, nnz] (trials None for BPR).  All
+        torch CUDA tensors."""
+        self._check_vdim(P, X)
+        if Q.shape[1] != P.shape[1] or Qb.numel() != Q.shape[0] or Xb.numel() != X.shape[0]:
+            raise ValueError("Q must be [rows, %d] with one Qb entry per row, and Xb one entry per row of X"
+                             % P.shape[1])
+        if indptr.shape[0] != X.shape[0]:
+            raise ValueError("indptr must hold one END offset per row of X (%d), got %d" % (X.shape[0], indptr.shape[0]))
+        negs, trials = trace if trace is not None else (None, None)
+        _cabi.check(self._lib.bfl_sgd_fold_in_items_device(
+            self._h, _dev(P, "float32", "P"), P.shape[0], _dev(Q, "float32", "Q"), _dev(Qb, "float32", "Qb"),
+            Q.shape[0], _dev(train_indptr, "int64", "train_indptr"), _dev(train_keys, "int32", "train_keys"),
+            None if cum is None else _dev(cum, "int64", "cum"), _dev(indptr, "int64", "indptr"),
+            _dev(users, "int32", "users"), X.shape[0], users.shape[0], _dev(X, "float32", "X"),
+            _dev(Xb, "float32", "Xb"), int(epochs), None if negs is None else _dev(negs, "int32", "negs"),
+            None if trials is None else _dev(trials, "int32", "trials"), _stream_ptr(stream)),
+            "bfl_sgd_fold_in_items_device")
+
 
 class CuPLSI(_Holder):
     """pLSI backend (CyPLSI, buffalo/algo/_plsi.pyx:13-57).  Holder methods take the [rows, d] host arrays of

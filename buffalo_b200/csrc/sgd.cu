@@ -810,6 +810,211 @@ __global__ void __launch_bounds__(256) det_loss_final_kernel(const double* part,
     if (threadIdx.x == 0) *loss += s[0];
 }
 
+// ---------------------------------------------------------------------------------------
+// Item fold-in (DESIGN.md 4.16): the item side of training's epoch for rows x that are not in Q, with P, Q and Qb
+// frozen.  One warp per new row, grid-striding; the row, its bias and its optimizer state stay in registers for all
+// epochs.  Positive (u, x) is history entry `it` of row r, visited in CSR order; its negatives come from the model's
+// sampler against user u's row of the training CSR (a.indptr / a.keys).  Draw keys: Philox key (seed, 0x5EED),
+// epoch word kFoldInDomain + epoch, index (r << 32) + sample of the row (position * num_neg + k for BPR, the position
+// for WARP), draw number t.  No atomics: a row's result depends on its history, start row and index only.
+// ---------------------------------------------------------------------------------------
+constexpr uint32_t kFoldInDomain = 0xF01D0000u;
+
+struct FoldArgs {
+    const int64_t* h_ind;    // history END offsets [n]
+    const int32_t* h_users;  // history user ids, ascending within a row
+    float* X;                // [n, ld] rows, in / out (padding columns zero)
+    float* Xb;               // [n] biases, in / out
+    int32_t* trace_negs;     // optional [epochs, nnz * per]: negative of each sample, -1 for a WARP discard
+    int32_t* trace_trials;   // optional [epochs, nnz]: WARP trial count, 0 for a discard
+    int64_t n, nnz;
+    int epochs;
+    double inv_epochs, lr0, min_lr, beta1;
+};
+
+// warp_score with the row in registers: dot or negative squared distance (warp.cc:21-28)
+template <int NV>
+__device__ __forceinline__ float fold_score(const float4 (&vp)[NV], const float4 (&x)[NV], int nv4, int lane, int l2) {
+    float part = 0.f;
+#pragma unroll
+    for (int k = 0; k < NV; ++k) {
+        if (lane + 32 * k < nv4) {
+            if (l2) {
+                const float dx = vp[k].x - x[k].x, dy = vp[k].y - x[k].y, dz = vp[k].z - x[k].z, dw = vp[k].w - x[k].w;
+                part -= dx * dx + dy * dy + dz * dz + dw * dw;
+            } else {
+                part += vp[k].x * x[k].x + vp[k].y * x[k].y + vp[k].z * x[k].z + vp[k].w * x[k].w;
+            }
+        }
+    }
+    return warp_sum(part);
+}
+
+// sgd_apply_kernel's element step on one value: count normalisation, regulariser, adagrad / adam, theta += lr0 * step;
+// the gradient accumulator keeps the step, as there
+__device__ __forceinline__ void fold_step(const SgdArgs& a, float& th, float& g, float& m, float& v, int cnt,
+                                          float two_reg, float lr0, float b1, float omb1, float bc1, float bc2) {
+    float s = g;
+    if (a.pcn && cnt) s /= (float)cnt;
+    s -= th * two_reg;
+    if (a.optimizer == 2) {
+        m = b1 * m + omb1 * s;
+        v = b1 * v + omb1 * (s * s);
+        s = (m / bc1) / (sqrtf(v / bc2) + 1e-10f);
+    } else {
+        v = v + s * s;
+        s = s / (sqrtf(v) + 1e-10f);
+    }
+    g = s;
+    th = th + lr0 * s;
+}
+
+__device__ __forceinline__ void fold_step4(const SgdArgs& a, float4& th, float4& g, float4& m, float4& v, int cnt,
+                                           float two_reg, float lr0, float b1, float omb1, float bc1, float bc2) {
+    fold_step(a, th.x, g.x, m.x, v.x, cnt, two_reg, lr0, b1, omb1, bc1, bc2);
+    fold_step(a, th.y, g.y, m.y, v.y, cnt, two_reg, lr0, b1, omb1, bc1, bc2);
+    fold_step(a, th.z, g.z, m.z, v.z, cnt, two_reg, lr0, b1, omb1, bc1, bc2);
+    fold_step(a, th.w, g.w, m.w, v.w, cnt, two_reg, lr0, b1, omb1, bc1, bc2);
+}
+
+template <int NV, bool kWarp>
+__global__ void __launch_bounds__(256, 2) sgd_fold_in_items_kernel(SgdArgs a, FoldArgs f) {
+    const int lane = threadIdx.x & 31;
+    const int64_t w0 = (int64_t)blockIdx.x * (blockDim.x >> 5) + warp_id_uniform();
+    const int64_t nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    const int nv4 = a.ld >> 2;
+    const int per = kWarp ? 1 : a.num_neg;
+    const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int64_t r = w0; r < f.n; r += nw) {
+        const int64_t hb = uni((long long)(r == 0 ? 0 : __ldg(f.h_ind + r - 1))), he = uni((long long)__ldg(f.h_ind + r));
+        float* xr = f.X + r * a.ld;
+        float4 x[NV], g[NV], m[NV], v[NV];
+#pragma unroll
+        for (int k = 0; k < NV; ++k) {
+            x[k] = lane + 32 * k < nv4 ? ld4(xr + 4 * (lane + 32 * k)) : zero;
+            g[k] = m[k] = v[k] = zero;
+        }
+        float xb = f.Xb[r], gb = 0.f, mb = 0.f, vb = 0.f;
+        double b1pow = 1.0;  // beta1^(e + 1) of adam's bias correction, as a running product
+        for (int e = 0; e < f.epochs; ++e) {
+            a.epoch = kFoldInDomain + (uint32_t)e;
+            // training's linear decay (run_jobs), over the fold-in's own epochs
+            const double lr = f.lr0 - (f.lr0 - f.min_lr) * ((double)e * f.inv_epochs);
+            a.lr = (float)(lr > f.min_lr ? lr : f.min_lr);
+            int cnt = 0;
+            for (int64_t it = hb; it < he; ++it) {
+                const int u = uni(__ldg(f.h_users + it));
+                const int64_t ub = u == 0 ? 0 : __ldg(a.indptr + u - 1), ue = __ldg(a.indptr + u);
+                const int32_t* rk = a.keys + ub;
+                const float* pu = a.P + (int64_t)u * a.ld;
+                float4 vp[NV];
+#pragma unroll
+                for (int k = 0; k < NV; ++k) vp[k] = lane + 32 * k < nv4 ? ld4(pu + 4 * (lane + 32 * k)) : zero;
+                const uint64_t sid0 = ((uint64_t)r << 32) + (uint64_t)(it - hb) * (uint64_t)per;
+                int32_t* tn = f.trace_negs ? f.trace_negs + ((int64_t)e * f.nnz + it) * per : nullptr;
+                if constexpr (kWarp) {
+                    const float ui = uni(fold_score<NV>(vp, x, nv4, lane, a.score_l2));
+                    float4 vj[NV];
+                    float uj = 0.f;
+                    int neg = 0;
+                    const int trial = warp_rank_draw<NV>(a, (int64_t)sid0, rk, ue - ub, vp, ui, nv4, lane, vj, neg, uj);
+                    const bool discard = trial >= a.max_trials;  // warp.cc:149-150
+                    if (lane == 0 && tn) {
+                        tn[0] = discard ? -1 : neg;
+                        f.trace_trials[(int64_t)e * f.nnz + it] = discard ? 0 : trial;
+                    }
+                    if (discard) continue;
+                    // :152 in 32 bits (num_items and the row length are int32): no 64-bit division subroutine
+                    int ratio = (a.num_items - (int)(ue - ub) - 1) / trial;
+                    if (ratio < 1) ratio = 1;
+                    const float Phi = logf((float)ratio);
+#pragma unroll
+                    for (int k = 0; k < NV; ++k) {
+                        if (lane + 32 * k < nv4) {
+                            float4 di;
+                            if (!a.score_l2) di = make_float4(Phi * vp[k].x, Phi * vp[k].y, Phi * vp[k].z, Phi * vp[k].w);
+                            else di = make_float4(Phi * (vp[k].x - x[k].x), Phi * (vp[k].y - x[k].y),
+                                                  Phi * (vp[k].z - x[k].z), Phi * (vp[k].w - x[k].w));
+                            g[k].x += di.x - a.reg_i * x[k].x;  // warp.cc:156-158
+                            g[k].y += di.y - a.reg_i * x[k].y;
+                            g[k].z += di.z - a.reg_i * x[k].z;
+                            g[k].w += di.w - a.reg_i * x[k].w;
+                        }
+                    }
+                    cnt += 1;
+                } else {
+                    for (int s = 0; s < per; ++s) {
+                        const int neg = uni(bpr_draw_negative(a, sid0 + (uint64_t)s, rk, ue - ub));
+                        const float* qj = a.Q + (int64_t)neg * a.ld;
+                        float part = 0.f;
+#pragma unroll
+                        for (int k = 0; k < NV; ++k) {
+                            if (lane + 32 * k < nv4) {
+                                const float4 vj = ld4(qj + 4 * (lane + 32 * k));
+                                part += vp[k].x * (x[k].x - vj.x) + vp[k].y * (x[k].y - vj.y) +
+                                        vp[k].z * (x[k].z - vj.z) + vp[k].w * (x[k].w - vj.w);
+                            }
+                        }
+                        float xs = warp_sum(part);  // bpr.cc:119-121
+                        if (a.use_bias) xs += xb - __ldg(a.Qb + neg);
+                        const float logit = xs > 6.f ? 0.f : (xs < -6.f ? 1.f : 1.0f / (1.0f + __expf(xs)));
+                        if (lane == 0 && tn) tn[s] = neg;
+                        if (a.optimizer == 0) {  // the positive side of bpr_apply_kernel's step, after every sample
+#pragma unroll
+                            for (int k = 0; k < NV; ++k) {
+                                if (lane + 32 * k < nv4) {
+                                    x[k].x += a.lr * (logit * vp[k].x - a.reg_i * x[k].x);
+                                    x[k].y += a.lr * (logit * vp[k].y - a.reg_i * x[k].y);
+                                    x[k].z += a.lr * (logit * vp[k].z - a.reg_i * x[k].z);
+                                    x[k].w += a.lr * (logit * vp[k].w - a.reg_i * x[k].w);
+                                }
+                            }
+                            if (a.use_bias) xb += a.lr * (logit - a.reg_b * xb);
+                        } else {
+#pragma unroll
+                            for (int k = 0; k < NV; ++k) {
+                                if (lane + 32 * k < nv4) {
+                                    g[k].x += logit * vp[k].x;
+                                    g[k].y += logit * vp[k].y;
+                                    g[k].z += logit * vp[k].z;
+                                    g[k].w += logit * vp[k].w;
+                                }
+                            }
+                            gb += logit;
+                        }
+                    }
+                    cnt += 1;  // per_coordinate_normalize counts the positive once (bpr.cc:140-143)
+                }
+            }
+            if (a.optimizer != 0) {  // one step per epoch (apply_optimizer)
+                const float b1 = (float)f.beta1, omb1 = (float)(1.0 - f.beta1);
+                b1pow *= f.beta1;
+                const float bc1 = (float)(1.0 - b1pow), lr0 = (float)f.lr0;
+#pragma unroll
+                for (int k = 0; k < NV; ++k)
+                    if (lane + 32 * k < nv4) fold_step4(a, x[k], g[k], m[k], v[k], cnt, 2.f * a.reg_i, lr0, b1, omb1, bc1, bc1);
+                if (!kWarp && a.use_bias) fold_step(a, xb, gb, mb, vb, cnt, 2.f * a.reg_b, lr0, b1, omb1, bc1, bc1);
+            }
+            if constexpr (kWarp) {  // warp_project_kernel: row /= max(1, ||row||)
+                float ss = 0.f;
+#pragma unroll
+                for (int k = 0; k < NV; ++k)
+                    if (lane + 32 * k < nv4) ss += x[k].x * x[k].x + x[k].y * x[k].y + x[k].z * x[k].z + x[k].w * x[k].w;
+                const float nrm = sqrtf(warp_sum(ss));
+                if (nrm > 1.0f) {
+#pragma unroll
+                    for (int k = 0; k < NV; ++k)
+                        if (lane + 32 * k < nv4) x[k] = make_float4(x[k].x / nrm, x[k].y / nrm, x[k].z / nrm, x[k].w / nrm);
+                }
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < NV; ++k)
+            if (lane + 32 * k < nv4) *reinterpret_cast<float4*>(xr + 4 * (lane + 32 * k)) = x[k];
+        if (lane == 0) f.Xb[r] = xb;
+    }
+}
+
 }  // namespace
 
 struct bfl_sgd : Holder {
@@ -1437,6 +1642,50 @@ int bfl_sgd_set_trace_device(bfl_sgd_t* h, int32_t* d_trials, int32_t* d_negs) {
     if (!h) BFL_FAIL(BFL_ERR_ARG, "null handle");
     h->trace_trials = d_trials;
     h->trace_negs = d_negs;
+    return BFL_OK;
+}
+
+int bfl_sgd_fold_in_items_device(bfl_sgd_t* h, const float* dP, int64_t P_rows, const float* dQ, const float* dQb,
+                                 int64_t Q_rows, const int64_t* d_train_indptr, const int32_t* d_train_keys,
+                                 const int64_t* d_cum, const int64_t* d_hist_indptr, const int32_t* d_hist_users,
+                                 int64_t n, int64_t hist_nnz, float* dX, float* dXb, int epochs,
+                                 int32_t* d_trace_negs, int32_t* d_trace_trials, void* stream) {
+    if (!h || !h->opt_set) BFL_FAIL(BFL_ERR_STATE, "init() must precede fold_in_items");
+    if (epochs < 1) BFL_FAIL(BFL_ERR_ARG, "fold_in_items: epochs must be >= 1");
+    if (n < 0 || n > (int64_t)INT32_MAX || hist_nnz < 0) BFL_FAIL(BFL_ERR_ARG, "fold_in_items: bad row count");
+    if (P_rows < 1 || Q_rows < 1 || Q_rows > (int64_t)INT32_MAX) BFL_FAIL(BFL_ERR_ARG, "fold_in_items: bad factor shapes");
+    if (n == 0) return BFL_OK;
+    if (!dP || !dQ || !dQb || !d_train_indptr || !d_train_keys || !d_hist_indptr || !d_hist_users || !dX || !dXb)
+        BFL_FAIL(BFL_ERR_ARG, "fold_in_items: null array");
+    if (h->kind == BFL_SGD_WARP && (d_trace_negs == nullptr) != (d_trace_trials == nullptr))
+        BFL_FAIL(BFL_ERR_ARG, "fold_in_items: a WARP trace needs both the negatives and the trial counts");
+    SgdArgs a;
+    fill_args(h, a, d_train_keys, 0, 0, P_rows, 0, 0);
+    a.P = const_cast<float*>(dP); a.Q = const_cast<float*>(dQ); a.Qb = const_cast<float*>(dQb);
+    a.gP = a.gQ = a.gQb = nullptr; a.cP = a.cQ = nullptr;
+    a.indptr = d_train_indptr;
+    a.cum = d_cum;
+    a.uniform = h->uniform || !d_cum;
+    a.trace_trials = a.trace_negs = nullptr;
+    a.num_items = (int32_t)Q_rows;
+    FoldArgs f;
+    f.h_ind = d_hist_indptr; f.h_users = d_hist_users; f.X = dX; f.Xb = dXb;
+    f.trace_negs = d_trace_negs; f.trace_trials = d_trace_trials;
+    f.n = n; f.nnz = hist_nnz; f.epochs = epochs; f.inv_epochs = 1.0 / (double)epochs;
+    f.lr0 = h->lr0; f.min_lr = h->min_lr; f.beta1 = h->beta1;
+    const int grid = (int)std::min<int64_t>((n + 7) / 8, (int64_t)h->num_sms * 16);
+    const int nv = (h->vdim / 4 + 31) / 32;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (h->kind == BFL_SGD_WARP) {
+        if (nv <= 1) sgd_fold_in_items_kernel<1, true><<<grid, 256, 0, st>>>(a, f);
+        else if (nv <= 2) sgd_fold_in_items_kernel<2, true><<<grid, 256, 0, st>>>(a, f);
+        else sgd_fold_in_items_kernel<4, true><<<grid, 256, 0, st>>>(a, f);
+    } else {
+        if (nv <= 1) sgd_fold_in_items_kernel<1, false><<<grid, 256, 0, st>>>(a, f);
+        else if (nv <= 2) sgd_fold_in_items_kernel<2, false><<<grid, 256, 0, st>>>(a, f);
+        else sgd_fold_in_items_kernel<4, false><<<grid, 256, 0, st>>>(a, f);
+    }
+    BFL_LAUNCHED();
     return BFL_OK;
 }
 

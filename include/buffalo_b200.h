@@ -242,6 +242,23 @@ int bfl_sgd_read_stats(bfl_sgd_t* h, double* loss_sum, int64_t* num_updates);
 int bfl_sgd_reduce_items_device(bfl_sgd_t* h, void* stream);
 /* samples / item entries per segment of the deterministic user and item sums */
 int bfl_sgd_segment_len(void);
+/* Item fold-in (DESIGN.md 4.16): `epochs` epochs of the item side of training for n new rows, with the trained factors
+ * frozen.  Uses the holder's options only (init() must have succeeded; no factors need to be bound).  All arrays are
+ * DEVICE memory:
+ *   dP [P_rows, vdim], dQ [Q_rows, vdim], dQb [Q_rows]     the trained factors, read only;
+ *   d_train_indptr int64 [P_rows] END offsets, d_train_keys  the training data's rowwise CSR, each row ascending
+ *                                                          (the negatives' seen check);
+ *   d_cum int64 [Q_rows] or NULL                           BPR popularity table (NULL: uniform negatives);
+ *   d_hist_indptr int64 [n] END offsets, d_hist_users int32 [hist_nnz]   the new rows' users, ascending per row;
+ *   dX [n, vdim], dXb [n]                                  start rows and biases in, folded rows and biases out.
+ * d_trace_negs (int32 [epochs, hist_nnz * samples per positive]) and, for WARP, d_trace_trials (int32 [epochs,
+ * hist_nnz]) are optional records of the draws: the negative of each sample (-1 for a WARP discard) and WARP's trial
+ * count (0 for a discard).  Each row's result depends only on its history, start row and index: no atomics. */
+int bfl_sgd_fold_in_items_device(bfl_sgd_t* h, const float* dP, int64_t P_rows, const float* dQ, const float* dQb,
+                                 int64_t Q_rows, const int64_t* d_train_indptr, const int32_t* d_train_keys,
+                                 const int64_t* d_cum, const int64_t* d_hist_indptr, const int32_t* d_hist_users,
+                                 int64_t n, int64_t hist_nnz, float* dX, float* dXb, int epochs,
+                                 int32_t* d_trace_negs, int32_t* d_trace_trials, void* stream);
 
 /* ======================================================================================
  * PLSI -- replaces CyPLSI (buffalo/algo/_plsi.pyx:13-57 -> plsi::CPLSI, lib/algo_impl/plsi/plsi.cc)
