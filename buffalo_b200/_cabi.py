@@ -49,6 +49,8 @@ PROTOTYPES = {
     "bfl_als_update_device": (C.c_int, [_vp, C.c_int, _i64, _i64, _vp, _vp]),
     "bfl_als_set_peer_replicas": (C.c_int, [_vp, C.c_int, C.c_int, C.POINTER(_vp)]),
     "bfl_als_explain_device": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, C.c_int, C.c_int, _vp, _vp, _vp, _vp]),
+    "bfl_als_posterior_sample_device": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, C.c_int, _vp, C.c_uint32, _f, _vp,
+                                                  _vp, _vp]),
     "bfl_als_gram_device": (_vp, [_vp]),
     "bfl_als_gram_device_mut": (_vp, [_vp]),
     # SGD (BPRMF / WARP)

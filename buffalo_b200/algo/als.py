@@ -204,6 +204,61 @@ class ALS(Algo, ALSOption, Evaluable, Serializable):
             h._keep = []
         return tuple(t.cpu().numpy() for t in out)
 
+    # ---- exploration (DESIGN.md 4.17) ---------------------------------------------------------
+    def posterior_sample(self, histories, mean, scale=1.0, seed=0, draw_keys=None):
+        """float32 [n, d]: one draw per history row from the Gaussian posterior of its user row, for Thompson sampling.
+        Read as Bayesian least squares -- observations p_j with noise precision c_j / sigma^2 and the prior
+        N(0, sigma^2 / (reg_u kappa) I) -- the objective of the user half-epoch gives, with the item factors fixed, the
+        posterior N(A_r^-1 b_r, sigma^2 A_r^-1), A_r = Q'Q + alpha sum v_j q_j q_j' + reg_u kappa I (kappa = the row's
+        entry count with adaptive_reg, else 1).  A draw here is mean[r] + scale L_r^-T z with A_r = L_r L_r' and
+        z ~ N(0, I): the caller's mean (P[u], or a fold_in row) with the spread of that posterior.  scale is sigma, the
+        caller's choice (not estimated): smaller explores less, 0 returns mean itself.
+
+        histories: as fold_in takes them.  mean: an (n, d) array.  seed: an integer in [0, 2^32).  draw_keys: n distinct
+        non-negative integers, default arange(n); z of a row depends only on seed and its draw key (DESIGN.md 4.17 gives
+        the Philox words), so a row's draw does not depend on the other rows of the call.  A row whose A_r is not
+        positive definite in fp32 comes back as its mean, with a logged warning counting such rows.  d <= 256.  On the
+        GPU only: without one the backend's "no CPU fallback" error is raised."""
+        tX = self._posterior_sample_device(histories, mean, scale, seed, draw_keys)
+        return tX[:, :self.opt.d].cpu().numpy()
+
+    def _posterior_sample_device(self, histories, mean, scale=1.0, seed=0, draw_keys=None):
+        """posterior_sample's rows as a torch CUDA tensor [n, vdim] (padding zero); every check before device work."""
+        if self.opt._nrz_Q:
+            raise RuntimeError("Cannot sample posterior rows with normalized item factors")
+        if self.opt.d > self.EXPLAIN_DMAX:
+            raise ValueError("posterior_sample supports d <= %d, got %d" % (self.EXPLAIN_DMAX, self.opt.d))
+        scale, seed = fold_in.posterior_args(scale, seed)
+        indptr, keys, vals = fold_in.history_csr(self, histories, self.Q.shape[0])
+        n, d = len(indptr), self.opt.d
+        M = np.asarray(mean)
+        if M.shape != (n, d) or (M.size and not np.issubdtype(M.dtype, np.number)):
+            raise ValueError("mean must be an (%d, %d) array, got %s %s" % (n, d, M.dtype, M.shape))
+        K = fold_in.draw_key_array(draw_keys, n)
+        st, h = fold_in.resident_state(self, CuALS)
+        import torch
+        ind_t, keys_t, vals_t, tM = fold_in.to_device(indptr, keys, vals, M.astype(np.float32), h.get_vdim())
+        if n == 0:
+            return tM
+        return self._sample_rows(st, h, (ind_t, keys_t, vals_t), tM, torch.from_numpy(K).to(tM.device), seed, scale)
+
+    def _sample_rows(self, st, h, csr, tM, tK, seed, scale):
+        """tM (CUDA [n, vdim], the means) replaced in place by the posterior draws of the device history CSR csr with draw
+        keys tK (int64 CUDA [n]); arguments already checked.  Returns tM."""
+        import torch
+        n = tM.shape[0]
+        try:
+            # the draws read Q and its Gram only; the bound rows are a placeholder
+            self._bind_fold_items(st, h, torch.zeros((1, h.get_vdim()), dtype=torch.float32, device=tM.device))
+            _, failed = h.posterior_sample_device(*csr, tM, tK, seed, scale, out=tM)
+        finally:
+            h._keep = []
+        failed = int(failed.item())
+        if failed:
+            self.logger.warning("posterior_sample: %d of %d rows left at their mean (A_r not positive definite in fp32)"
+                                % (failed, n))
+        return tM
+
     # ---- training -----------------------------------------------------------------------------
     def _get_buffer(self):
         buf = BufferedDataMatrix()

@@ -1,5 +1,5 @@
-"""Folding-in (DESIGN.md 4.10, 4.16): the host side that ALS.fold_in, PLSI.fold_in, ALS.explain (4.11) and the item
-fold-ins (ALS / BPRMF / WARP .fold_in_items) share.
+"""Folding-in (DESIGN.md 4.10, 4.16): the host side that ALS.fold_in, PLSI.fold_in, ALS.explain (4.11),
+ALS.posterior_sample (4.17) and the item fold-ins (ALS / BPRMF / WARP .fold_in_items) share.
 
 A user fold-in computes user rows from their histories with the model's item factors held fixed; an item fold-in
 computes item rows from the users who interacted with them, with the user factors held fixed.  This module turns the
@@ -91,6 +91,29 @@ def positive_int(value, name):
     if isinstance(value, bool) or not isinstance(value, (int, np.integer)) or value < 1:
         raise ValueError("%s must be an integer >= 1, got %r" % (name, value))
     return int(value)
+
+
+def posterior_args(scale, seed, scale_name="scale", seed_name="seed"):
+    """(float32-rounded scale, seed) of a posterior draw: scale a finite real >= 0, seed an integer in [0, 2^32)."""
+    if isinstance(scale, bool) or not isinstance(scale, (int, float, np.integer, np.floating)) \
+            or not 0 <= scale <= float(np.finfo(np.float32).max):
+        raise ValueError("%s must be a finite real number >= 0, got %r" % (scale_name, scale))
+    if isinstance(seed, bool) or not isinstance(seed, (int, np.integer)) or not 0 <= seed < 2 ** 32:
+        raise ValueError("%s must be an integer in [0, 2^32), got %r" % (seed_name, seed))
+    return float(np.float32(scale)), int(seed)
+
+
+def draw_key_array(draw_keys, n):
+    """int64 [n] draw keys: arange(n) when None, else n distinct non-negative integers (ValueError otherwise)."""
+    if draw_keys is None:
+        return np.arange(n, dtype=np.int64)
+    K = np.asarray(draw_keys)
+    if K.shape != (n,) or (K.size and not np.issubdtype(K.dtype, np.integer)):
+        raise ValueError("draw_keys must be %d integers, got %s %s" % (n, K.dtype, K.shape))
+    K = K.astype(np.int64)
+    if K.size and (int(K.min()) < 0 or len(np.unique(K)) != n):
+        raise ValueError("draw_keys must be distinct non-negative integers")
+    return K
 
 
 class ItemState(object):

@@ -186,6 +186,35 @@ class CuALS(_Holder):
                 contrib.data_ptr(), _stream_ptr(stream)), "bfl_als_explain_device")
         return scores, out_keys, contrib
 
+    def posterior_sample_device(self, indptr, keys, vals, mean, draw_keys, seed, scale, out=None, stream=None):
+        """bfl_als_posterior_sample_device: (rows float32 CUDA [n, ld], failed int64 CUDA [1]) -- one draw per history row
+        (indptr int64 [n] END offsets, keys int32 items in [0, Q_rows), ascending within a row, not checked here; vals
+        float32) from N(mean[r], scale^2 A_r^-1), against the bound Q and the Gram of precompute_device(0).  mean float32
+        CUDA [n, ld] (any ld >= d: the pitch of mean and out only, Q is read at the holder's own), draw_keys int64 CUDA
+        [n], seed in [0, 2^32), scale finite >= 0.  out: None (a new zero tensor, so its padding columns are zero) or a
+        float32 CUDA [n, ld] tensor, which may be mean itself.  failed holds the number of rows left at their mean."""
+        import torch
+        if mean.ndim != 2 or indptr.ndim != 1 or indptr.shape[0] != mean.shape[0]:
+            raise ValueError("mean must be [n, ld] with one row per END offset (got %s for %d rows)"
+                             % (tuple(mean.shape), indptr.shape[0]))
+        if draw_keys.shape != (mean.shape[0],):
+            raise ValueError("draw_keys must be [%d], got %s" % (mean.shape[0], tuple(draw_keys.shape)))
+        if not 0 <= int(seed) < 2 ** 32:
+            raise ValueError("seed must be in [0, 2^32), got %r" % (seed,))
+        n, ld = mean.shape
+        if out is None:
+            out = torch.zeros_like(mean)
+        elif tuple(out.shape) != (n, ld):
+            raise ValueError("out must be [%d, %d], got %s" % (n, ld, tuple(out.shape)))
+        failed = torch.zeros(1, dtype=torch.int64, device=mean.device)
+        if n:
+            _cabi.check(self._lib.bfl_als_posterior_sample_device(
+                self._h, _dev(indptr, "int64", "indptr"), _dev(keys, "int32", "keys"), _dev(vals, "float32", "vals"), n,
+                _dev(mean, "float32", "mean"), int(ld), _dev(draw_keys, "int64", "draw_keys"), int(seed),
+                float(scale), _dev(out, "float32", "out"), failed.data_ptr(), _stream_ptr(stream)),
+                "bfl_als_posterior_sample_device")
+        return out, failed
+
     def gram_tensor(self):
         """View of the current d x d Gram matrix as a torch tensor (multi-GPU all-reduce, tests)."""
         ptr = self._lib.bfl_als_gram_device_mut(self._h)
@@ -590,6 +619,12 @@ class Serve(_Holder):
                                                     queries.stride(0)), "bind_queries")
         self._bound["queries"] = queries
         self.num_queries = queries.shape[0]
+
+    def unbind_queries(self):
+        """Drops this object's hold on the tensor given to bind_queries, so it can be freed; the handle has no queries
+        until the next set_queries / bind_queries."""
+        self._bound.pop("queries", None)
+        self.num_queries = 0
 
     def set_pool(self, pool):
         """pool: int32 indices into the items (None removes it).  An empty pool is an error."""

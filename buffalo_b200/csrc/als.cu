@@ -553,6 +553,38 @@ int bfl_als_explain_device(bfl_als_t* h, const int64_t* d_indptr, const int32_t*
     return explain_launch(a, h->num_sms, (cudaStream_t)stream);
 }
 
+int bfl_als_posterior_sample_device(bfl_als_t* h, const int64_t* d_indptr, const int32_t* d_keys, const float* d_vals,
+                                    int64_t n, const float* d_mean, int ld, const int64_t* d_draw_keys, uint32_t seed,
+                                    float scale, float* d_out, int64_t* d_failed, void* stream) {
+    if (!h || !h->factors_ready) BFL_FAIL(BFL_ERR_STATE, "factors not bound");
+    if (h->gram_axis != 0) BFL_FAIL(BFL_ERR_STATE, "posterior_sample needs the Gram of Q: bfl_als_precompute_device(axis 0) first");
+    if (h->d > EXPLAIN_DMAX) BFL_FAIL(BFL_ERR_ARG, "posterior_sample supports d <= " + std::to_string(EXPLAIN_DMAX));
+    if (ld < h->d) BFL_FAIL(BFL_ERR_ARG, "ld must be at least d");
+    if (!(scale >= 0.f && scale <= 3.402823466e38f)) BFL_FAIL(BFL_ERR_ARG, "scale must be finite and >= 0");
+    if (n < 0 || (n > 0 && (!d_indptr || !d_keys || !d_vals || !d_mean || !d_draw_keys || !d_out || !d_failed)))
+        BFL_FAIL(BFL_ERR_ARG, "bad posterior_sample arguments");
+    PosteriorArgs a;
+    a.G = h->G.p;
+    a.Q = h->dQ;
+    a.D = h->d;
+    a.ldq = h->vdim;
+    a.alpha = h->alpha;
+    a.reg = h->reg_u;
+    a.adaptive_reg = h->adaptive_reg;
+    a.indptr = d_indptr;
+    a.keys = d_keys;
+    a.vals = d_vals;
+    a.n = n;
+    a.ld = ld;
+    a.mean = d_mean;
+    a.draw_keys = d_draw_keys;
+    a.seed = seed;
+    a.scale = scale;
+    a.out = d_out;
+    a.failed = d_failed;
+    return posterior_sample_launch(a, h->num_sms, (cudaStream_t)stream);
+}
+
 const float* bfl_als_gram_device(bfl_als_t* h) { return h ? h->G.p : nullptr; }
 float* bfl_als_gram_device_mut(bfl_als_t* h) { return h ? h->G.p : nullptr; }
 

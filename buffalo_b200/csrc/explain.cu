@@ -3,17 +3,18 @@
 //   contribution_rij = (q_i' A_r^-1 q_j) * (1 + alpha v_j),
 // with the top-m terms per (row, target).  One CTA owns one row at a time; no atomics, so a row's outputs depend only on
 // the row, its targets, Q, the Gram and the options.
+//
+// Posterior draws (DESIGN.md 4.17): for the same A_r, x~ = mean + scale * L^-T z with A_r = L L' and z ~ N(0, I) from
+// Philox, i.e. a draw from N(mean, scale^2 A_r^-1), the posterior of the row under the Gaussian reading of the user
+// half-epoch.  One CTA per row at a time, no atomics: a row's draw depends only on the seed, its draw key, its history,
+// its mean, Q, the Gram and the options.
 #include "explain.cuh"
 
 namespace bfl {
 namespace {
 
-constexpr int EX_THREADS = 256, EX_WARPS = EX_THREADS / 32;
-constexpr int EX_T = 16;    // targets per tile
-constexpr int EX_NB = 16;   // history entries per gathered chunk (EX_T * EX_NB == EX_THREADS: one dot per thread)
+constexpr int EX_T = 16;    // targets per tile (EX_T * EX_NB == EX_THREADS: one dot per thread)
 static_assert(EX_T * EX_NB == EX_THREADS, "one (target, entry) pair per thread");
-
-__device__ __forceinline__ int tri(int i) { return i * (i + 1) / 2; }   // start of row i of the packed lower triangle
 
 // floats of dynamic shared memory: the packed lower triangle, pivots, one column, b, the target tile, the gathered
 // chunk, its contributions, weights and keys, and the top-m lists.  Rows of the tiles are S = D | 1 floats apart, an
@@ -21,21 +22,6 @@ __device__ __forceinline__ int tri(int i) { return i * (i + 1) / 2; }   // start
 size_t explain_smem_floats(int D, int topm) {
     const size_t S = (size_t)(D | 1);
     return (size_t)D * (D + 1) / 2 + 3 * (size_t)D + (EX_T + EX_NB) * S + EX_T * EX_NB + 2 * EX_NB + 2 * (size_t)EX_T * topm;
-}
-
-// the chunk's item rows into Qc (warp per entry, coalesced), its keys into ck and w(v) into cw
-template <typename W>
-__device__ __forceinline__ void gather_chunk(const ExplainArgs& a, int64_t b0, int nb, int S, float* Qc, float* cw, int* ck,
-                                             W w) {
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    for (int b = wid; b < nb; b += EX_WARPS) {
-        const float* q = a.Q + (int64_t)__ldg(a.keys + b0 + b) * a.ld;
-        for (int c = lane; c < a.D; c += 32) Qc[b * S + c] = __ldg(q + c);
-    }
-    if (tid < nb) {
-        ck[tid] = __ldg(a.keys + b0 + tid);
-        cw[tid] = w(__ldg(a.vals + b0 + tid));
-    }
 }
 
 // one item's total into a descending list of cnt <= topm entries.  Keys arrive in ascending order, so on a tie the
@@ -89,51 +75,10 @@ __global__ void __launch_bounds__(EX_THREADS) explain_kernel(ExplainArgs a) {
 
         // 1. A_r = G + reg*kappa*I + sum alpha v q q' (lower part), b_r = sum (1 + alpha v) q, in entry order
         const float regk = a.reg * (a.adaptive_reg ? (float)(end - beg) : 1.0f);
-        for (int i = wid; i < D; i += EX_WARPS)
-            for (int j = lane; j <= i; j += 32) L[tri(i) + j] = a.G[i * D + j] + (i == j ? regk : 0.f);
-        for (int i = tid; i < D; i += EX_THREADS) bv[i] = 0.f;
-        for (int64_t b0 = beg; b0 < end; b0 += EX_NB) {
-            const int nb = (int)min((int64_t)EX_NB, end - b0);
-            __syncthreads();
-            gather_chunk(a, b0, nb, S, Qc, cw, ck, [](float v) { return v; });
-            __syncthreads();
-            for (int i = wid; i < D; i += EX_WARPS)
-                for (int j = lane; j <= i; j += 32) {
-                    float acc = 0.f;
-                    for (int b = 0; b < nb; ++b) acc += (alpha * cw[b] * Qc[b * S + i]) * Qc[b * S + j];
-                    L[tri(i) + j] += acc;
-                }
-            for (int i = tid; i < D; i += EX_THREADS) {
-                float acc = 0.f;
-                for (int b = 0; b < nb; ++b) acc += (1.0f + alpha * cw[b]) * Qc[b * S + i];
-                bv[i] += acc;
-            }
-        }
-        __syncthreads();
+        build_row_system<true>(a.G, a.Q, a.ld, D, S, alpha, regk, a.keys, a.vals, beg, end, L, bv, Qc, cw, ck);
 
-        // 2. Cholesky A_r = L L', right-looking, in place.  Every thread reads the same pivot, so a non-positive (or
-        // NaN) one stops all of them at the same column.
-        for (int j = 0; j < D; ++j) {
-            const float p = L[tri(j) + j];
-            if (!(p > 0.f)) {
-                if (tid == 0) s_fail = 1;
-                break;
-            }
-            const float ljj = sqrtf(p);
-            for (int i = j + 1 + tid; i < D; i += EX_THREADS) {
-                const float lij = L[tri(i) + j] / ljj;
-                L[tri(i) + j] = lij;
-                colv[i] = lij;
-            }
-            if (tid == 0) diag[j] = ljj;
-            __syncthreads();
-            for (int i = j + 1 + wid; i < D; i += EX_WARPS) {
-                const float lij = colv[i];
-                float* row = L + tri(i);
-                for (int c = j + 1 + lane; c <= i; c += 32) row[c] -= lij * colv[c];
-            }
-            __syncthreads();
-        }
+        // 2. Cholesky A_r = L L', right-looking, in place
+        if (!cholesky_packed(L, diag, colv, D) && tid == 0) s_fail = 1;
 
         // 3.-6. per tile of EX_T targets
         for (int t0 = 0; t0 < k; t0 += EX_T) {
@@ -194,7 +139,7 @@ __global__ void __launch_bounds__(EX_THREADS) explain_kernel(ExplainArgs a) {
                 for (int64_t b0 = beg; b0 < end; b0 += EX_NB) {
                     const int nb = (int)min((int64_t)EX_NB, end - b0);
                     __syncthreads();
-                    gather_chunk(a, b0, nb, S, Qc, cw, ck, [alpha](float v) { return 1.0f + alpha * v; });
+                    gather_chunk(a.Q, a.ld, D, a.keys, a.vals, b0, nb, S, Qc, cw, ck, [alpha](float v) { return 1.0f + alpha * v; });
                     __syncthreads();
                     if (pt < nt && pb < nb) {
                         const float* u = U + pt * S;
@@ -232,7 +177,129 @@ __global__ void __launch_bounds__(EX_THREADS) explain_kernel(ExplainArgs a) {
     }
 }
 
+// floats of dynamic shared memory: the packed lower triangle, pivots, z (also the factorisation's column), y, the
+// gathered chunk (rows S = D | 1 floats apart), its weights and keys
+size_t posterior_smem_floats(int D) {
+    const size_t S = (size_t)(D | 1);
+    return (size_t)D * (D + 1) / 2 + 3 * (size_t)D + EX_NB * S + 2 * EX_NB;
+}
+
+// z_c for c < D of one row: quad q of the draw key's Philox stream gives words w[0..3] = draw_u32(seed, POSTERIOR_TAG,
+// key, 4q + i), and pair k = 2q + h the Box-Muller normals of u1 = (w[2h] + 1) 2^-32, u2 = w[2h + 1] 2^-32:
+// sqrt(-2 ln u1) cos(2 pi u2), sqrt(-2 ln u1) sin(2 pi u2) (u1 and u2 rounded to fp32; precise logf / sincospif)
+__device__ __forceinline__ void normal_draws(uint32_t seed, uint64_t key, int D, float* z) {
+    for (int q = threadIdx.x; 4 * q < D; q += EX_THREADS) {
+        uint32_t w[4];
+        philox4x32_10((uint32_t)key, (uint32_t)(key >> 32), (uint32_t)q, POSTERIOR_TAG, seed, 0x5EEDu, w);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int c = 4 * q + 2 * h;
+            if (c < D) {
+                const float u1 = (float)((uint64_t)w[2 * h] + 1u) * 0x1p-32f, u2 = (float)w[2 * h + 1] * 0x1p-32f;
+                const float rad = sqrtf(-2.0f * logf(u1));
+                float sn, cs;
+                sincospif(2.0f * u2, &sn, &cs);
+                z[c] = rad * cs;
+                if (c + 1 < D) z[c + 1] = rad * sn;
+            }
+        }
+    }
+}
+
+__global__ void __launch_bounds__(EX_THREADS) posterior_sample_kernel(PosteriorArgs a, int64_t* failed_part) {
+    extern __shared__ float sm[];
+    const int D = a.D, S = D | 1;
+    float* L = sm;                        // packed lower triangle: A_r, then its Cholesky factor (strictly lower part)
+    float* diag = L + tri(D);             // [D] pivots L[j][j]
+    float* zv = diag + D;                 // [D] the factorisation's column j, then z, solved in place
+    float* yv = zv + D;                   // [D] y = L'^-1 z
+    float* Qc = yv + D;                   // [EX_NB][S] gathered history rows
+    float* cw = Qc + EX_NB * S;           // [EX_NB] v
+    int* ck = (int*)(cw + EX_NB);         // [EX_NB] the chunk's keys
+    const int tid = threadIdx.x, lane = tid & 31;
+    int64_t nfail = 0;                    // rows of this CTA left at their mean (thread 0's count)
+
+    for (int64_t r = blockIdx.x; r < a.n; r += gridDim.x) {
+        const float* mean = a.mean + r * a.ld;
+        float* out = a.out + r * a.ld;
+        if (a.scale == 0.f) {             // no exploration: the mean itself, whatever its bits
+            for (int c = tid; c < D; c += EX_THREADS) out[c] = mean[c];
+            continue;
+        }
+        const int64_t beg = r == 0 ? 0 : a.indptr[r - 1], end = a.indptr[r];
+        __syncthreads();   // the previous row is done with the shared arrays
+
+        // 1.-2. A_r = G + reg*kappa*I + sum alpha v q q' in entry order, then A_r = L L'
+        const float regk = a.reg * (a.adaptive_reg ? (float)(end - beg) : 1.0f);
+        build_row_system<false>(a.G, a.Q, a.ldq, D, S, a.alpha, regk, a.keys, a.vals, beg, end, L, nullptr, Qc, cw, ck);
+        if (!cholesky_packed(L, diag, zv, D)) {
+            for (int c = tid; c < D; c += EX_THREADS) out[c] = mean[c];
+            if (tid == 0) ++nfail;
+            continue;
+        }
+
+        // 3. z ~ N(0, I)
+        normal_draws(a.seed, (uint64_t)a.draw_keys[r], D, zv);
+        __syncthreads();
+
+        // 4. L' y = z by back substitution, one warp: column j from D - 1 down, y_j = z_j / L_jj, then
+        // z_i -= L_ji y_j for i < j (row j of the packed triangle, contiguous)
+        if (tid < 32) {
+            for (int j = D - 1; j >= 0; --j) {
+                const float yj = zv[j] / diag[j];
+                if (lane == 0) yv[j] = yj;
+                const float* row = L + tri(j);
+                for (int i = lane; i < j; i += 32) zv[i] -= row[i] * yj;
+                __syncwarp();
+            }
+        }
+        __syncthreads();
+
+        // 5. out = mean + scale y (out may be mean: each element is read before it is written, by the same thread)
+        for (int c = tid; c < D; c += EX_THREADS) out[c] = mean[c] + a.scale * yv[c];
+    }
+    if (tid == 0) failed_part[blockIdx.x] = nfail;
+}
+
+// *failed += the per-CTA counts, one CTA
+__global__ void __launch_bounds__(256) failed_sum_kernel(const int64_t* part, int n, int64_t* failed) {
+    __shared__ int64_t s[256];
+    int64_t t = 0;
+    for (int i = threadIdx.x; i < n; i += 256) t += part[i];
+    s[threadIdx.x] = t;
+    __syncthreads();
+    for (int w = 128; w > 0; w >>= 1) {
+        if (threadIdx.x < w) s[threadIdx.x] += s[threadIdx.x + w];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) *failed += s[0];
+}
+
 }  // namespace
+
+int posterior_sample_launch(const PosteriorArgs& a, int num_sms, cudaStream_t st) {
+    if (a.n <= 0) return BFL_OK;
+    const size_t smem = posterior_smem_floats(a.D) * sizeof(float);
+    BFL_CUDA(cudaFuncSetAttribute(posterior_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int per_sm = 0;
+    BFL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, posterior_sample_kernel, EX_THREADS, smem));
+    if (per_sm < 1)
+        BFL_FAIL(BFL_ERR_CUDA, "posterior_sample_kernel does not fit on an SM with " + std::to_string(smem) + " B of shared memory");
+    const int grid = (int)std::min<int64_t>(a.n, (int64_t)num_sms * per_sm);
+    int64_t* part = nullptr;
+    BFL_CUDA(cudaMallocAsync(&part, sizeof(int64_t) * (size_t)grid, st));
+    posterior_sample_kernel<<<grid, EX_THREADS, smem, st>>>(a, part);
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) {
+        g_launches.fetch_add(1, std::memory_order_relaxed);
+        failed_sum_kernel<<<1, 256, 0, st>>>(part, grid, a.failed);
+        e = cudaGetLastError();
+    }
+    cudaFreeAsync(part, st);
+    BFL_CUDA(e);
+    BFL_LAUNCHED();
+    return BFL_OK;
+}
 
 int explain_launch(const ExplainArgs& a, int num_sms, cudaStream_t st) {
     if (a.n <= 0) return BFL_OK;

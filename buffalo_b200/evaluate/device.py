@@ -23,8 +23,9 @@ def _nonempty(keys):
     return keys if len(keys) else np.zeros(1, dtype=np.int32)
 
 
-def _gather_rows(indptr, keys, rows):
-    """(END offsets int64, keys int32) of the CSR rows `rows` (in that order) of a host CSR of END offsets."""
+def _gather_positions(indptr, rows):
+    """(END offsets int64, entry positions int64) of the CSR rows `rows` (in that order) of a host CSR of END offsets:
+    row i of the gathered CSR is entries pos[out_ptr[i - 1]:out_ptr[i]] of the source."""
     rows = np.asarray(rows, dtype=np.int64)
     ends = indptr[rows]
     begs = np.where(rows > 0, indptr[np.maximum(rows - 1, 0)], 0)
@@ -32,6 +33,12 @@ def _gather_rows(indptr, keys, rows):
     out_ptr = np.cumsum(lens).astype(np.int64)
     pos = np.arange(int(out_ptr[-1]) if len(out_ptr) else 0, dtype=np.int64)
     pos += np.repeat(begs - (out_ptr - lens), lens)
+    return out_ptr, pos
+
+
+def _gather_rows(indptr, keys, rows):
+    """(END offsets int64, keys int32) of the CSR rows `rows` (in that order) of a host CSR of END offsets."""
+    out_ptr, pos = _gather_positions(indptr, rows)
     return out_ptr, np.ascontiguousarray(keys[pos], dtype=np.int32)
 
 

@@ -274,18 +274,36 @@ class Parallel(object):
                 and B.shape[0] < 2 ** 31
                 and all(x.dtype == np.float32 and x.flags["C_CONTIGUOUS"] for x in (A, B)))
 
-    def _run(self, indexes, A, B, Bb, topk, pool, seen=None):
-        """seen: None, or (END offsets int64, keys int32) whose row i holds the items query indexes[i] must not get."""
+    @staticmethod
+    def _set_queries(h, A, indexes, queries):
+        """The handle's queries: the rows A[indexes], or the device rows `queries` (CUDA [len(indexes), >= d]) in their
+        place."""
+        if queries is not None:
+            h.bind_queries(queries)
+        else:
+            # only the rows asked for go to the device, read from the live array at every call
+            h.set_queries(np.ascontiguousarray(A[indexes]))
+
+    @staticmethod
+    def _host_queries(A, indexes, queries, d):
+        """(A, indexes) of the NumPy path: the device rows `queries` copied to the host in place of A[indexes]."""
+        if queries is None:
+            return A, indexes
+        return np.ascontiguousarray(queries[:, :d].cpu().numpy()), np.arange(len(indexes), dtype=np.int32)
+
+    def _run(self, indexes, A, B, Bb, topk, pool, seen=None, queries=None):
+        """seen: None, or (END offsets int64, keys int32) whose row i holds the items query indexes[i] must not get.
+        queries: None, or CUDA rows that query i ranks with instead of A[indexes[i]]."""
         if Bb is not None and not Bb.size:
             Bb = None
         if self._on_device(indexes, A, B, topk):
             h = self._serve_handle(B, None if Bb is None else np.ascontiguousarray(Bb, dtype=np.float32))
-            # only the rows asked for go to the device, read from the live array at every call
-            h.set_queries(np.ascontiguousarray(A[indexes]))
+            self._set_queries(h, A, indexes, queries)
             h.set_pool(None if pool is None or len(pool) == 0 else pool)
             if seen is not None:
                 return h.topk_seen(np.arange(len(indexes), dtype=np.int32), topk, *seen)
             return h.topk(np.arange(len(indexes), dtype=np.int32), topk)
+        A, indexes = self._host_queries(A, indexes, queries, B.shape[1])
         keys = np.zeros((len(indexes), topk), dtype=np.int32)
         scores = np.zeros((len(indexes), topk), dtype=np.float32)
         if seen is not None:
@@ -294,18 +312,19 @@ class Parallel(object):
             dot_topn(indexes, A, B, Bb, keys, scores, pool, topk, self.num_workers)
         return keys, scores
 
-    def _run_cands(self, indexes, A, B, Bb, topk, cands, seen=None):
+    def _run_cands(self, indexes, A, B, Bb, topk, cands, seen=None, queries=None):
         """_run with a candidate list per query instead of one pool: cands (END offsets int64, keys int32) whose row i
         lists the items query indexes[i] ranks."""
         if Bb is not None and not Bb.size:
             Bb = None
         if self._on_device(indexes, A, B, topk):
             h = self._serve_handle(B, None if Bb is None else np.ascontiguousarray(Bb, dtype=np.float32))
-            h.set_queries(np.ascontiguousarray(A[indexes]))
+            self._set_queries(h, A, indexes, queries)
             return h.topk_candidates(np.arange(len(indexes), dtype=np.int32), topk, *cands, seen=seen)
+        A, indexes = self._host_queries(A, indexes, queries, B.shape[1])
         return cand_topn(indexes, A, B, Bb, topk, *cands, *(seen or ()))
 
-    def _run_diverse(self, indexes, A, B, Bb, topk, div, pool=None, seen=None, cands=None):
+    def _run_diverse(self, indexes, A, B, Bb, topk, div, pool=None, seen=None, cands=None, queries=None):
         """_run (or _run_cands with cands) at k = M, then the MMR re-ranking of those M candidates down to topk against
         the item rows B; div = (w, M) of _check_diversify.  On the device the candidates never leave it."""
         w, M = div
@@ -314,15 +333,15 @@ class Parallel(object):
         if self._on_device(indexes, A, B, M):
             import torch
             h = self._serve_handle(B, None if Bb is None else np.ascontiguousarray(Bb, dtype=np.float32))
-            h.set_queries(np.ascontiguousarray(A[indexes]))
+            self._set_queries(h, A, indexes, queries)
             if cands is None:
                 h.set_pool(None if pool is None or len(pool) == 0 else pool)
             dev = torch.device("cuda", torch.cuda.current_device())
             return _rerank_batches(h, len(indexes), topk, w, M, dev, _device_stage(h, M, dev, seen, cands))
         if cands is not None:
-            keys, scores = self._run_cands(indexes, A, B, Bb, M, cands, seen)
+            keys, scores = self._run_cands(indexes, A, B, Bb, M, cands, seen, queries)
         else:
-            keys, scores = self._run(indexes, A, B, Bb, M, pool, seen)
+            keys, scores = self._run(indexes, A, B, Bb, M, pool, seen, queries)
         return mmr_numpy(keys, scores, B, topk, w)
 
 
@@ -368,8 +387,9 @@ class ParALS(Parallel):
             return None
         return np.ascontiguousarray(Qb, dtype=np.float32).reshape(-1)
 
-    def _search_index(self, group, idx, A, topk, nprobe, with_bias, normalized):
-        """The IVF search of the rows A[idx] in the group's index; every check before any device work."""
+    def _search_index(self, group, idx, A, topk, nprobe, with_bias, normalized, queries=None):
+        """The IVF search of the rows A[idx] (or of the CUDA rows `queries` in their place) in the group's index; every
+        check before any device work."""
         ivf = (getattr(self, "_indexes", None) or {}).get(group)
         if ivf is None:
             raise RuntimeError("no %s index: call build_index(nlist, group=%r) first" % (group, group))
@@ -380,6 +400,10 @@ class ParALS(Parallel):
         if now[0] != ivf.keys[0] or (with_bias and now[1] != ivf.keys[1]):
             raise RuntimeError("the %s index is stale: the factors changed since build_index; call build_index again%s"
                                % (group, " after algo.normalize(%r)" % group if normalized else ""))
+        if queries is not None:
+            ivf._attach()
+            out = ivf.search_device(queries, nprobe, topk, use_bias=with_bias and ivf.has_bias)
+            return tuple(t.cpu().numpy() for t in out)
         return ivf.search(np.ascontiguousarray(A[idx], dtype=np.float32), nprobe, topk,
                           use_bias=with_bias and ivf.has_bias)
 
@@ -422,8 +446,50 @@ class ParALS(Parallel):
         from buffalo_b200.evaluate.device import _gather_rows
         return _gather_rows(*seen_csr(self.algo, exclude_seen), idx)
 
+    def _check_explore(self, explore, explore_seed):
+        """(scale, seed) of explore / explore_seed, or None when explore is None; ValueError on bad values and
+        NotImplementedError for models without a least-squares posterior, before any device work."""
+        from buffalo_b200.algo import fold_in
+        args = fold_in.posterior_args(0.0 if explore is None else explore, explore_seed, "explore", "explore_seed")
+        if explore is None:
+            return None
+        if not callable(getattr(self.algo, "posterior_sample", None)):
+            raise NotImplementedError("explore needs a least-squares model (ALS), not %s" % type(self.algo).__name__)
+        return args
+
+    def _training_data(self, what):
+        data = getattr(self.algo, "data", None)
+        if data is None:
+            raise ValueError("%s needs the training data attached to the model" % what)
+        return data
+
+    def _training_rows(self, idx, what):
+        """scipy CSR (len(idx), num_items) of users idx's rows of the algo's training data ("rowwise" group, keys and
+        values): only those rows' entries are gathered."""
+        from buffalo_b200.evaluate.device import _gather_positions
+        grp = self._training_data(what).get_group("rowwise")
+        ends = np.asarray(grp["indptr"][:], dtype=np.int64)
+        nnz = int(ends[-1]) if len(ends) else 0
+        out_ptr, pos = _gather_positions(ends, idx)
+        keys = np.asarray(grp["key"][:nnz])[pos]
+        vals = np.asarray(grp["val"][:nnz], dtype=np.float32)[pos]
+        return scipy.sparse.csr_matrix((vals, keys, np.concatenate([[0], out_ptr])),
+                                       shape=(len(out_ptr), self.algo.Q.shape[0]))
+
+    def _explore_rows(self, idx, explore):
+        """CUDA [len(idx), vdim]: posterior_sample of the training rows of users idx around P[idx], draw key = user
+        index.  A user listed twice is sampled once and gets the same row at both places."""
+        idx = np.asarray(idx, dtype=np.int64)
+        users, where = np.unique(idx, return_inverse=True)
+        rows = self.algo._posterior_sample_device(self._training_rows(users, "explore"),
+                                                  self.algo.P[users, :self.algo.opt.d], *explore, draw_keys=users)
+        if np.array_equal(users, idx):
+            return rows
+        import torch
+        return rows[torch.from_numpy(where.reshape(-1)).to(rows.device)]
+
     def topk_recommendation(self, keys, topk=10, pool=None, repr=False, exclude_seen=False, nprobe=None,
-                            diversify=None, diversify_candidates=None):
+                            diversify=None, diversify_candidates=None, explore=None, explore_seed=0):
         """pool: None ranks every item; a list of item ids (or an index array) is one candidate pool for every user; a
         scipy sparse (num_users, num_items) matrix gives each user its own candidates, row u (as tocsr() stores it,
         values ignored, duplicates kept, ties to the earlier entry): a user's row of the result is then what a call
@@ -436,8 +502,17 @@ class ParALS(Parallel):
         diversify_candidates best candidates (M, default min(4 topk, 256), in [topk, 256]) by Maximal Marginal
         Relevance (DESIGN.md 4.15): topk picks, each the candidate of the largest (1 - w) relevance - w largest cosine
         of its item factors to the picks before it, with the candidates' scores (not sorted).  Every candidate stage
-        above takes it, nprobe does not (rerank_mmr reranks IVF results); w = 0 gives the plain result."""
+        above takes it, nprobe does not (rerank_mmr reranks IVF results); w = 0 gives the plain result.
+
+        explore: None ranks with P[u]; a finite real sigma >= 0 ranks with one Thompson-sampling draw per user instead,
+        algo.posterior_sample(user u's training row, mean P[u], scale=sigma, seed=explore_seed, draw key u) (DESIGN.md
+        4.17): P[u] moved within the Gaussian posterior of the user row that the least-squares objective implies, with
+        sigma^2 its noise variance.  Smaller sigma explores less; 0 gives the plain result.  A user's draw depends only on
+        explore_seed (an integer in [0, 2^32)) and the user, not on the batch, so a fresh seed per impression gives fresh
+        lists.  Every mode above takes it, pool, exclude_seen, diversify and nprobe included; the draws stay on the
+        device.  ALS only, with its training data attached; on the GPU only."""
         div = _check_diversify(diversify, diversify_candidates, topk)
+        exp = self._check_explore(explore, explore_seed)
         if nprobe is not None:
             if div is not None:
                 raise ValueError("nprobe does not take diversify")
@@ -448,49 +523,67 @@ class ParALS(Parallel):
         if self.algo.opt._nrz_P or self.algo.opt._nrz_Q:
             raise RuntimeError("Cannot make topk recommendation with normalized factors")
         Qb = self.algo.Qb if self._bias and self.algo.opt.get("use_bias") else None
+        if exp is not None:
+            self._training_data("explore")
         if scipy.sparse.issparse(pool):
             kept, idx, _ = self._resolve(keys, None, "user")
             topk = backend.Serve._check_k(topk)
             from buffalo_b200.evaluate.device import _gather_rows
             cands = _gather_rows(*self._pool_matrix(pool, self.algo.P.shape[0], self.algo.Q.shape[0]), idx)
             seen = self._seen_rows(idx, exclude_seen) if scipy.sparse.issparse(exclude_seen) or exclude_seen else None
-            if div is not None:
-                topks, scores = self._run_diverse(idx, self.algo.P, self.algo.Q, Qb, topk, div, seen=seen, cands=cands)
-            else:
-                topks, scores = self._run_cands(idx, self.algo.P, self.algo.Q, Qb, topk, cands, seen)
+            q = None if exp is None else self._explore_rows(idx, exp)
+            try:
+                if div is not None:
+                    topks, scores = self._run_diverse(idx, self.algo.P, self.algo.Q, Qb, topk, div, seen=seen,
+                                                      cands=cands, queries=q)
+                else:
+                    topks, scores = self._run_cands(idx, self.algo.P, self.algo.Q, Qb, topk, cands, seen, queries=q)
+            finally:
+                self._release_queries(q)
             if repr:
                 topks = [[self.algo._idmanager.itemids[t] for t in tt if t != -1] for tt in topks]
             return kept, topks, scores
         kept, idx, pool = self._resolve(keys, pool, "user")
-        if nprobe is not None:
-            topks, scores = self._search_index("item", idx, self.algo.P, topk, nprobe,
-                                               self._index_bias("item") is not None, False)
-        elif scipy.sparse.issparse(exclude_seen) or exclude_seen:
-            seen = self._seen_rows(idx, exclude_seen)
-            if div is not None:
-                topks, scores = self._run_diverse(idx, self.algo.P, self.algo.Q, Qb, topk, div, pool, seen)
+        seen = self._seen_rows(idx, exclude_seen) if nprobe is None and (
+            scipy.sparse.issparse(exclude_seen) or exclude_seen) else None
+        q = None if exp is None else self._explore_rows(idx, exp)
+        try:
+            if nprobe is not None:
+                topks, scores = self._search_index("item", idx, self.algo.P, topk, nprobe,
+                                                   self._index_bias("item") is not None, False, queries=q)
+            elif div is not None:
+                topks, scores = self._run_diverse(idx, self.algo.P, self.algo.Q, Qb, topk, div, pool, seen, queries=q)
             else:
-                topks, scores = self._run(idx, self.algo.P, self.algo.Q, Qb, topk, pool, seen)
-        elif div is not None:
-            topks, scores = self._run_diverse(idx, self.algo.P, self.algo.Q, Qb, topk, div, pool)
-        else:
-            topks, scores = self._run(idx, self.algo.P, self.algo.Q, Qb, topk, pool)
+                topks, scores = self._run(idx, self.algo.P, self.algo.Q, Qb, topk, pool, seen, queries=q)
+        finally:
+            self._release_queries(q)
         if repr:
             topks = [[self.algo._idmanager.itemids[t] for t in tt if t != -1] for tt in topks]
         return kept, topks, scores
 
+    def _release_queries(self, queries):
+        """Frees an explore call's device rows from the serve handle (every query sets its own queries first)."""
+        h = getattr(self, "_serve", None)
+        if queries is not None and h is not None:
+            h.unbind_queries()
+
     def fold_in_recommendation(self, histories, topk=10, pool=None, exclude_seen=True, repr=False, diversify=None,
-                               diversify_candidates=None):
+                               diversify_candidates=None, explore=None, explore_seed=0):
         """(topks, scores), one row per history row, for users folded into the model (DESIGN.md 4.10): the rows of
         algo.fold_in(histories) with its defaults, ranked against the items as topk_recommendation ranks (pools, -1 / 0.0
         padding).  pool may also be a scipy sparse (n, num_items) matrix: row i lists history row i's own candidates,
         as topk_recommendation takes a per-user pool.  exclude_seen: leave each row's history items out.  All on the device: the folded rows are bound as the
         serve handle's queries and never reach the host.  diversify / diversify_candidates as topk_recommendation takes
-        them: the folded rows' candidates are reranked on the device too.  Models with fold_in: ALS and PLSI."""
+        them: the folded rows' candidates are reranked on the device too.  Models with fold_in: ALS and PLSI.
+        explore / explore_seed as topk_recommendation takes them (ALS only): each folded row is replaced on the device by
+        algo.posterior_sample of its history around it, with draw key = its history row index."""
         if not callable(getattr(self.algo, "_fold_in_device", None)):
             raise NotImplementedError("fold_in_recommendation needs a model with fold_in (ALS, PLSI), not %s"
                                       % type(self.algo).__name__)
         div = _check_diversify(diversify, diversify_candidates, topk)
+        exp = self._check_explore(explore, explore_seed)
+        if exp is not None and self.algo.opt.d > self.algo.EXPLAIN_DMAX:
+            raise ValueError("explore supports d <= %d, got %d" % (self.algo.EXPLAIN_DMAX, self.algo.opt.d))
         topk = backend.Serve._check_k(topk)
         cands = None
         if scipy.sparse.issparse(pool):
@@ -504,11 +597,17 @@ class ParALS(Parallel):
             pool = self.algo.get_index_pool(pool, group="item")
             if len(pool) == 0:
                 raise RuntimeError("pool is empty")
-        tX, (indptr, keys, _) = self.algo._fold_in_device(histories)
+        tX, (indptr, keys, vals) = self.algo._fold_in_device(histories)
         n = tX.shape[0]
         if n == 0:
             return np.zeros((0, topk), np.int32), np.zeros((0, topk), np.float32)
         import torch
+        if exp is not None:
+            from buffalo_b200.algo import fold_in
+            from buffalo_b200.backend import CuALS
+            st, fh = fold_in.resident_state(self.algo, CuALS)
+            tX = self.algo._sample_rows(st, fh, (indptr, keys, vals), tX,
+                                        torch.arange(n, dtype=torch.int64, device=tX.device), seed=exp[1], scale=exp[0])
         h = self._serve_handle(np.ascontiguousarray(self.algo.Q, dtype=np.float32), None)
         try:
             h.bind_queries(tX)
@@ -528,8 +627,7 @@ class ParALS(Parallel):
                 topks, scores = idx.cpu().numpy(), val.cpu().numpy()
         finally:
             # the folded rows are freed with this call; every query on the handle sets its own queries first
-            h._bound.pop("queries", None)
-            h.num_queries = 0
+            h.unbind_queries()
         if repr:
             topks = [[self.algo._idmanager.itemids[t] for t in tt if t != -1] for tt in topks]
         return topks, scores
@@ -556,15 +654,7 @@ class ParALS(Parallel):
                 raise ValueError("keys must be a list of user ids or a 1-d array of user indexes")
             if idx.size and (int(idx.min()) < 0 or int(idx.max()) >= num_users):
                 raise ValueError("user index outside [0, %d)" % num_users)
-        data = getattr(self.algo, "data", None)
-        if data is None:
-            raise ValueError("explain needs the training data attached to the model")
-        grp = data.get_group("rowwise")
-        ends = np.asarray(grp["indptr"][:], dtype=np.int64)
-        nnz = int(ends[-1]) if len(ends) else 0
-        rows = scipy.sparse.csr_matrix((np.asarray(grp["val"][:nnz], dtype=np.float32), np.asarray(grp["key"][:nnz]),
-                                        np.concatenate([[0], ends])), shape=(len(ends), self.algo.Q.shape[0]))
-        scores, out_keys, contrib = self.algo.explain(rows[idx.astype(np.int64)], items, topm)
+        scores, out_keys, contrib = self.algo.explain(self._training_rows(idx, "explain"), items, topm)
         if repr:
             names = self.algo._idmanager.itemids
             out_keys = [[[names[t] for t in tt if t != -1] for tt in row] for row in out_keys]

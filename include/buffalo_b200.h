@@ -147,6 +147,23 @@ int bfl_als_explain_device(bfl_als_t* h, const int64_t* d_indptr, const int32_t*
                            const int32_t* d_targets, int k, int topm, float* d_scores, int32_t* d_out_keys,
                            float* d_out_contrib, void* stream);
 
+/* Posterior draws of the exact row solve (csrc/explain.cu, DESIGN.md 4.17).  For n history rows (DEVICE CSR: d_indptr
+ * int64 END offsets, d_keys int32 items in [0, Q_rows) ascending within a row (not checked), d_vals float32), with
+ * A_r = Q'Q + alpha sum v_j q_j q_j' + reg_u kappa I = L L' (kappa = the row's entry count with adaptive_reg, else 1;
+ * an empty row gives Q'Q + reg_u kappa I), writes
+ *   d_out [n, ld]              d_mean[r] + scale L^-T z_r in columns [0, d) (columns d..ld-1 are not written),
+ * where ld >= d is the row pitch of d_mean and d_out only (Q is read at the handle's own pitch),
+ * one draw from N(mean_r, scale^2 A_r^-1).  z_r ~ N(0, I) is Box-Muller on the Philox words
+ * draw_u32(seed, 0x54530417, d_draw_keys[r], t) (int64 [n], non-negative), so a row's draw depends only on the seed,
+ * its key, its history, its mean, Q, the Gram and the options, not on the other rows of the call.  d_out may be d_mean.
+ * scale = 0 copies the mean.  A row whose A_r meets a non-positive or NaN Cholesky pivot is written as its mean and
+ * counted: *d_failed (a device int64) += the number of such rows.  Reads the bound Q, the Gram of the last
+ * bfl_als_precompute_device(axis 0) (else BFL_ERR_STATE), alpha, reg_u and adaptive_reg.  d <= 256, ld >= d and a
+ * finite scale >= 0, else BFL_ERR_ARG.  No atomics. */
+int bfl_als_posterior_sample_device(bfl_als_t* h, const int64_t* d_indptr, const int32_t* d_keys, const float* d_vals,
+                                    int64_t n, const float* d_mean, int ld, const int64_t* d_draw_keys, uint32_t seed,
+                                    float scale, float* d_out, int64_t* d_failed, void* stream);
+
 /* device pointer of the current Gram matrix [d x d] (tests) */
 const float* bfl_als_gram_device(bfl_als_t* h);
 /* multi-GPU: when several ranks each computed the Gram of their shard of Y, the host
