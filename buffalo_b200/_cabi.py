@@ -127,6 +127,8 @@ PROTOTYPES = {
     "bfl_cand_topk_device": (C.c_int, [_vp, _vp, _i64, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bfl_cand_set_budget": (C.c_int, [_vp, _i64]),
     "bfl_mmr_rerank_device": (C.c_int, [_vp, _vp, _vp, _i64, C.c_int, C.c_int, C.c_float, _vp, _vp, _vp]),
+    "bfl_category_walk_device": (C.c_int, [_vp, _vp, _i64, C.c_int, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int, _vp, _vp,
+                                           _vp, _vp]),
     # IVF index
     "bfl_ivf_create": (_vp, []),
     "bfl_ivf_destroy": (None, [_vp]),

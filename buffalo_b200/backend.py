@@ -865,6 +865,33 @@ def csr_from_triples_device(major, minor, vals, num_major, num_minor, sort_minor
     return indptr, key[:n], val[:n]
 
 
+def category_table_slots(topk):
+    """Slots of a row's (category, count) table in category_walk_device's state: a power of two >= max(32, 2 topk)."""
+    return 1 << max(5, (2 * int(topk) - 1).bit_length())
+
+
+def category_walk_device(cand_idx, cand_val, rows, categories, caps, topk, state, out_idx, out_val, stream=None):
+    """One round of the per-category cap walk (bfl_category_walk_device) on torch CUDA tensors: candidate row r (int32
+    cand_idx / float32 cand_val [n, m], best first, -1 skipped) continues the walk of state / output row rows[r] (int32
+    [n], or None: row r).  categories int32 [num_items] in [-1, C); caps an int (one cap for every category) or int32
+    [C]; state int32 [R, 1 + 2 category_table_slots(topk)] zero-filled before the first round; out_idx / out_val [R,
+    topk] filled with -1 / 0.0 before it.  Stream-ordered."""
+    n, m = cand_idx.shape
+    slots = category_table_slots(topk)
+    if cand_val.shape != cand_idx.shape or state.shape[1] != 1 + 2 * slots or out_idx.shape[1] != topk \
+            or out_val.shape != out_idx.shape or state.shape[0] != out_idx.shape[0]:
+        raise ValueError("category walk: inconsistent shapes")
+    if rows is not None and rows.shape[0] != n:
+        raise ValueError("category walk: rows must name one row per candidate row")
+    scalar = isinstance(caps, (int, np.integer))
+    _cabi.check(_cabi.lib().bfl_category_walk_device(
+        _dev(cand_idx, "int32", "cand_idx"), _dev(cand_val, "float32", "cand_val"), n, m,
+        None if rows is None else _dev(rows, "int32", "rows"), _dev(categories, "int32", "categories"),
+        None if scalar else _dev(caps, "int32", "caps"), int(caps) if scalar else 0, int(topk), slots,
+        _dev(state, "int32", "state"), _dev(out_idx, "int32", "out_idx"), _dev(out_val, "float32", "out_val"),
+        _stream_ptr(stream)), "bfl_category_walk_device")
+
+
 def eval_unsorted_rows(indptr, keys, stream=None):
     """Number of rows of a device CSR (END offsets) whose keys are not non-decreasing; synchronises."""
     import torch

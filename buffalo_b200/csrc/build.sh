@@ -11,6 +11,7 @@ SRCS="$HERE/bfl_common.cu $HERE/als.cu"
 [ -f "$HERE/ivf.cu" ] && SRCS="$SRCS $HERE/ivf.cu"
 [ -f "$HERE/candidates.cu" ] && SRCS="$SRCS $HERE/candidates.cu"
 [ -f "$HERE/rerank.cu" ] && SRCS="$SRCS $HERE/rerank.cu"
+[ -f "$HERE/category.cu" ] && SRCS="$SRCS $HERE/category.cu"
 [ -f "$HERE/evaluate.cu" ] && SRCS="$SRCS $HERE/evaluate.cu"
 [ -f "$HERE/offline_eval.cu" ] && SRCS="$SRCS $HERE/offline_eval.cu"
 [ -f "$HERE/ingest.cu" ] && SRCS="$SRCS $HERE/ingest.cu"

@@ -1,1 +1,2 @@
-from buffalo_b200.parallel.base import ParALS, ParBPRMF, ParCFR, ParW2V, dot_topn, quickselect, rerank_mmr
+from buffalo_b200.parallel.base import (ParALS, ParBPRMF, ParCFR, ParW2V, cap_categories, dot_topn, quickselect,
+                                        rerank_mmr)

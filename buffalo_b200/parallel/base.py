@@ -233,6 +233,208 @@ def rerank_mmr(cand_idx, cand_val, item_factors, topk, diversify):
         h.close()
 
 
+CATEGORY_M0 = None                # first candidate depth of a capped call; None: min(SERVE_KMAX, max(4 topk, 64))
+CATEGORY_BATCH_BYTES = 1 << 30    # device buffers (deepest candidate lists, walk state, output) per batch of rows
+
+
+def _category_depth(topk):
+    return CATEGORY_M0 if CATEGORY_M0 is not None else min(backend.SERVE_KMAX, max(4 * int(topk), 64))
+
+
+def _is_int(x):
+    return isinstance(x, (int, np.integer)) and not isinstance(x, (bool, np.bool_))
+
+
+def _check_caps(categories, category_cap, rows):
+    """(categories int32 [rows], caps) of a categories / category_cap pair, caps an int (one cap for every category) or
+    int32 [C]; ValueError on anything else."""
+    cats = np.asarray(categories)
+    if cats.ndim != 1 or not np.issubdtype(cats.dtype, np.integer) or len(cats) != rows:
+        raise ValueError("categories must be a 1-d integer array with one entry per item row (%d), got %s of shape %s"
+                         % (rows, cats.dtype, cats.shape))
+    lo, hi = (int(cats.min()), int(cats.max())) if cats.size else (-1, -1)
+    if _is_int(category_cap):
+        if category_cap < 0:
+            raise ValueError("category_cap must be >= 0, got %d" % category_cap)
+        caps = int(min(category_cap, 2 ** 31 - 1))
+        ncat = hi + 1
+    else:
+        c = np.asarray(category_cap)
+        if c.ndim != 1 or not np.issubdtype(c.dtype, np.integer) or (c.size and int(c.min()) < 0):
+            raise ValueError("category_cap must be an integer >= 0 or a 1-d integer array of caps >= 0")
+        caps = np.minimum(c, 2 ** 31 - 1).astype(np.int32)
+        ncat = len(caps)
+    if lo < -1 or hi >= max(ncat, 0):
+        raise ValueError("categories must lie in [-1, %d) for this category_cap, got [%d, %d]" % (ncat, lo, hi))
+    return np.ascontiguousarray(cats, dtype=np.int32), caps
+
+
+def _check_categories(categories, category_cap, rows, topk, nprobe=None, diversify=None):
+    """(categories int32, caps) of the categories / category_cap keywords (_check_caps, rows() of them), or None when
+    neither is given; ValueError on a keyword given alone, on nprobe or diversify next to them, on a topk outside
+    [1, SERVE_KMAX] and on bad values."""
+    if categories is None and category_cap is None:
+        return None
+    if categories is None or category_cap is None:
+        raise ValueError("categories and category_cap go together")
+    if nprobe is not None:
+        raise ValueError("nprobe does not take categories (cap_categories caps IVF results)")
+    if diversify is not None:
+        raise ValueError("diversify does not take categories")
+    if not _is_int(topk) or not 1 <= topk <= backend.SERVE_KMAX:
+        raise ValueError("topk must be an integer in [1, %d] with categories, got %r" % (backend.SERVE_KMAX, topk))
+    return _check_caps(categories, category_cap, rows())
+
+
+def _check_unique_pool(pool=None, cands=None):
+    """ValueError when the shared pool, or a row of the per-user pools (END offsets, keys), lists an item twice: a
+    capped call's deeper rounds leave out items already walked, which would drop a later copy."""
+    if pool is not None and len(pool) and len(np.unique(pool)) != len(pool):
+        raise ValueError("with categories, the pool must not list an item twice")
+    if cands is not None and len(cands[1]):
+        ends = np.asarray(cands[0], dtype=np.int64)
+        keys = np.asarray(cands[1])[:int(ends[-1])]
+        row = np.repeat(np.arange(len(ends)), np.diff(ends, prepend=0))
+        o = np.lexsort((keys, row))
+        if ((row[o][1:] == row[o][:-1]) & (keys[o][1:] == keys[o][:-1])).any():
+            raise ValueError("with categories, a pool row must not list an item twice")
+
+
+def category_walk_numpy(cand_idx, cand_val, categories, caps, topk):
+    """The walk of bfl_category_walk_device in NumPy over whole lists: per row, in order, -1 skipped, an item accepted
+    when its category is -1 or fewer than its cap of that category are accepted, until topk.  (keys int32, scores
+    float32) [n, topk], -1 / 0.0 padded."""
+    n = len(cand_idx)
+    keys = np.full((n, topk), -1, dtype=np.int32)
+    scores = np.zeros((n, topk), dtype=np.float32)
+    for r in range(n):
+        count, t = {}, 0
+        for c, s in zip(cand_idx[r], cand_val[r]):
+            if t == topk:
+                break
+            if c < 0:
+                continue
+            g = int(categories[c])
+            if g >= 0:
+                if count.get(g, 0) >= (caps if _is_int(caps) else caps[g]):
+                    continue
+                count[g] = count.get(g, 0) + 1
+            keys[r, t], scores[r, t] = c, s
+            t += 1
+    return keys, scores
+
+
+def _csr_row_triples(csr, rows):
+    """(major, keys) CUDA int32 of the entries of rows `rows` (int32 CUDA) of a CUDA CSR (END offsets, keys): each
+    entry with its row number."""
+    import torch
+    ptr, keys = csr
+    r = rows.long()
+    ends = ptr[r]
+    starts = torch.cat([ptr.new_zeros(1), ptr[:-1]])[r]
+    lens = ends - starts
+    first = torch.cumsum(lens, 0) - lens
+    off = torch.arange(int(lens.sum().item()), device=ptr.device) + torch.repeat_interleave(starts - first, lens)
+    return torch.repeat_interleave(rows, lens), keys[off]
+
+
+def _capped_batches(h, n, topk, cats, caps, dev, num_items, seen=None, cands=None, stats=None):
+    """(keys int32, scores float32) host [n, topk] of the capped walk over the complete ranking of each query row of a
+    serve handle whose queries (and pool) are set, with seen / candidate CSRs as _device_stage takes them (DESIGN.md
+    4.18).  Per batch of rows: the candidate stage at depth M0, the walk, then rounds for the rows still short whose
+    stage returned M valid candidates: the stage again at twice the depth (up to SERVE_KMAX) with seen plus every item
+    walked so far left out, which is the next part of the same ranking.  stats (a list) gets (round, rows, M) per
+    round."""
+    import torch
+    if seen is not None:
+        seen = (_on_torch(seen[0], dev), _on_torch(seen[1], dev))
+    if cands is not None:
+        cands = (_on_torch(cands[0], dev), _on_torch(cands[1], dev))
+    tcats = torch.from_numpy(cats).to(dev)
+    tcaps = caps if _is_int(caps) else _on_torch(caps, dev)
+    slots = backend.category_table_slots(topk)
+    M0 = _category_depth(topk)
+    rows_max = max(1, CATEGORY_BATCH_BYTES // (8 * backend.SERVE_KMAX + 4 * (1 + 2 * slots) + 8 * topk))
+    keys = np.empty((n, topk), dtype=np.int32)
+    scores = np.empty((n, topk), dtype=np.float32)
+    for b0 in range(0, n, rows_max):
+        nb = min(rows_max, n - b0)
+        state = torch.zeros((nb, 1 + 2 * slots), dtype=torch.int32, device=dev)
+        oi = torch.full((nb, topk), -1, dtype=torch.int32, device=dev)
+        ov = torch.zeros((nb, topk), dtype=torch.float32, device=dev)
+        q = torch.arange(b0, b0 + nb, dtype=torch.int32, device=dev)
+        M, rnd = M0, 0
+        ci, cv = _device_stage(h, M, dev, seen, cands)(q)
+        w_row = w_item = torch.empty(0, dtype=torch.int32, device=dev)
+        while True:
+            rows = q - b0
+            backend.category_walk_device(ci, cv, rows, tcats, tcaps, topk, state, oi, ov)
+            if stats is not None:
+                stats.append((rnd, len(q), M))
+            more = (state[rows.long(), 0] < topk) & (ci[:, M - 1] >= 0)
+            if not bool(more.any().item()):
+                break
+            valid = ci >= 0
+            w_row = torch.cat([w_row, torch.repeat_interleave(q, valid.sum(1))])
+            w_item = torch.cat([w_item, ci[valid]])
+            q = q[more]
+            live = torch.zeros(n, dtype=torch.bool, device=dev)
+            live[q.long()] = True
+            keep = live[w_row.long()]
+            w_row, w_item = w_row[keep], w_item[keep]
+            major, minor = w_row, w_item
+            if seen is not None:
+                sm, sk = _csr_row_triples(seen, q)
+                major, minor = torch.cat([sm, major]), torch.cat([sk, minor])
+            excl = backend.csr_from_triples_device(major, minor, torch.ones(len(major), dtype=torch.float32, device=dev),
+                                                   n, num_items)[:2]
+            M, rnd = min(2 * M, backend.SERVE_KMAX), rnd + 1
+            ci, cv = _device_stage(h, M, dev, excl, cands)(q)
+        keys[b0:b0 + nb], scores[b0:b0 + nb] = oi.cpu().numpy(), ov.cpu().numpy()
+    return keys, scores
+
+
+def cap_categories(cand_idx, cand_val, categories, category_cap, topk):
+    """Per-category caps over ranked lists made elsewhere, such as IVF results or rerank_mmr output: cand_idx an (n, m)
+    integer array of item indexes best first (-1 entries skipped), cand_val their scores, categories one integer per
+    item in [-1, C) (-1: not capped), category_cap an integer >= 0 (every category's cap) or an array of C caps >= 0 (0
+    bans a category).  Per row, the list is walked in order and an item kept when its category is -1 or fewer than its
+    cap items of that category are kept already, until topk are kept.  Returns (keys int32, scores float32) [n, topk],
+    the scores as given, -1 / 0.0 padded.  The result is exact with respect to the given lists only: an item that a
+    deeper list would have brought in is not considered, so a row can come back short where the ranking it was cut
+    from had more to give (topk_recommendation(categories=...) walks the complete ranking).  On the GPU when one is
+    present, in NumPy otherwise."""
+    ci, cv = np.asarray(cand_idx), np.asarray(cand_val)
+    if ci.ndim != 2 or not np.issubdtype(ci.dtype, np.integer) or ci.shape[1] < 1 or cv.shape != ci.shape:
+        raise ValueError("cand_idx must be an (n, m) integer array with m >= 1 and cand_val of the same shape, got %s "
+                         "and %s" % (ci.shape, cv.shape))
+    if not _is_int(topk) or topk < 1:
+        raise ValueError("topk must be an integer >= 1, got %r" % (topk,))
+    cats = np.asarray(categories)
+    cats, caps = _check_caps(cats, category_cap, cats.shape[0] if cats.ndim == 1 else -1)
+    if ci.size and (int(ci.min()) < -1 or int(ci.max()) >= len(cats)):
+        raise ValueError("cand_idx holds an index outside [-1, %d)" % len(cats))
+    n, m = ci.shape
+    k = min(int(topk), m)
+    ci, cv = np.ascontiguousarray(ci, dtype=np.int32), np.ascontiguousarray(cv, dtype=np.float32)
+    keys = np.full((n, int(topk)), -1, dtype=np.int32)
+    scores = np.zeros((n, int(topk)), dtype=np.float32)
+    if not (backend.device_available() and n and len(cats)):
+        keys[:, :k], scores[:, :k] = category_walk_numpy(ci, cv, cats, caps, k)
+        return keys, scores
+    import torch
+    dev = torch.device("cuda", torch.cuda.current_device())
+    slots = backend.category_table_slots(k)
+    state = torch.zeros((n, 1 + 2 * slots), dtype=torch.int32, device=dev)
+    oi = torch.full((n, k), -1, dtype=torch.int32, device=dev)
+    ov = torch.zeros((n, k), dtype=torch.float32, device=dev)
+    backend.category_walk_device(torch.from_numpy(ci).to(dev), torch.from_numpy(cv).to(dev), None,
+                                 torch.from_numpy(cats).to(dev), caps if _is_int(caps) else _on_torch(caps, dev), k,
+                                 state, oi, ov)
+    keys[:, :k], scores[:, :k] = oi.cpu().numpy(), ov.cpu().numpy()
+    return keys, scores
+
+
 class Parallel(object):
     def __init__(self, algo, *argv, **kwargs):
         self.algo = algo
@@ -344,6 +546,32 @@ class Parallel(object):
             keys, scores = self._run(indexes, A, B, Bb, M, pool, seen, queries)
         return mmr_numpy(keys, scores, B, topk, w)
 
+    def _run_capped(self, indexes, A, B, Bb, topk, cat, pool=None, seen=None, cands=None, queries=None):
+        """_run (or _run_cands with cands) with the per-category caps cat = (categories, caps) of _check_categories
+        applied over each query's complete ranking (DESIGN.md 4.18).  On the device the candidates never leave it;
+        without one the complete ranking is computed in NumPy and walked."""
+        if Bb is not None and not Bb.size:
+            Bb = None
+        if self._on_device(indexes, A, B, _category_depth(topk)):
+            import torch
+            h = self._serve_handle(B, None if Bb is None else np.ascontiguousarray(Bb, dtype=np.float32))
+            self._set_queries(h, A, indexes, queries)
+            if cands is None:
+                h.set_pool(None if pool is None or len(pool) == 0 else pool)
+            dev = torch.device("cuda", torch.cuda.current_device())
+            return _capped_batches(h, len(indexes), topk, *cat, dev, B.shape[0], seen, cands)
+        A, indexes = self._host_queries(A, indexes, queries, B.shape[1])
+        if cands is not None:
+            ends = np.asarray(cands[0], dtype=np.int64)
+            depth = max(1, int(np.diff(ends, prepend=0).max()) if len(ends) else 1)
+            keys, scores = cand_topn(indexes, A, B, Bb, depth, *cands, *(seen or ()))
+        else:
+            depth = B.shape[0] if pool is None or len(pool) == 0 else len(pool)
+            keys = np.zeros((len(indexes), depth), dtype=np.int32)
+            scores = np.zeros((len(indexes), depth), dtype=np.float32)
+            dot_topn(indexes, A, B, Bb, keys, scores, pool, depth, self.num_workers, *(seen or ()))
+        return category_walk_numpy(keys, scores, *cat, topk)
+
 
 class ParALS(Parallel):
     _bias = False
@@ -408,12 +636,16 @@ class ParALS(Parallel):
                           use_bias=with_bias and ivf.has_bias)
 
     def most_similar(self, keys, topk=10, group="item", pool=None, repr=False, ef_search=-1, use_mmap=True,
-                     nprobe=None):
+                     nprobe=None, categories=None, category_cap=None):
         """nprobe: None ranks every row; an integer in [1, nlist] searches the group's index (build_index, after
-        algo.normalize(group)) and ranks the rows of the nprobe lists nearest each query.  ef_search and use_mmap are
-        accepted and ignored."""
+        algo.normalize(group)) and ranks the rows of the nprobe lists nearest each query.  categories / category_cap
+        as topk_recommendation takes them, one category per row of the group, without nprobe.  ef_search and use_mmap
+        are accepted and ignored."""
         if nprobe is not None and pool is not None:
             raise ValueError("nprobe does not take a pool")
+        if group in ("item", "user"):
+            cat = _check_categories(categories, category_cap,
+                                    lambda: (self.algo.Q if group == "item" else self.algo.P).shape[0], topk, nprobe)
         self.algo.normalize(group=group)
         _, idx, pool = self._resolve(keys, pool, group)
         if group not in ("item", "user"):
@@ -422,6 +654,9 @@ class ParALS(Parallel):
         names = self.algo._idmanager.itemids if group == "item" else self.algo._idmanager.userids
         if nprobe is not None:
             topks, scores = self._search_index(group, idx, F, topk, nprobe, False, True)
+        elif cat is not None:
+            _check_unique_pool(pool)
+            topks, scores = self._run_capped(idx, F, F, None, topk, cat, pool)
         else:
             topks, scores = self._run(idx, F, F, None, topk, pool)
         if repr:
@@ -489,7 +724,8 @@ class ParALS(Parallel):
         return rows[torch.from_numpy(where.reshape(-1)).to(rows.device)]
 
     def topk_recommendation(self, keys, topk=10, pool=None, repr=False, exclude_seen=False, nprobe=None,
-                            diversify=None, diversify_candidates=None, explore=None, explore_seed=0):
+                            diversify=None, diversify_candidates=None, explore=None, explore_seed=0, categories=None,
+                            category_cap=None):
         """pool: None ranks every item; a list of item ids (or an index array) is one candidate pool for every user; a
         scipy sparse (num_users, num_items) matrix gives each user its own candidates, row u (as tocsr() stores it,
         values ignored, duplicates kept, ties to the earlier entry): a user's row of the result is then what a call
@@ -510,8 +746,18 @@ class ParALS(Parallel):
         sigma^2 its noise variance.  Smaller sigma explores less; 0 gives the plain result.  A user's draw depends only on
         explore_seed (an integer in [0, 2^32)) and the user, not on the batch, so a fresh seed per impression gives fresh
         lists.  Every mode above takes it, pool, exclude_seen, diversify and nprobe included; the draws stay on the
-        device.  ALS only, with its training data attached; on the GPU only."""
+        device.  ALS only, with its training data attached; on the GPU only.
+
+        categories / category_cap: None, or both: categories a 1-d integer array with one category in [-1, C) per item
+        row (algo.Q.shape[0], items of add_items included; -1: not capped), category_cap an integer >= 0 (the cap of
+        every category, C = max(categories) + 1) or an integer array of C caps >= 0 (0 bans a category).  Each row is
+        then the walk of the user's complete ranking (what this call without them returns at topk = the number of
+        candidates: pool, per-user pool, exclude_seen, explore and bias included), in order, that accepts an item when
+        its category is -1 or fewer than its cap items of that category are accepted already, until topk (DESIGN.md
+        4.18), with that ranking's keys and score bits, -1 / 0.0 padded when it runs out.  Not with nprobe or diversify
+        (cap_categories caps lists made elsewhere); a pool must not list an item twice; topk in [1, 4096]."""
         div = _check_diversify(diversify, diversify_candidates, topk)
+        cat = _check_categories(categories, category_cap, lambda: self.algo.Q.shape[0], topk, nprobe, diversify)
         exp = self._check_explore(explore, explore_seed)
         if nprobe is not None:
             if div is not None:
@@ -530,10 +776,15 @@ class ParALS(Parallel):
             topk = backend.Serve._check_k(topk)
             from buffalo_b200.evaluate.device import _gather_rows
             cands = _gather_rows(*self._pool_matrix(pool, self.algo.P.shape[0], self.algo.Q.shape[0]), idx)
+            if cat is not None:
+                _check_unique_pool(cands=cands)
             seen = self._seen_rows(idx, exclude_seen) if scipy.sparse.issparse(exclude_seen) or exclude_seen else None
             q = None if exp is None else self._explore_rows(idx, exp)
             try:
-                if div is not None:
+                if cat is not None:
+                    topks, scores = self._run_capped(idx, self.algo.P, self.algo.Q, Qb, topk, cat, seen=seen,
+                                                     cands=cands, queries=q)
+                elif div is not None:
                     topks, scores = self._run_diverse(idx, self.algo.P, self.algo.Q, Qb, topk, div, seen=seen,
                                                       cands=cands, queries=q)
                 else:
@@ -544,6 +795,8 @@ class ParALS(Parallel):
                 topks = [[self.algo._idmanager.itemids[t] for t in tt if t != -1] for tt in topks]
             return kept, topks, scores
         kept, idx, pool = self._resolve(keys, pool, "user")
+        if cat is not None:
+            _check_unique_pool(pool)
         seen = self._seen_rows(idx, exclude_seen) if nprobe is None and (
             scipy.sparse.issparse(exclude_seen) or exclude_seen) else None
         q = None if exp is None else self._explore_rows(idx, exp)
@@ -551,6 +804,8 @@ class ParALS(Parallel):
             if nprobe is not None:
                 topks, scores = self._search_index("item", idx, self.algo.P, topk, nprobe,
                                                    self._index_bias("item") is not None, False, queries=q)
+            elif cat is not None:
+                topks, scores = self._run_capped(idx, self.algo.P, self.algo.Q, Qb, topk, cat, pool, seen, queries=q)
             elif div is not None:
                 topks, scores = self._run_diverse(idx, self.algo.P, self.algo.Q, Qb, topk, div, pool, seen, queries=q)
             else:
@@ -568,7 +823,8 @@ class ParALS(Parallel):
             h.unbind_queries()
 
     def fold_in_recommendation(self, histories, topk=10, pool=None, exclude_seen=True, repr=False, diversify=None,
-                               diversify_candidates=None, explore=None, explore_seed=0):
+                               diversify_candidates=None, explore=None, explore_seed=0, categories=None,
+                               category_cap=None):
         """(topks, scores), one row per history row, for users folded into the model (DESIGN.md 4.10): the rows of
         algo.fold_in(histories) with its defaults, ranked against the items as topk_recommendation ranks (pools, -1 / 0.0
         padding).  pool may also be a scipy sparse (n, num_items) matrix: row i lists history row i's own candidates,
@@ -576,11 +832,13 @@ class ParALS(Parallel):
         serve handle's queries and never reach the host.  diversify / diversify_candidates as topk_recommendation takes
         them: the folded rows' candidates are reranked on the device too.  Models with fold_in: ALS and PLSI.
         explore / explore_seed as topk_recommendation takes them (ALS only): each folded row is replaced on the device by
-        algo.posterior_sample of its history around it, with draw key = its history row index."""
+        algo.posterior_sample of its history around it, with draw key = its history row index.  categories /
+        category_cap as topk_recommendation takes them: each row walks the folded row's complete ranking."""
         if not callable(getattr(self.algo, "_fold_in_device", None)):
             raise NotImplementedError("fold_in_recommendation needs a model with fold_in (ALS, PLSI), not %s"
                                       % type(self.algo).__name__)
         div = _check_diversify(diversify, diversify_candidates, topk)
+        cat = _check_categories(categories, category_cap, lambda: self.algo.Q.shape[0], topk, None, diversify)
         exp = self._check_explore(explore, explore_seed)
         if exp is not None and self.algo.opt.d > self.algo.EXPLAIN_DMAX:
             raise ValueError("explore supports d <= %d, got %d" % (self.algo.EXPLAIN_DMAX, self.algo.opt.d))
@@ -597,6 +855,8 @@ class ParALS(Parallel):
             pool = self.algo.get_index_pool(pool, group="item")
             if len(pool) == 0:
                 raise RuntimeError("pool is empty")
+        if cat is not None:
+            _check_unique_pool(pool, cands)
         tX, (indptr, keys, vals) = self.algo._fold_in_device(histories)
         n = tX.shape[0]
         if n == 0:
@@ -613,7 +873,10 @@ class ParALS(Parallel):
             h.bind_queries(tX)
             h.set_pool(pool)
             qidx = torch.arange(n, dtype=torch.int32, device=tX.device)
-            if div is not None:
+            if cat is not None:
+                topks, scores = _capped_batches(h, n, topk, *cat, tX.device, self.algo.Q.shape[0],
+                                                (indptr, keys) if exclude_seen else None, cands)
+            elif div is not None:
                 topks, scores = _rerank_batches(h, n, topk, div[0], div[1], tX.device, _device_stage(
                     h, div[1], tX.device, (indptr, keys) if exclude_seen else None, cands))
             elif cands is not None:
@@ -623,7 +886,7 @@ class ParALS(Parallel):
                 idx, val = h.topk_seen_device(qidx, topk, indptr, keys)
             else:
                 idx, val = h.topk_device(qidx, topk)
-            if div is None:
+            if div is None and cat is None:
                 topks, scores = idx.cpu().numpy(), val.cpu().numpy()
         finally:
             # the folded rows are freed with this call; every query on the handle sets its own queries first

@@ -477,6 +477,25 @@ int bfl_mmr_rerank_device(bfl_serve_t* h, const int32_t* d_cand_idx, const float
                           int k, float diversify, int32_t* d_out_idx, float* d_out_val, void* stream);
 
 /* =====================================================================================
+ * Per-category caps over ranked lists (DESIGN.md 4.18): the walk of ParALS / ParBPRMF topk_recommendation(categories,
+ * category_cap) and buffalo_b200.parallel.cap_categories.  Row r of the candidates, d_cand_idx / d_cand_val
+ * [r * m .. r * m + m) (item ids best first, -1 entries skipped, with their scores), continues the walk of state and
+ * output row d_rows[r] (d_rows nullable: row r): in order, an item is accepted when its category d_categories[item] is
+ * -1 or fewer than its cap items of that category are accepted already, until topk are accepted.  The cap of category
+ * g is d_caps[g] (d_caps nullable: cap_all for every category); every category of a candidate must be in [-1, C) for
+ * d_caps of C entries.  Accepted items go to d_out_idx / d_out_val [rows x topk] at the row's next free places with
+ * their score bits; the caller fills those with -1 / 0.0f before the first call.  d_state [rows x (1 + 2 slots)] int32
+ * holds per row the accepted count and an open-addressed table of `slots` (category + 1, count) pairs; the caller
+ * zero-fills it before the first call.  slots: a power of two of at least 2 topk.  So calls over consecutive parts of
+ * one ranking give what one call over the whole ranking gives, and a row's result depends on its own candidates alone.
+ * One warp per row, no atomics.  Bad arguments are BFL_ERR_ARG before any launch.  DEVICE arrays, stream-ordered.
+ * ===================================================================================== */
+int bfl_category_walk_device(const int32_t* d_cand_idx, const float* d_cand_val, int64_t n, int m,
+                             const int32_t* d_rows /* nullable */, const int32_t* d_categories,
+                             const int32_t* d_caps /* nullable */, int cap_all, int topk, int slots, int32_t* d_state,
+                             int32_t* d_out_idx, float* d_out_val, void* stream);
+
+/* =====================================================================================
  * Inverted-file (IVF-Flat) index for batch serving (DESIGN.md 4.12).  build_device clusters n DEVICE rows (pitch ld,
  * first d columns, d <= 256) by spherical k-means into nlist lists (nlist in [1, min(n, 65536)], iters >= 1): nlist
  * distinct rows drawn with `seed` start it, each row goes to the centroid of the largest dot product (ties to the
