@@ -13,7 +13,7 @@ folded into a model of 100k and of 1M items (random factors; only the item facto
                + 8 * vdim B per row (read start row, write result); GB/s = model bytes / kernel seconds (item rows that
                hit L2 count as if read from HBM, so this is an effective rate, not a measured DRAM rate).
   - serve    : ParALS.fold_in_recommendation (k = 10, exclude_seen) against fold_in followed by the host-array path
-               topk_recommendation(exclude_seen=...) runs (Parallel._run: folded rows and seen CSR uploaded from the
+               topk_recommendation(exclude_seen=...) runs (Parallel._rank: folded rows and seen CSR uploaded from the
                host, bfl_seen_topk), both with a resident item handle; host clock; keys compared.
 The median of `--repeats` timed calls after one warm-up call is printed.  One JSON line per case; the card's name and
 power limit are read in the same process.
@@ -149,7 +149,7 @@ def main():
 
                 def host_path():
                     X = m.fold_in(H)
-                    return par._run(np.arange(a.users, dtype=np.int32), X, m.Q, None, 10, None, (indptr, keys))
+                    return par._rank(np.arange(a.users, dtype=np.int32), X, m.Q, None, 10, seen=(indptr, keys))
                 (k2, _), t_host = timed(host_path, a.repeats)
                 print(json.dumps(dict(base, case="serve", items=num_items, d=d, k=10, device_path_s=round(t_dev, 4),
                                       host_round_trip_s=round(t_host, 4), same_keys=bool(np.array_equal(k1, k2)))),

@@ -645,19 +645,32 @@ class Serve(_Holder):
             raise ValueError("k must be in [1, %d]" % SERVE_KMAX)
         return k
 
-    def topk(self, query_idx, k, want_scores=True):
-        """(int32 [n, k] item ids, float32 [n, k] scores or None) for the rows query_idx of the query matrix: best
-        first, ties to the smaller id, -1 / 0.0 where fewer than k candidates exist."""
+    def _topk_host(self, name, query_idx, k, want_scores, rows=lambda n: ()):
+        """The host-array entries: k and the query indexes checked, then rows(n) (the entry's CSR arguments for n
+        queries, checked: arrays or None), then bfl_<name>(handle, queries, n, k, *their pointers, outputs), which
+        batches the queries and copies each batch back while the next one runs; not called for no queries."""
         k = self._check_k(k)
         q = np.ascontiguousarray(query_idx, dtype=np.int32).reshape(-1)
         if q.size and (q.min() < 0 or q.max() >= self.num_queries):
             raise ValueError("query index out of range")
+        arrays = rows(q.size)
         idx = np.empty((q.size, k), dtype=np.int32)
         val = np.empty((q.size, k), dtype=np.float32) if want_scores else None
         if q.size:
-            _cabi.check(self._fn("topk")(self._h, q.ctypes.data, q.size, k, idx.ctypes.data,
-                                         None if val is None else val.ctypes.data), "bfl_serve_topk")
+            ptrs = [None if a is None else a.ctypes.data for a in arrays]
+            _cabi.check(getattr(self._lib, "bfl_" + name)(self._h, q.ctypes.data, q.size, k, *ptrs, idx.ctypes.data,
+                                                          None if val is None else val.ctypes.data), "bfl_" + name)
         return idx, val
+
+    def _host_rows(self, n, indptr, keys, what="seen"):
+        """(END offsets, keys) of a host CSR argument checked by _check_seen (keys: one zero when empty)."""
+        nnz = self._check_seen(n, indptr, keys, host=True, what=what)
+        return indptr, keys if nnz else np.zeros(1, np.int32)
+
+    def topk(self, query_idx, k, want_scores=True):
+        """(int32 [n, k] item ids, float32 [n, k] scores or None) for the rows query_idx of the query matrix: best
+        first, ties to the smaller id, -1 / 0.0 where fewer than k candidates exist."""
+        return self._topk_host("serve_topk", query_idx, k, want_scores)
 
     def topk_device(self, query_idx, k, stream=None):
         """torch CUDA int32 query_idx [n] -> (int32 [n, k], float32 [n, k]) CUDA tensors, stream-ordered."""
@@ -696,19 +709,24 @@ class Serve(_Holder):
         """topk with query i's seen items left out: row i of the host CSR (seen_indptr int64 END offsets [n], seen_keys
         int32 item ids in any order, duplicates allowed).  The survivors keep their order and score bits; -1 / 0.0 pad
         when fewer than k candidates remain."""
-        k = self._check_k(k)
-        q = np.ascontiguousarray(query_idx, dtype=np.int32).reshape(-1)
-        if q.size and (q.min() < 0 or q.max() >= self.num_queries):
-            raise ValueError("query index out of range")
-        nnz = self._check_seen(q.size, seen_indptr, seen_keys, host=True)
-        keys = seen_keys if nnz else np.zeros(1, np.int32)
-        idx = np.empty((q.size, k), dtype=np.int32)
-        val = np.empty((q.size, k), dtype=np.float32) if want_scores else None
-        if q.size:
-            _cabi.check(self._lib.bfl_seen_topk(self._h, q.ctypes.data, q.size, k, seen_indptr.ctypes.data,
-                                                keys.ctypes.data, idx.ctypes.data,
-                                                None if val is None else val.ctypes.data), "bfl_seen_topk")
-        return idx, val
+        return self._topk_host("seen_topk", query_idx, k, want_scores,
+                               lambda n: self._host_rows(n, seen_indptr, seen_keys))
+
+    def _device_rows(self, indptr, keys, row, n, what, stream):
+        """(END offsets, keys, row map) of a CSR of torch CUDA tensors (int64 END offsets, int32 keys) that n queries
+        read: checked by _check_seen (keys: one zero when empty); seen rows not in ascending order sorted first with the
+        device radix sort (eval_unsorted_rows, csr_from_triples_device; that check synchronises), candidate lists kept
+        in their order; the row map checked by _check_rows."""
+        import torch
+        dev = indptr.device
+        nnz = self._check_seen(indptr.shape[0], indptr, keys, host=False, what=what)
+        keys = keys[:nnz] if nnz else torch.zeros(1, dtype=torch.int32, device=dev)
+        if what == "seen" and nnz and eval_unsorted_rows(indptr, keys, stream):
+            lens = torch.diff(indptr, prepend=indptr.new_zeros(1))
+            major = torch.repeat_interleave(torch.arange(indptr.shape[0], dtype=torch.int32, device=dev), lens)
+            indptr, keys, _ = csr_from_triples_device(major, keys, torch.ones(nnz, dtype=torch.float32, device=dev),
+                                                      indptr.shape[0], self.num_items, stream=stream)
+        return indptr, keys, self._check_rows(row, n, indptr.shape[0], what)
 
     def topk_seen_device(self, query_idx, k, seen_indptr, seen_keys, seen_row=None, stream=None):
         """topk_device with query q's seen items left out: row seen_row[q] (default q) of a CSR of torch CUDA tensors
@@ -718,21 +736,9 @@ class Serve(_Holder):
         k = self._check_k(k)
         n = query_idx.shape[0]
         dev = query_idx.device
-        nnz = self._check_seen(seen_indptr.shape[0], seen_indptr, seen_keys, host=False)
-        keys = seen_keys[:nnz] if nnz else torch.zeros(1, dtype=torch.int32, device=dev)
-        if nnz and eval_unsorted_rows(seen_indptr, keys, stream):
-            lens = torch.diff(seen_indptr, prepend=seen_indptr.new_zeros(1))
-            major = torch.repeat_interleave(torch.arange(seen_indptr.shape[0], dtype=torch.int32, device=dev), lens)
-            seen_indptr, keys, _ = csr_from_triples_device(major, keys, torch.ones(nnz, dtype=torch.float32, device=dev),
-                                                           seen_indptr.shape[0], self.num_items, stream=stream)
+        seen_indptr, keys, seen_row = self._device_rows(seen_indptr, seen_keys, seen_row, n, "seen", stream)
         if seen_row is None:
-            if seen_indptr.shape[0] != n:
-                raise ValueError("without seen_row the CSR needs one row per query")
-            seen_row = torch.arange(n, dtype=torch.int32, device=dev)
-        elif seen_row.shape[0] != n:
-            raise ValueError("seen_row must name one row per query")
-        elif n and (int(seen_row.min().item()) < 0 or int(seen_row.max().item()) >= seen_indptr.shape[0]):
-            raise ValueError("seen_row names a row outside the seen CSR")
+            seen_row = torch.arange(n, dtype=torch.int32, device=dev)     # bfl_seen_topk_device takes a row map
         idx = torch.empty((n, k), dtype=torch.int32, device=dev)
         val = torch.empty((n, k), dtype=torch.float32, device=dev)
         if n:
@@ -742,32 +748,14 @@ class Serve(_Holder):
                 "bfl_seen_topk_device")
         return idx, val
 
-
     def topk_candidates(self, query_idx, k, cand_indptr, cand_keys, seen=None, want_scores=True):
         """topk where query i ranks only its own candidate list, row i of the host CSR (cand_indptr int64 END offsets
         [n], cand_keys int32 item ids in any order, duplicates allowed) instead of the pool: row i is bitwise what topk
         returns for query i alone with set_pool(its list), ties to the earlier list position.  seen: None or
         (seen_indptr, seen_keys) as topk_seen takes them.  An empty list, or fewer than k candidates left, pads with
         -1 / 0.0."""
-        k = self._check_k(k)
-        q = np.ascontiguousarray(query_idx, dtype=np.int32).reshape(-1)
-        if q.size and (q.min() < 0 or q.max() >= self.num_queries):
-            raise ValueError("query index out of range")
-        nc = self._check_seen(q.size, cand_indptr, cand_keys, host=True, what="cand")
-        ckeys = cand_keys if nc else np.zeros(1, np.int32)
-        sptr = skeys = None
-        if seen is not None:
-            sptr, skeys = seen
-            ns = self._check_seen(q.size, sptr, skeys, host=True)
-            skeys = skeys if ns else np.zeros(1, np.int32)
-        idx = np.empty((q.size, k), dtype=np.int32)
-        val = np.empty((q.size, k), dtype=np.float32) if want_scores else None
-        if q.size:
-            _cabi.check(self._lib.bfl_cand_topk(self._h, q.ctypes.data, q.size, k, cand_indptr.ctypes.data,
-                                                ckeys.ctypes.data, None if sptr is None else sptr.ctypes.data,
-                                                None if skeys is None else skeys.ctypes.data, idx.ctypes.data,
-                                                None if val is None else val.ctypes.data), "bfl_cand_topk")
-        return idx, val
+        return self._topk_host("cand_topk", query_idx, k, want_scores, lambda n: self._host_rows(
+            n, cand_indptr, cand_keys, "cand") + ((None, None) if seen is None else self._host_rows(n, *seen)))
 
     def topk_candidates_device(self, query_idx, k, cand_indptr, cand_keys, cand_row=None, seen=None, stream=None):
         """topk_candidates on torch CUDA tensors, stream-ordered: query q ranks row cand_row[q] (default q) of the
@@ -778,21 +766,11 @@ class Serve(_Holder):
         k = self._check_k(k)
         n = query_idx.shape[0]
         dev = query_idx.device
-        nc = self._check_seen(cand_indptr.shape[0], cand_indptr, cand_keys, host=False, what="cand")
-        ckeys = cand_keys[:nc] if nc else torch.zeros(1, dtype=torch.int32, device=dev)
-        cand_row = self._check_rows(cand_row, n, cand_indptr.shape[0], "cand")
+        cand_indptr, ckeys, cand_row = self._device_rows(cand_indptr, cand_keys, cand_row, n, "cand", stream)
         sptr = skeys = srow = None
         if seen is not None:
-            sptr, skeys = seen[0], seen[1]
-            srow = seen[2] if len(seen) > 2 else None
-            ns = self._check_seen(sptr.shape[0], sptr, skeys, host=False)
-            skeys = skeys[:ns] if ns else torch.zeros(1, dtype=torch.int32, device=dev)
-            if ns and eval_unsorted_rows(sptr, skeys, stream):
-                lens = torch.diff(sptr, prepend=sptr.new_zeros(1))
-                major = torch.repeat_interleave(torch.arange(sptr.shape[0], dtype=torch.int32, device=dev), lens)
-                sptr, skeys, _ = csr_from_triples_device(major, skeys, torch.ones(ns, dtype=torch.float32, device=dev),
-                                                         sptr.shape[0], self.num_items, stream=stream)
-            srow = self._check_rows(srow, n, sptr.shape[0], "seen")
+            sptr, skeys, srow = self._device_rows(seen[0], seen[1], seen[2] if len(seen) > 2 else None, n, "seen",
+                                                  stream)
         idx = torch.empty((n, k), dtype=torch.int32, device=dev)
         val = torch.empty((n, k), dtype=torch.float32, device=dev)
         if n:

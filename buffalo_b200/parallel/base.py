@@ -115,12 +115,11 @@ def _check_diversify(diversify, candidates, topk):
     if isinstance(diversify, bool) or not isinstance(diversify, (int, float, np.integer, np.floating)) \
             or not 0 <= diversify <= 1:
         raise ValueError("diversify must be None or a real number in [0, 1], got %r" % (diversify,))
-    if isinstance(topk, bool) or not isinstance(topk, (int, np.integer)) or not 1 <= topk <= backend.MMR_MMAX:
+    if not _is_int(topk) or not 1 <= topk <= backend.MMR_MMAX:
         raise ValueError("topk must be an integer in [1, %d] with diversify, got %r" % (backend.MMR_MMAX, topk))
     if candidates is None:
         candidates = min(4 * int(topk), backend.MMR_MMAX)
-    if isinstance(candidates, bool) or not isinstance(candidates, (int, np.integer)) \
-            or not topk <= candidates <= backend.MMR_MMAX:
+    if not _is_int(candidates) or not topk <= candidates <= backend.MMR_MMAX:
         raise ValueError("diversify_candidates must be an integer in [topk, %d] = [%d, %d], got %r"
                          % (backend.MMR_MMAX, topk, backend.MMR_MMAX, candidates))
     return float(np.float32(diversify)), int(candidates)
@@ -214,7 +213,7 @@ def rerank_mmr(cand_idx, cand_val, item_factors, topk, diversify):
     n, m = ci.shape
     if m > backend.MMR_MMAX:
         raise ValueError("at most %d candidates per row, got %d" % (backend.MMR_MMAX, m))
-    if isinstance(topk, bool) or not isinstance(topk, (int, np.integer)) or not 1 <= topk <= m:
+    if not _is_int(topk) or not 1 <= topk <= m:
         raise ValueError("topk must be an integer in [1, %d], got %r" % (m, topk))
     w, _ = _check_diversify(diversify, m, topk)
     if ci.size and (int(ci.min()) < -1 or int(ci.max()) >= F.shape[0]):
@@ -469,18 +468,23 @@ class Parallel(object):
         return self._serve
 
     @staticmethod
-    def _on_device(indexes, A, B, topk):
+    def _on_device(indexes, A, B, topk, queries=None):
         # On the device when one is present and the call is within the kernels' limits.  The items must fit in device
         # memory next to the gathered query rows: an allocation failure is an error, not a silent switch to NumPy.
+        # Device query rows stand in for A, which is then not looked at.
         return (backend.device_available() and len(indexes) and 0 < topk <= backend.SERVE_KMAX
                 and B.shape[0] < 2 ** 31
-                and all(x.dtype == np.float32 and x.flags["C_CONTIGUOUS"] for x in (A, B)))
+                and all(x.dtype == np.float32 and x.flags["C_CONTIGUOUS"]
+                        for x in ((A, B) if queries is None else (B,))))
 
     @staticmethod
     def _set_queries(h, A, indexes, queries):
         """The handle's queries: the rows A[indexes], or the device rows `queries` (CUDA [len(indexes), >= d]) in their
         place."""
         if queries is not None:
+            import torch
+            # the host entries read the rows on the handle's own streams, which do not wait for the caller's
+            torch.cuda.current_stream(queries.device).synchronize()
             h.bind_queries(queries)
         else:
             # only the rows asked for go to the device, read from the live array at every call
@@ -493,84 +497,63 @@ class Parallel(object):
             return A, indexes
         return np.ascontiguousarray(queries[:, :d].cpu().numpy()), np.arange(len(indexes), dtype=np.int32)
 
-    def _run(self, indexes, A, B, Bb, topk, pool, seen=None, queries=None):
-        """seen: None, or (END offsets int64, keys int32) whose row i holds the items query indexes[i] must not get.
-        queries: None, or CUDA rows that query i ranks with instead of A[indexes[i]]."""
+    def _rank(self, indexes, A, B, Bb, topk, pool=None, cands=None, seen=None, queries=None, div=None, cat=None):
+        """(keys int32, scores float32) [len(indexes), topk]: query i, the row A[indexes[i]] or row i of the CUDA rows
+        `queries` in its place, ranked against the items B (bias Bb).  pool: None (or empty) ranks every item, else
+        the item indexes every query ranks; cands instead: (END offsets int64, keys int32) whose row i lists the items
+        query i ranks.  seen: None, or (END offsets int64, keys int32; host arrays, or CUDA tensors with `queries`)
+        whose row i holds the items query i must not get.  div = (w, M) of _check_diversify reranks each query's M best
+        by MMR against B; cat = (categories, caps) of _check_categories walks each query's complete ranking under the
+        caps (DESIGN.md 4.18).  On the device the candidates never leave it.  The NumPy path takes host seen rows
+        only."""
         if Bb is not None and not Bb.size:
             Bb = None
-        if self._on_device(indexes, A, B, topk):
-            h = self._serve_handle(B, None if Bb is None else np.ascontiguousarray(Bb, dtype=np.float32))
-            self._set_queries(h, A, indexes, queries)
-            h.set_pool(None if pool is None or len(pool) == 0 else pool)
-            if seen is not None:
-                return h.topk_seen(np.arange(len(indexes), dtype=np.int32), topk, *seen)
-            return h.topk(np.arange(len(indexes), dtype=np.int32), topk)
-        A, indexes = self._host_queries(A, indexes, queries, B.shape[1])
-        keys = np.zeros((len(indexes), topk), dtype=np.int32)
-        scores = np.zeros((len(indexes), topk), dtype=np.float32)
-        if seen is not None:
-            dot_topn(indexes, A, B, Bb, keys, scores, pool, topk, self.num_workers, *seen)
-        else:
-            dot_topn(indexes, A, B, Bb, keys, scores, pool, topk, self.num_workers)
-        return keys, scores
-
-    def _run_cands(self, indexes, A, B, Bb, topk, cands, seen=None, queries=None):
-        """_run with a candidate list per query instead of one pool: cands (END offsets int64, keys int32) whose row i
-        lists the items query indexes[i] ranks."""
-        if Bb is not None and not Bb.size:
-            Bb = None
-        if self._on_device(indexes, A, B, topk):
-            h = self._serve_handle(B, None if Bb is None else np.ascontiguousarray(Bb, dtype=np.float32))
-            self._set_queries(h, A, indexes, queries)
-            return h.topk_candidates(np.arange(len(indexes), dtype=np.int32), topk, *cands, seen=seen)
-        A, indexes = self._host_queries(A, indexes, queries, B.shape[1])
-        return cand_topn(indexes, A, B, Bb, topk, *cands, *(seen or ()))
-
-    def _run_diverse(self, indexes, A, B, Bb, topk, div, pool=None, seen=None, cands=None, queries=None):
-        """_run (or _run_cands with cands) at k = M, then the MMR re-ranking of those M candidates down to topk against
-        the item rows B; div = (w, M) of _check_diversify.  On the device the candidates never leave it."""
-        w, M = div
-        if Bb is not None and not Bb.size:
-            Bb = None
-        if self._on_device(indexes, A, B, M):
+        if pool is not None and len(pool) == 0:
+            pool = None
+        if self._on_device(indexes, A, B, div[1] if div is not None else _category_depth(topk) if cat is not None
+                           else topk, queries):
             import torch
             h = self._serve_handle(B, None if Bb is None else np.ascontiguousarray(Bb, dtype=np.float32))
-            self._set_queries(h, A, indexes, queries)
-            if cands is None:
-                h.set_pool(None if pool is None or len(pool) == 0 else pool)
-            dev = torch.device("cuda", torch.cuda.current_device())
-            return _rerank_batches(h, len(indexes), topk, w, M, dev, _device_stage(h, M, dev, seen, cands))
-        if cands is not None:
-            keys, scores = self._run_cands(indexes, A, B, Bb, M, cands, seen, queries)
-        else:
-            keys, scores = self._run(indexes, A, B, Bb, M, pool, seen, queries)
-        return mmr_numpy(keys, scores, B, topk, w)
-
-    def _run_capped(self, indexes, A, B, Bb, topk, cat, pool=None, seen=None, cands=None, queries=None):
-        """_run (or _run_cands with cands) with the per-category caps cat = (categories, caps) of _check_categories
-        applied over each query's complete ranking (DESIGN.md 4.18).  On the device the candidates never leave it;
-        without one the complete ranking is computed in NumPy and walked."""
-        if Bb is not None and not Bb.size:
-            Bb = None
-        if self._on_device(indexes, A, B, _category_depth(topk)):
-            import torch
-            h = self._serve_handle(B, None if Bb is None else np.ascontiguousarray(Bb, dtype=np.float32))
-            self._set_queries(h, A, indexes, queries)
-            if cands is None:
-                h.set_pool(None if pool is None or len(pool) == 0 else pool)
-            dev = torch.device("cuda", torch.cuda.current_device())
-            return _capped_batches(h, len(indexes), topk, *cat, dev, B.shape[0], seen, cands)
+            n = len(indexes)
+            dev = queries.device if queries is not None else torch.device("cuda", torch.cuda.current_device())
+            try:
+                self._set_queries(h, A, indexes, queries)
+                h.set_pool(pool)
+                if div is not None:
+                    return _rerank_batches(h, n, topk, div[0], div[1], dev, _device_stage(h, div[1], dev, seen, cands))
+                if cat is not None:
+                    return _capped_batches(h, n, topk, *cat, dev, B.shape[0], seen, cands)
+                if seen is not None and not isinstance(seen[0], np.ndarray):
+                    ci, cv = _device_stage(h, topk, dev, seen, cands)(torch.arange(n, dtype=torch.int32, device=dev))
+                    return ci.cpu().numpy(), cv.cpu().numpy()
+                # the host entries batch the queries and overlap each batch's copy back with the next batch
+                q = np.arange(n, dtype=np.int32)
+                if cands is not None:
+                    return h.topk_candidates(q, topk, *cands, seen=seen)
+                return h.topk(q, topk) if seen is None else h.topk_seen(q, topk, *seen)
+            finally:
+                if queries is not None:
+                    # the rows belong to the caller; every query on the handle sets its own queries first
+                    h.unbind_queries()
+        # NumPy: each query's ranked candidates (M of them to rerank, the complete ranking to walk), then the post-step
         A, indexes = self._host_queries(A, indexes, queries, B.shape[1])
-        if cands is not None:
+        depth = topk if div is None else div[1]
+        if cat is not None and cands is not None:
             ends = np.asarray(cands[0], dtype=np.int64)
             depth = max(1, int(np.diff(ends, prepend=0).max()) if len(ends) else 1)
+        elif cat is not None:
+            depth = B.shape[0] if pool is None else len(pool)
+        if cands is not None:
             keys, scores = cand_topn(indexes, A, B, Bb, depth, *cands, *(seen or ()))
         else:
-            depth = B.shape[0] if pool is None or len(pool) == 0 else len(pool)
             keys = np.zeros((len(indexes), depth), dtype=np.int32)
             scores = np.zeros((len(indexes), depth), dtype=np.float32)
             dot_topn(indexes, A, B, Bb, keys, scores, pool, depth, self.num_workers, *(seen or ()))
-        return category_walk_numpy(keys, scores, *cat, topk)
+        if div is not None:
+            return mmr_numpy(keys, scores, B, topk, div[0])
+        if cat is not None:
+            return category_walk_numpy(keys, scores, *cat, topk)
+        return keys, scores
 
 
 class ParALS(Parallel):
@@ -595,11 +578,10 @@ class ParALS(Parallel):
             raise ValueError(f"Not supported group: {group}")
         F = self.algo.Q if group == "item" else self.algo.P
         Fb = self._index_bias(group)
-        if isinstance(nlist, bool) or not isinstance(nlist, (int, np.integer)) or not 1 <= nlist <= min(
-                F.shape[0], backend.IVF_MAX_LISTS):
+        if not _is_int(nlist) or not 1 <= nlist <= min(F.shape[0], backend.IVF_MAX_LISTS):
             raise ValueError("nlist must be an integer in [1, min(rows, %d)] = [1, %d], got %r"
                              % (backend.IVF_MAX_LISTS, min(F.shape[0], backend.IVF_MAX_LISTS), nlist))
-        if isinstance(iters, bool) or not isinstance(iters, (int, np.integer)) or iters < 1:
+        if not _is_int(iters) or iters < 1:
             raise ValueError("iters must be an integer of at least 1, got %r" % (iters,))
         F = np.ascontiguousarray(F, dtype=np.float32)
         ivf = backend.IVF()
@@ -654,14 +636,11 @@ class ParALS(Parallel):
         names = self.algo._idmanager.itemids if group == "item" else self.algo._idmanager.userids
         if nprobe is not None:
             topks, scores = self._search_index(group, idx, F, topk, nprobe, False, True)
-        elif cat is not None:
-            _check_unique_pool(pool)
-            topks, scores = self._run_capped(idx, F, F, None, topk, cat, pool)
         else:
-            topks, scores = self._run(idx, F, F, None, topk, pool)
-        if repr:
-            topks = [[names[t] for t in tt if t != -1] for tt in topks]
-        return topks, scores
+            if cat is not None:
+                _check_unique_pool(pool)
+            topks, scores = self._rank(idx, F, F, None, topk, pool, cat=cat)
+        return _names(names, topks) if repr else topks, scores
 
     @staticmethod
     def _pool_matrix(pool, rows, num_items):
@@ -771,56 +750,26 @@ class ParALS(Parallel):
         Qb = self.algo.Qb if self._bias and self.algo.opt.get("use_bias") else None
         if exp is not None:
             self._training_data("explore")
+        cands = None
         if scipy.sparse.issparse(pool):
             kept, idx, _ = self._resolve(keys, None, "user")
             topk = backend.Serve._check_k(topk)
             from buffalo_b200.evaluate.device import _gather_rows
             cands = _gather_rows(*self._pool_matrix(pool, self.algo.P.shape[0], self.algo.Q.shape[0]), idx)
-            if cat is not None:
-                _check_unique_pool(cands=cands)
-            seen = self._seen_rows(idx, exclude_seen) if scipy.sparse.issparse(exclude_seen) or exclude_seen else None
-            q = None if exp is None else self._explore_rows(idx, exp)
-            try:
-                if cat is not None:
-                    topks, scores = self._run_capped(idx, self.algo.P, self.algo.Q, Qb, topk, cat, seen=seen,
-                                                     cands=cands, queries=q)
-                elif div is not None:
-                    topks, scores = self._run_diverse(idx, self.algo.P, self.algo.Q, Qb, topk, div, seen=seen,
-                                                      cands=cands, queries=q)
-                else:
-                    topks, scores = self._run_cands(idx, self.algo.P, self.algo.Q, Qb, topk, cands, seen, queries=q)
-            finally:
-                self._release_queries(q)
-            if repr:
-                topks = [[self.algo._idmanager.itemids[t] for t in tt if t != -1] for tt in topks]
-            return kept, topks, scores
-        kept, idx, pool = self._resolve(keys, pool, "user")
+            pool = None
+        else:
+            kept, idx, pool = self._resolve(keys, pool, "user")
         if cat is not None:
-            _check_unique_pool(pool)
+            _check_unique_pool(pool, cands)
         seen = self._seen_rows(idx, exclude_seen) if nprobe is None and (
             scipy.sparse.issparse(exclude_seen) or exclude_seen) else None
         q = None if exp is None else self._explore_rows(idx, exp)
-        try:
-            if nprobe is not None:
-                topks, scores = self._search_index("item", idx, self.algo.P, topk, nprobe,
-                                                   self._index_bias("item") is not None, False, queries=q)
-            elif cat is not None:
-                topks, scores = self._run_capped(idx, self.algo.P, self.algo.Q, Qb, topk, cat, pool, seen, queries=q)
-            elif div is not None:
-                topks, scores = self._run_diverse(idx, self.algo.P, self.algo.Q, Qb, topk, div, pool, seen, queries=q)
-            else:
-                topks, scores = self._run(idx, self.algo.P, self.algo.Q, Qb, topk, pool, seen, queries=q)
-        finally:
-            self._release_queries(q)
-        if repr:
-            topks = [[self.algo._idmanager.itemids[t] for t in tt if t != -1] for tt in topks]
-        return kept, topks, scores
-
-    def _release_queries(self, queries):
-        """Frees an explore call's device rows from the serve handle (every query sets its own queries first)."""
-        h = getattr(self, "_serve", None)
-        if queries is not None and h is not None:
-            h.unbind_queries()
+        if nprobe is not None:
+            topks, scores = self._search_index("item", idx, self.algo.P, topk, nprobe,
+                                               self._index_bias("item") is not None, False, queries=q)
+        else:
+            topks, scores = self._rank(idx, self.algo.P, self.algo.Q, Qb, topk, pool, cands, seen, q, div, cat)
+        return kept, _names(self.algo._idmanager.itemids, topks) if repr else topks, scores
 
     def fold_in_recommendation(self, histories, topk=10, pool=None, exclude_seen=True, repr=False, diversify=None,
                                diversify_candidates=None, explore=None, explore_seed=0, categories=None,
@@ -861,39 +810,18 @@ class ParALS(Parallel):
         n = tX.shape[0]
         if n == 0:
             return np.zeros((0, topk), np.int32), np.zeros((0, topk), np.float32)
-        import torch
         if exp is not None:
+            import torch
             from buffalo_b200.algo import fold_in
             from buffalo_b200.backend import CuALS
             st, fh = fold_in.resident_state(self.algo, CuALS)
             tX = self.algo._sample_rows(st, fh, (indptr, keys, vals), tX,
                                         torch.arange(n, dtype=torch.int64, device=tX.device), seed=exp[1], scale=exp[0])
-        h = self._serve_handle(np.ascontiguousarray(self.algo.Q, dtype=np.float32), None)
-        try:
-            h.bind_queries(tX)
-            h.set_pool(pool)
-            qidx = torch.arange(n, dtype=torch.int32, device=tX.device)
-            if cat is not None:
-                topks, scores = _capped_batches(h, n, topk, *cat, tX.device, self.algo.Q.shape[0],
-                                                (indptr, keys) if exclude_seen else None, cands)
-            elif div is not None:
-                topks, scores = _rerank_batches(h, n, topk, div[0], div[1], tX.device, _device_stage(
-                    h, div[1], tX.device, (indptr, keys) if exclude_seen else None, cands))
-            elif cands is not None:
-                cptr, ckeys = (torch.from_numpy(x).to(tX.device) for x in (cands[0], _nonempty(cands[1])))
-                idx, val = h.topk_candidates_device(qidx, topk, cptr, ckeys, seen=(indptr, keys) if exclude_seen else None)
-            elif exclude_seen:
-                idx, val = h.topk_seen_device(qidx, topk, indptr, keys)
-            else:
-                idx, val = h.topk_device(qidx, topk)
-            if div is None and cat is None:
-                topks, scores = idx.cpu().numpy(), val.cpu().numpy()
-        finally:
-            # the folded rows are freed with this call; every query on the handle sets its own queries first
-            h.unbind_queries()
-        if repr:
-            topks = [[self.algo._idmanager.itemids[t] for t in tt if t != -1] for tt in topks]
-        return topks, scores
+        # the folded rows and the history CSR stay on the device, so _rank takes its device path
+        Q = np.ascontiguousarray(self.algo.Q, dtype=np.float32)
+        topks, scores = self._rank(np.arange(n, dtype=np.int32), None, Q, None, topk, pool, cands,
+                                   (indptr, keys) if exclude_seen else None, tX, div, cat)
+        return _names(self.algo._idmanager.itemids, topks) if repr else topks, scores
 
     def explain(self, keys, items, topm=5, repr=False):
         """(scores, keys, contributions) of algo.explain (DESIGN.md 4.11) for trained users: their histories are their
@@ -919,8 +847,7 @@ class ParALS(Parallel):
                 raise ValueError("user index outside [0, %d)" % num_users)
         scores, out_keys, contrib = self.algo.explain(self._training_rows(idx, "explain"), items, topm)
         if repr:
-            names = self.algo._idmanager.itemids
-            out_keys = [[[names[t] for t in tt if t != -1] for tt in row] for row in out_keys]
+            out_keys = [_names(self.algo._idmanager.itemids, row) for row in out_keys]
         return scores, out_keys, contrib
 
 
@@ -931,6 +858,11 @@ class ParBPRMF(ParALS):
 def _nonempty(a):
     """a, or one zero when a is empty (a device array handed to the library holds at least one element)."""
     return a if a.size else np.zeros(1, a.dtype)
+
+
+def _names(names, topks):
+    """repr=True's rows: each row of indexes topks as names[index], the -1 padding dropped."""
+    return [[names[t] for t in tt if t != -1] for tt in topks]
 
 
 def _unsupported(name):
